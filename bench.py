@@ -2,16 +2,18 @@
 """bench.py -- clips/sec of the LFB hot path (BASELINE.json config 2: R50-I3D-NL + FBO-NL-2L,
 forward + backward + SGD, 2 synthetic 32x224x224 clips / 4 RoIs / 300-row bank per GPU).
 
-  python bench.py --gpus N --steps K --warmup W            # this implementation (tcgen05 path)
+  python bench.py --gpus N --steps K --warmup W            # this implementation (tensor-core wgmma path)
   python bench.py --impl reference --gpus N --steps K ...  # CPU reference arm (oracle restatement)
 
 One JSON line on stdout (rank 0).  `value` = device-resident throughput (inputs already in HBM, CUDA-graph replay),
 `e2e` = through EnqueueBlobs / RunNet / FetchBlob with pinned host buffers (H2D + loss D2H inside the timed region),
-`roofline` = the tcgen05 gathered-GEMM kernel (all launches of one step; by_stage / by_kind; DRAM traffic from the tracked
+`roofline` = the tensor-core gathered-GEMM kernel (all launches of one step; by_stage / by_kind; DRAM traffic from the tracked
 ncu launch list) against the measured tensor peak, `cpu_baseline` = the oracle timed on the host cores, `fbo_microbench` =
 bench_fbo.py cases (BASELINE configs[4]), `large_batch` = the same step at 8 clips per GPU (sub-process), `clocks` =
 nvidia-smi samples taken while the timed regions ran.  N > 1 (torchrun): max over ranks, weak scaling, the N=1-only extras
-are skipped.
+are skipped.  --dump-outputs DIR writes what the last timed step computed (loss, predictions, a fixed sample of the
+updated conv1 weights) as float32 .npy files; inputs and initial weights are seeded, so two builds compare output for
+output.
 """
 import argparse
 import json
@@ -76,8 +78,7 @@ def stage_of(label):
 
 class ClockSampler(threading.Thread):
     """Samples SM clocks / throttle reasons while the timed regions run: ONE long-lived `nvidia-smi -lms` process started
-    before them and read by this thread (no process is forked inside a timed region; scripts/diag_e2e.py measured the
-    end-to-end loop at 12.50 ms with this sampler running and 12.48 ms without, profiles/r02_diag_e2e_call_r.txt)."""
+    before them and read by this thread (no process is forked inside a timed region)."""
     Q = ('clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
          'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
 
@@ -122,14 +123,14 @@ def measured_peaks():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             return json.load(f), 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+        # H100 SXM data sheet (dense, 700 W card): not reached in practice, so fractions against it are lower bounds
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0}, 'data-sheet'
 
 
 # ------------------------------------------------------------------------------------ CPU reference arm
 def cpu_threads():
-    """Threads for the CPU arm.  Measured on the B200 host (profiles/r01_cpu_thread_sweep.txt, 128
-    logical cores): 8 -> 3.0 s/clip, 16 -> 2.65, 32 -> 2.95, 64 -> 4.7, 128 -> 95: oneDNN's 3-D
-    convolutions stop scaling at 16 threads, so that is what the baseline uses (all cores if fewer)."""
+    """Threads for the CPU arm: oneDNN's 3-D convolutions stop scaling at about 16 threads, so that is what the
+    baseline uses (all cores if fewer)."""
     return min(os.cpu_count() or 1, 16)
 
 
@@ -203,7 +204,22 @@ def workload_config(n_gpus):
             'clips_per_gpu': CLIPS_PER_GPU, 'parallelism': 'dp%d' % n_gpus}
 
 
-# ------------------------------------------------------------------------------------ B200 arm
+DUMP_SAMPLE = 65536          # elements of a larger output written by --dump-outputs (fixed, seeded positions)
+
+
+def dump_outputs(out_dir, workspace):
+    """What a caller of the timed training step receives after its last step: the loss, the predictions and the
+    updated weights (a fixed, seeded sample of conv1_w), as float32 .npy files (well under 64 MB in all)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name in ('loss', 'pred', 'conv1_w'):
+        a = np.asarray(workspace.FetchBlob('gpu_0/' + name), dtype=np.float32).reshape(-1)
+        if a.size > DUMP_SAMPLE:
+            a = a[np.sort(np.random.RandomState(0).choice(a.size, DUMP_SAMPLE, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
+# ------------------------------------------------------------------------------------ GPU arm
 def run_b200(args):
     import numpy as np
     import torch
@@ -272,6 +288,8 @@ def run_b200(args):
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1)) / args.steps
     launches = K.LAUNCHES // max(args.steps, 1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, workspace)
 
     # ---- end to end through the public API: every step's inputs travel host (pinned) -> device inside the timed
     # region and the loss is read back every step.  EnqueueBlobs is the stand-in for the reference's BlobsQueue
@@ -331,7 +349,7 @@ def run_b200(args):
         e2e_ms, e2e_mode = e2e_async_ms, 'FetchBlobAsync(loss): step i read back after step i+1 was launched'
     sampler.stop()
 
-    # ---- roofline of the dominant kernel: every tcgen05 GEMM launch of one more (eager) step is recorded and then
+    # ---- roofline of the dominant kernel: every tensor-core GEMM launch of one more (eager) step is recorded and then
     # replayed back to back between CUDA events (device time per launch; kernels.stop_profile)
     workspace.current().force_eager = True
     if not args.no_roofline:
@@ -349,7 +367,7 @@ def run_b200(args):
     if rank != 0:
         return
     peaks, peak_src = measured_peaks()
-    peak_tf32 = peaks['bf16_tflops_sustained'] / 2.0                  # kind::tf32 issues at half the bf16 rate
+    peak_tf32 = peaks['bf16_tflops_sustained'] / 2.0                  # tf32 MMAs issue at half the bf16 rate
     roof_ms = 0.0            # sum over launches of max(flops / tensor peak, algorithmic bytes / HBM peak)
     for kind, t, f, nb, lab in recs:
         t_roof = max(f / (peak_tf32 * 1e9), nb / (peaks['hbm_gbs'] * 1e6))        # ms
@@ -422,7 +440,7 @@ def run_b200(args):
                      'roofline_frac': sub['roofline']['frac'], 'roofline_achieved_tflops': sub['roofline']['achieved'],
                      'tensor_frac_by_stage': dict((k, v['tensor_frac']) for k, v in sub['roofline']['by_stage'].items()),
                      'gpu_launches': sub['gpu_launches'],
-                     'what': 'the same training step with %d clips (R=%d RoIs) per GPU: tiles fill the 148 SMs and the '
+                     'what': 'the same training step with %d clips (R=%d RoIs) per GPU: tiles fill the 132 SMs and the '
                              'per-launch fixed costs amortise; not the headline (the reference trains 2 clips / GPU)' % (
                                  args.large_batch, args.large_batch * ROIS_PER_CLIP)}
         except Exception as exc:
@@ -433,7 +451,7 @@ def run_b200(args):
         'unit': 'clips/s', 'n_gpus': n_gpus, 'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': ms,
         'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'tf32', 'data': 'synthetic',
         'config': dict(workload_config(n_gpus),
-                       l2='activations (>1 GB/step) exceed the 126 MB L2 between launches; no explicit flush',
+                       l2='activations (>1 GB/step) exceed the 50 MB L2 between launches; no explicit flush',
                        dropout='Philox, enabled', cuda_graph=bool(cfg.B200.CUDA_GRAPH), weights='random-init'),
         'e2e': {'value': clips / (e2e_ms / 1e3), 'unit': 'clips/s', 'h2d_bytes_per_step': h2d,
                 'd2h_bytes_per_step': 4, 'ms_per_step': e2e_ms, 'loss_readback': e2e_mode,
@@ -448,7 +466,7 @@ def run_b200(args):
                                'parameter block replayed 5x back to back between two CUDA events on the launching stream '
                                '(no host launch latency in the number): sum %.2f ms; the captured step takes %.2f ms in '
                                'total' % (len(recs), gemm_ms, ms),
-                     'peak_source': '%s bf16_tflops_sustained / 2 (kind::tf32)' % peak_src,
+                     'peak_source': '%s bf16_tflops_sustained / 2 (tf32)' % peak_src,
                      'per_launch_roofline': {
                          'what': 'sum over the GEMM launches of max(flops / tensor peak, algorithmic bytes / HBM peak) '
                                  '/ measured time: the fp32 activations make the res2/res3/stem layers HBM-bound',
@@ -472,13 +490,15 @@ def main():
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--dump-gemms', default='', help='write the per-launch GEMM table of one step here')
-    ap.add_argument('--no-graph', action='store_true', help='eager launches (for ncu / debugging)')
+    ap.add_argument('--no-graph', action='store_true', help='eager launches (for debugging)')
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='write the outputs of the last timed step to DIR/<name>.npy (float32)')
     ap.add_argument('--no-fbo', action='store_true', help='skip the FBO-NL microbenchmark cases (bench_fbo.py)')
-    ap.add_argument('--no-roofline', action='store_true', help='skip the per-launch replay profile (ncu launch lists)')
+    ap.add_argument('--no-roofline', action='store_true', help='skip the per-launch replay profile')
     ap.add_argument('--config', default='r50_2l', choices=sorted(CONFIGS), help='r50_2l = BASELINE configs[1] (default), '
                     'r50_3l = configs[2] (ava_r50_lfb_nl_3l.yaml), r101_3l = configs[3] architecture')
     ap.add_argument('--clips-per-gpu', type=int, default=CLIPS_PER_GPU, help='clips per GPU and step (default 2 = the '
-                    "reference's TRAIN.BATCH_SIZE 16 on 8 GPUs; larger batches fill the 148 SMs better)")
+                    "reference's TRAIN.BATCH_SIZE 16 on 8 GPUs; larger batches fill the 132 SMs better)")
     ap.add_argument('--large-batch', type=int, default=8, help='also time the step at this many clips per GPU in a '
                     'separate process (N=1 only; 0 = skip)')
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench_fbo.py -- BASELINE.json configs[4]: Feature-Bank-Operator (FBO-NL) microbenchmark on one B200.
+"""bench_fbo.py -- BASELINE.json configs[4]: Feature-Bank-Operator (FBO-NL) microbenchmark on one H100.
 
 Sweeps the bank length L and the RoI count R over the FBO-NL head alone (lfb_helper.add_fbo_nl_head: query
 reduction 2048->512, bank projection 'lfb_1x1', NUM_LAYERS single-query non-local layers), built through the same
@@ -16,7 +16,7 @@ One JSON line per (mode, R, L, layers) on stdout:
   (for infer_fold this is "effective" throughput: the folded path does not execute those FLOPs);
   scan = the fbo_bank_scan launches alone (CUDA events around each, eager pass): achieved GB/s of the dominant kernel.
 Inputs are resident in HBM; L2 is flushed (256 MB write) before every timed iteration, so a bank that would fit the
-126 MB L2 is still read from HBM once per iteration.
+50 MB L2 is still read from HBM once per iteration.
 """
 import argparse
 import json
@@ -190,7 +190,7 @@ def main():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             peaks = json.load(f)
     except Exception:
-        peaks = {'hbm_gbs': 6650.0, 'bf16_tflops_sustained': 1400.0}
+        peaks = {'hbm_gbs': 3350.0, 'bf16_tflops_sustained': 989.0}     # H100 SXM data sheet (dense, 700 W card)
     rows = []
     for layers in [int(v) for v in args.layers.split(',')]:
         for mode in args.modes.split(','):

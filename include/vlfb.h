@@ -1,5 +1,5 @@
 /*
- * vlfb.h -- C ABI of libvlfb.so: the B200 (sm_100a) hot path of
+ * vlfb.h -- C ABI of libvlfb.so: the H100 (sm_90a) hot path of
  * facebookresearch/video-long-term-feature-banks (R50/R101-I3D-NL backbone fwd/bwd +
  * Feature-Bank-Operator attention).
  *
@@ -106,8 +106,8 @@ typedef struct {
                                * epilogues. */
   size_t workspace_bytes;
   int engine;                 /* VLFB_ENGINE_TCGEN05 (0, default) or VLFB_ENGINE_SIMT (fp32 cross-check engine) */
-  int tile_n;                 /* 0 = chosen by the library, else the output-tile width (32..256, multiple of 32) */
-  int pair;                   /* 0 = auto, 1 = CTA pairs (cta_group::2, 256-row tiles) whenever legal, -1 = never */
+  int tile_n;                 /* 0 = chosen by the library, else the output-tile width (32, 64, 96 or 128; wider requests get 128) */
+  int pair;                   /* accepted and ignored: sm_90a has no CTA-pair MMA */
   int stream_k;               /* 0 = auto, 1 = stream-K whenever legal, -1 = never */
   /* ---- ReLU sign bits: one bit per element of d (bit e & 31 of word e >> 5, e = the element's offset from d) ---- */
   const uint32_t* relu_mask_bits; /* or NULL: v = bit ? v : 0, applied where relu_mask is (not both).  The mask of a ReLU's
@@ -122,10 +122,10 @@ enum { VLFB_ENGINE_TCGEN05 = 0, VLFB_ENGINE_SIMT = 1 };
 typedef struct {
   int tile_n;                 /* output-tile width */
   int split_k;                /* plain split-K factor (atomic epilogues) */
-  int pair;                   /* 1: 256 x tile_n tiles on CTA pairs (tcgen05 cta_group::2) */
-  int stream_k;               /* 1: equal (tile, K-chunk) ranges per SM (pair), shared tiles fixed up in the workspace */
+  int pair;                   /* always 0 (no CTA-pair MMA on sm_90a) */
+  int stream_k;               /* 1: equal (tile, K-chunk) ranges per SM, shared tiles fixed up in the workspace */
   int tiles;                  /* output tiles (x split_k) */
-  int units;                  /* CTAs (or CTA pairs) of the persistent grid */
+  int units;                  /* CTAs of the persistent grid */
 } vlfb_gemm_plan_t;
 
 /* Replaces: Caffe2 Conv (cuDNN) at resnet_video.py:169-179, model_builder_video.py:211-217,
@@ -134,7 +134,7 @@ typedef struct {
  * FC at resnet_video.py:327-331; and the AffineNd / Relu / Sum epilogues that follow
  * them (model_builder_video.py:218-219, resnet_helper.py:112-117). */
 int vlfb_gemm(const vlfb_gemm_params_t* p, void* stream);
-/* Host-only query: the tiling / schedule vlfb_gemm would use for `p` on a device with `num_sms` SMs (<= 0: 148),
+/* Host-only query: the tiling / schedule vlfb_gemm would use for `p` on a device with `num_sms` SMs (<= 0: 132),
  * assuming every operand is TMA-addressable.  No launch, no device access. */
 int vlfb_gemm_plan(const vlfb_gemm_params_t* p, int num_sms, vlfb_gemm_plan_t* plan);
 /* Bytes of vlfb_gemm_params_t.workspace that enable stream-K for every problem size (a constant of the build). */

@@ -41,7 +41,7 @@ class Graph(object):
     in 'run' mode it evaluates with torch ops."""
 
     def __init__(self, cfg, params=None, dropout_masks=None, emulate_tf32=False):
-        """emulate_tf32: round (to nearest, straight-through gradient) every tensor that the B200 path
+        """emulate_tf32: round (to nearest, straight-through gradient) every tensor that the tensor-core path
         stores as a TF32 tensor-core operand, at the same points of the graph (DESIGN.md section 3).  The
         resulting forward agrees with the GPU to fp32-accumulation error, so ReLU / max-pool decisions
         coincide and gradients can be compared tightly.  The default (False) is the plain fp32/fp64

@@ -1,5 +1,5 @@
 """Device-time table of the production GEMM shapes under the tiling / schedule variants of vlfb_gemm
-(tile_n, pair = tcgen05 cta_group::2, stream_k).  Each entry = mean of `reps` back-to-back launches (CUDA events
+(tile_n, stream_k).  Each entry = mean of `reps` back-to-back launches (CUDA events
 around the batch; operands stay L2-resident as they are inside a training step)."""
 import os
 import sys

@@ -5,7 +5,7 @@ set -e
 cd "$(dirname "$0")/../video-long-term-feature-banks_b200/csrc"
 mkdir -p /tmp/trace_build
 for f in api gemm_tc; do
-  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -I../../include -DVLFB_TRACE=1 -c $f.cu -o /tmp/trace_build/$f.o
+  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -I../../include -DVLFB_TRACE=1 -c $f.cu -o /tmp/trace_build/$f.o
 done
 nvcc -shared -o libvlfb_trace.so /tmp/trace_build/api.o /tmp/trace_build/gemm_tc.o gemm_simt.o ops.o fbo.o -lcudart
 python - <<'PY'

@@ -1,4 +1,4 @@
-"""GPU diagnostic: error table of the tcgen05 GEMM for every operand-major combination and
+"""GPU diagnostic: error table of the tensor-core GEMM for every operand-major combination and
 MN-major shared-memory layout mode (VLFB_MN_MODE).  Not a test; prints a table."""
 import os
 import sys

@@ -1,7 +1,7 @@
-// Probe of the TMA im2col mode (cuTensorMapEncodeIm2col + cp.async.bulk.tensor.5d...im2col) on sm_100a: which pixel
+// Probe of the TMA im2col mode (cuTensorMapEncodeIm2col + cp.async.bulk.tensor.5d...im2col) on sm_90a: which pixel
 // lands in which shared-memory row for given tensor coordinates / filter offsets / traversal strides.  The
 // tensor holds value n*1000 + d*100 + h*10 + w (+ c/100), so every row of the dump names its source pixel.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -o diag_im2col scripts/diag_im2col.cu -lcuda
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -o diag_im2col scripts/diag_im2col.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>

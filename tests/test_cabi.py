@@ -72,15 +72,15 @@ def test_wt_job_layout(tmp_path):
 
 
 def test_gemm_plan_query():
-    """Host-only: the tiling / schedule the tensor-core GEMM would use (vlfb_gemm_plan).  The res4/res5 layers of a
-    2-clip batch have M = 6272 = 49 row tiles of 128: with 128 x 256 tiles they fill 98 of 148 SMs (round 1).  CTA
-    pairs (cta_group::2, 256-row tiles) halve the operand bytes per SM and stream-K gives every pair the same number
-    of K chunks whatever the tile count."""
+    """Host-only: the tiling / schedule the tensor-core GEMM would use (vlfb_gemm_plan) on an H100 (132 SMs).  The
+    res4/res5 layers of a 2-clip batch have M = 6272 = 49 row tiles of 128: with 128 x 128 tiles (the widest a
+    warpgroup's registers hold) res5 branch2b is 196 tiles.  Stream-K gives every SM the same number of K chunks
+    whatever the tile count; CTA pairs do not exist on Hopper, so a pair request is ignored."""
     import ctypes as C
     from vlfb import libvlfb as L
     lib = L.load()
     ws_bytes = lib.vlfb_gemm_workspace_bytes()
-    assert ws_bytes >= 16384 * 4 + 148 * 2 * 128 * 256 * 4
+    assert ws_bytes >= 16384 * 4 + 132 * 2 * 128 * 128 * 4
 
     def plan(M, N, K, split=1, taps=1, flags=0, ws=True, **opts):
         p = L.GemmParams()
@@ -90,29 +90,31 @@ def test_gemm_plan_query():
         for k, v in opts.items():
             setattr(p, k, v)
         out = L.GemmPlan()
-        assert lib.vlfb_gemm_plan(C.byref(p), 148, C.byref(out)) == 0
+        assert lib.vlfb_gemm_plan(C.byref(p), 132, C.byref(out)) == 0
         return out
 
-    r5 = plan(6272, 512, 4608, pair=1, stream_k=1)               # res5 branch2b on pairs + stream-K (opt-in)
-    assert (r5.tile_n, r5.pair, r5.stream_k, r5.units, r5.tiles) == (256, 1, 1, 74, 50)
-    r4 = plan(6272, 256, 2304, pair=1, stream_k=1)               # res4 branch2b: 25 pair tiles over 74 pairs
-    assert (r4.tile_n, r4.pair, r4.stream_k, r4.units) == (256, 1, 1, 74)
+    r5 = plan(6272, 512, 4608, pair=1, stream_k=1)               # res5 branch2b + stream-K (opt-in); no pairs
+    assert (r5.tile_n, r5.pair, r5.stream_k, r5.units, r5.tiles) == (128, 0, 1, 132, 196)
+    r4 = plan(6272, 256, 2304, stream_k=1)                       # res4 branch2b: 98 tiles over 132 SMs
+    assert (r4.tile_n, r4.pair, r4.stream_k, r4.units) == (128, 0, 1, 132)
     nows = plan(6272, 512, 4608, ws=False, pair=1, stream_k=1)   # no workspace -> no fix-up schedule
-    assert nows.stream_k == 0 and nows.pair == 1
-    off = plan(6272, 512, 4608)                                  # default: the static tile loop on single CTAs
-    assert (off.tile_n, off.pair, off.stream_k, off.tiles, off.units) == (256, 0, 0, 98, 98)
+    assert nows.stream_k == 0 and nows.pair == 0
+    off = plan(6272, 512, 4608)                                  # default: the static tile loop
+    assert (off.tile_n, off.pair, off.stream_k, off.tiles, off.units) == (128, 0, 0, 196, 132)
     big = plan(200704, 256, 64)                                  # res2 1x1: thousands of tiles, static loop
-    assert big.stream_k == 0 and big.tile_n == 256
-    forced = plan(6272, 512, 4608, tile_n=192, pair=-1, stream_k=-1)
-    assert (forced.tile_n, forced.tiles) == (192, 147)
+    assert big.stream_k == 0 and big.tile_n == 128
+    forced = plan(6272, 512, 4608, tile_n=96, pair=-1, stream_k=-1)
+    assert (forced.tile_n, forced.tiles) == (96, 294)
+    wide = plan(6272, 512, 4608, tile_n=256, pair=-1, stream_k=-1)   # wider than a warpgroup holds: the widest tile
+    assert (wide.tile_n, wide.tiles) == (128, 196)
     for M, N, K in [(4, 80, 2560), (3136, 784, 256), (512, 4608, 6272), (64, 224, 802816), (1, 300, 512)]:
         o = plan(M, N, K, split=0, flags=L.EPI_ATOMIC)
-        assert o.tile_n % 32 == 0 and 32 <= o.tile_n <= 256 and o.split_k >= 1
+        assert o.tile_n % 32 == 0 and 32 <= o.tile_n <= 128 and o.split_k >= 1
         assert o.tile_n & (o.tile_n - 1) == 0
         assert o.tile_n == 32 or N > o.tile_n // 2               # never pad N by 2x or more
-        assert o.tiles == -(-M // (256 if o.pair else 128)) * -(-N // o.tile_n) * o.split_k
+        assert o.pair == 0 and o.tiles == -(-M // 128) * -(-N // o.tile_n) * o.split_k
         assert not (o.stream_k and o.split_k != 1)
-    assert lib.vlfb_gemm_plan(None, 148, None) == -1
+    assert lib.vlfb_gemm_plan(None, 132, None) == -1
 
 
 def test_fbo_bank_scan_split_table_properties():

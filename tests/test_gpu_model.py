@@ -1,7 +1,7 @@
 """GPU parity of the whole hot path through the builder API + workspace (C ABI underneath):
 R50-I3D-NL (+FBO) forward / backward / SGD step on cuda:0 versus the fp64 oracle.
 
-Tolerances.  The contractions run on tcgen05 kind::tf32 (10-bit mantissa operands, fp32
+Tolerances.  The contractions run on tensor-core tf32 MMAs (10-bit mantissa operands, fp32
 accumulate).
   * Forward outputs vs the PLAIN fp64 oracle: the north-star bound 1e-3 (max|a-b|/max|b|).
   * Gradients: a TF32-level perturbation (5e-4 relative) of an activation flips ReLUs / LayerNorm->ReLU
@@ -391,7 +391,7 @@ def test_full_size_config4_r101_fbo_nl_3l_tf32(ws):
 
 
 def test_full_size_config2_simt_fp32_engine(ws):
-    """The same full-size step on the SIMT fp32 engine (no tensor cores, same rounding points): separates tcgen05 /
+    """The same full-size step on the SIMT fp32 engine (no tensor cores, same rounding points): separates tensor-core /
     TMA kernel error from the ReLU-flip noise that TF32 rounding of the activations causes in both engines."""
     _train_case(ws, 'ava_r50_lfb_nl.yaml', FULL, 224, 32, 2, backend='simt', check_all_grads=True)
 

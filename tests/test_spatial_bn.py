@@ -4,7 +4,7 @@ CPU part: oracle/ops.spatial_bn pinned against torch.nn.functional.batch_norm (a
 published operator), the engine's lowering of a `MODEL.USE_AFFINE False` / `NONLOCAL.USE_BN True` net against the
 oracle in fp64 (forward blobs, batch / running statistics, every gradient, test-mode forward), and the precise-BN
 helper against a direct numpy computation of the population statistics.
-GPU part (-m gpu): csrc/bn.cu against the oracle op on the production shapes; a tiny training step on the tcgen05 path.
+GPU part (-m gpu): csrc/bn.cu against the oracle op on the production shapes; a tiny training step on the tensor-core path.
 """
 import numpy as np
 import pytest
@@ -205,7 +205,7 @@ def test_spatial_bn_kernels_match_oracle_op(rows, C):
 
 @pytest.mark.gpu
 def test_tiny_bn_train_step_on_gpu():
-    """MODEL.USE_AFFINE False: conv (tcgen05) -> SpatialBN -> ReLU ...; forward blobs, batch statistics and gradients
+    """MODEL.USE_AFFINE False: conv (tensor cores) -> SpatialBN -> ReLU ...; forward blobs, batch statistics and gradients
     against the fp64 oracle with the tolerances of the Affine path's tiny-model test."""
     from oracle import model as OM
     from vlfb import kernels, workspace

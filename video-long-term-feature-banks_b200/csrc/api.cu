@@ -99,7 +99,7 @@ int vlfb_version(void) { return 100; }
 const char* vlfb_last_error(void) { return g_err; }
 int vlfb_gemm_plan(const vlfb_gemm_params_t* p, int num_sms, vlfb_gemm_plan_t* plan) {
   VLFB_CHECK_ARG(p && plan && p->M > 0 && p->N > 0 && p->K > 0);
-  gemm_tc_plan(*p, num_sms > 0 ? num_sms : 148, plan);
+  gemm_tc_plan(*p, num_sms > 0 ? num_sms : 132, plan);
   return VLFB_OK;
 }
 

@@ -144,7 +144,7 @@ inline Ws carve(void* workspace, int C) {
 }
 inline void reduce_dims(int64_t rows, int C, dim3* grid, int64_t* rpb) {
   const int cb = ceil_div(C, 32);
-  int slabs = (4 * 148 + cb - 1) / cb;                      // ~4 blocks of 256 threads per SM
+  int slabs = (4 * 132 + cb - 1) / cb;                      // ~4 blocks of 256 threads per SM
   const int64_t max_slabs = (rows + 127) / 128;
   if (slabs > max_slabs) slabs = (int)max_slabs;
   if (slabs < 1) slabs = 1;

@@ -1,4 +1,4 @@
-// Shared helpers of libvlfb (sm_100a only).
+// Shared helpers of libvlfb (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -40,10 +40,10 @@ static inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 blo
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// Grid for streaming kernels: a multiple of the SM count (148 on B200), capped by the work.
+// Grid for streaming kernels: a multiple of the SM count (132 on H100 SXM), capped by the work.
 static inline int stream_grid(int64_t work_items, int threads, int per_thread = 1) {
   int64_t blocks = (work_items + (int64_t)threads * per_thread - 1) / ((int64_t)threads * per_thread);
-  const int64_t cap = 148 * 16;
+  const int64_t cap = 132 * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (int)blocks;

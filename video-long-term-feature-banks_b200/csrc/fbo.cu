@@ -1,4 +1,4 @@
-// Feature-bank kernels that work on the RAW long-term bank (HBM-bound scans / gathers), sm_100a.
+// Feature-bank kernels that work on the RAW long-term bank (HBM-bound scans / gathers), sm_90a.
 //
 // 1. fbo_bank_scan / fbo_bank_combine: the inference-mode Feature-Bank Operator.  Without dropout between
 //    'lfb_1x1' and the phi/g projections (lfb_helper.py:320-338 with test_mode), one FBO-NL layer with a single
@@ -21,10 +21,9 @@ namespace vlfb {
 namespace {
 
 constexpr int SCAN_TPB = 256;
-// bf16 bank rows (2048 elements = 4 KB): rows per tile / resident CTAs per SM of the scan.  Measured at R=256, L=3600
-// (calls J / K / M, profiles/r02_fbo_bf16_scan_variants.txt): 12 rows at 2 CTAs per SM 3.7 TB/s, 8 rows at 3 CTAs
-// 4.8, 6 rows at 3 CTAs 4.7, 4 rows at 4 CTAs (64 registers, no spills) 5.0 TB/s -- occupancy beats tile depth because the
-// unpacked rows cost registers.
+// bf16 bank rows (2048 elements = 4 KB): rows per tile / resident CTAs per SM of the scan.  4 rows at 4 CTAs per SM
+// (64 registers, no spills): the unpacked rows cost registers, so occupancy is favoured over tile depth.  A build
+// parameter; not re-tuned on the H100.
 #ifndef VLFB_SCAN16_ROWS
 #define VLFB_SCAN16_ROWS 4
 #endif
@@ -251,7 +250,7 @@ __global__ void lfb_gather_k(const float4* __restrict__ bank, const int32_t* __r
 //        sum_j p_j (W_g B'_j + b_g) = W_g (sum_j p_j B'_j) + b_g                        (sum_j p_j = 1)
 //    i.e. phi and g (2 x R*L x dB x d MACs per layer forward, 4 more GEMMs backward) are never formed: a layer is four
 //    d x d mat-vecs and two passes over B' per RoI.  The as-written graph spends 41 GEMM launches + ~70 streaming
-//    launches of 10-25 us each on R*L = 1200 rows (r01: 0.97 ms of a 15.8 ms step); here one CTA per RoI walks all
+//    launches on R*L = 1200 rows; here one CTA per RoI walks all
 //    layers.  Gradients: exact (the b_phi / theta terms that multiply sum_j dscore_j = 0 are kept for parity with the
 //    reference's autograd); the rank-R weight gradients are accumulated by fbo_nl_outer_k from the per-RoI vectors.
 constexpr int NL_TPB = 512;
@@ -297,9 +296,8 @@ __device__ __forceinline__ float block_max_nl(float v, float* red) {
   return red[0];
 }
 // One CTA streams ~5 MB of weights / bank rows per layer from L2: the loads must be deep enough in flight to hide the
-// ~1 us latency (Little's law).  r2 call C: with 4 scalar loads per thread in flight (8 KB per CTA) the stack ran at
-// ~10 GB/s per CTA and was slower than the 40 launches it replaces -- hence 4 rows per warp (matvec_rows: 16 x 16-byte
-// loads per lane) and 8 rows x 16 bytes per thread (colsum_w) below.
+// L2 latency (Little's law): 4 scalar loads per thread in flight would leave a CTA latency-bound -- hence 4 rows per
+// warp (matvec_rows: 16 x 16-byte loads per lane) and 8 rows x 16 bytes per thread (colsum_w) below.
 // out[row] = bias[row] + sum_c W[row][c] x[c]   (one warp per 4 rows, 128-bit lanes; cols % 4 == 0)
 __device__ __forceinline__ void matvec_rows(const float* __restrict__ W, const float* x, float* out,
                                             const float* __restrict__ bias, int rows, int cols) {
@@ -652,12 +650,12 @@ static int scan_rows(int D, int dt) {
 }
 
 /* Split of the L bank rows of every RoI over `S` CTAs: minimise waves x (tiles per CTA + partial-result cost) with
- * 2 resident CTAs per SM (296 per wave on B200). */
+ * 2 resident CTAs per SM (264 per wave on H100). */
 int vlfb_fbo_bank_scan_splits_dt(int R, int L, int D, int bank_dtype) {
   const int rows = scan_rows(D, bank_dtype);
   if (R <= 0 || L <= 0 || rows == 0) return 0;
   const int max_s = (L + rows - 1) / rows;
-  const int wave = 296;
+  const int wave = 264;
   int best = 1;
   double best_cost = 1e30;
   for (int s = 1; s <= max_s && s <= 1024; ++s) {

@@ -1,6 +1,6 @@
 // SIMT fp32 gathered GEMM -- bring-up / on-GPU cross-check engine only (vlfb_set_gemm_backend(1)).
 // It evaluates the operand semantics of common.cuh element by element, so it is the
-// executable definition the tcgen05 loaders in gemm_tc.cu are tested against.
+// executable definition the tensor-core loaders in gemm_tc.cu are tested against.
 #include "common.cuh"
 
 namespace vlfb {

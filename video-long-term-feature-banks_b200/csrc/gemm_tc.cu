@@ -1,22 +1,21 @@
-// tcgen05 (5th-gen tensor core) gathered GEMM for sm_100a.
+// Hopper (sm_90a) warpgroup-MMA gathered GEMM.
 //
-//   D[m,n] = epi( sum_k A[m,k] * B[n,k] ),  fp32 storage, kind::tf32 MMA, fp32 accumulate in TMEM.
+//   D[m,n] = epi( sum_k A[m,k] * B[n,k] ),  fp32 storage, wgmma tf32 MMA, fp32 accumulate in registers.
 //
 // Persistent kernel: grid = min(#tiles, #SMs), one CTA per SM walks a static sequence of 128 x BN output
-// tiles (UMMA M=128, N=BN, cta_group::1), 544 threads:
-//   warps 0-7  PRODUCERS -- the A/B K-chunks (32 fp32 = one 128-byte swizzle row) go straight from NDHWC
-//              tensors into the UMMA canonical swizzled shared-memory layouts, never through an im2col
-//              buffer: dense operands by TMA tiled boxes (SWIZZLE_128B K-major, SWIZZLE_128B_ATOM_32B
-//              MN-major), convolution gathers by TMA im2col copies (conv fwd, unit-stride dgrad, wgrad;
-//              one thread issues), and what TMA cannot express (conv1 stem with 16-byte pixels, strided
-//              dgrad, unaligned operands) by 16-byte cp.async with zero-fill = padding (all 8 warps);
-//   warp 8     TMEM allocator + single-thread tcgen05.mma issuer; tcgen05.commit releases each smem
-//              stage back to the producers and hands finished accumulators to the epilogue;
-//   warps 9-16 EPILOGUE -- tcgen05.ld TMEM -> registers -> smem transpose -> fused affine / residual /
-//              ReLU / TF32 rounding -> coalesced 128-bit global stores (or atomics for split-K).
-// The smem ring (full[s]/empty[s] mbarriers) runs continuously across tiles and the accumulator is double
-// buffered in TMEM (tmem_full[a]/tmem_empty[a]), so the epilogue of one tile overlaps the loads and MMAs
-// of the next.
+// tiles (BN <= 128):
+//   PRODUCERS  -- the A/B K-chunks (32 fp32 = one 128-byte swizzle row) go straight from NDHWC tensors into
+//              swizzled shared-memory tiles, never through an im2col buffer: dense operands by TMA tiled
+//              boxes (SWIZZLE_128B K-major, SWIZZLE_128B_ATOM_32B MN-major), convolution gathers by TMA
+//              im2col copies (conv fwd, unit-stride dgrad, wgrad; one thread issues), and what TMA cannot
+//              express (conv1 stem with 16-byte pixels, strided dgrad, unaligned operands) by 16-byte
+//              cp.async with zero-fill = padding (8 warps; a TMA-only build has one issuing warp of four);
+//   CONSUMERS  -- two warpgroups; warpgroup w issues wgmma.m64nBNk8 for tile rows [64 w, 64 w + 64) and then
+//              runs the epilogue of those rows from its registers: smem transpose -> fused affine /
+//              residual / ReLU / TF32 rounding -> coalesced 128-bit global stores (or atomics for split-K).
+// wgmma reads tf32 operands K-major only, so an MN-major stage tile (wgrad, transposed matmul operands) is
+// first rewritten by the consumers into a K-major image in shared memory.  The smem ring (full[s]/empty[s]
+// mbarriers) runs continuously across tiles, so the producers load the next tile during the epilogue.
 //
 // Operand kinds are described in include/vlfb.h; their element-level definition is
 // operand_elem() in common.cuh, which the SIMT engine evaluates literally and the tests
@@ -35,30 +34,27 @@
 namespace vlfb {
 namespace tc {
 
-constexpr int BM = 128;        // tile rows (UMMA M)
+constexpr int BM = 128;        // tile rows (two wgmma M = 64 warpgroups)
+constexpr int BN_MAX = 128;    // widest tile: a warpgroup holds 64 x BN fp32 accumulators = BN / 2 registers per thread
 constexpr int KC = 32;         // fp32 per K chunk (128 B)
-constexpr int NPROD = 256;     // 8 producer warps = 2 per scheduler, so the address-generation latency of one warp
-                               // hides behind the other (ncu r01: with one producer warp per scheduler 'wait' +
-                               // 'selected' stalls dominated).  Measured alternatives (profiles/r01_perf_log.md):
-                               // 7 producer warps (16 warps total -> 128 instead of 96 registers, no spills) lose
-                               // 3-5% of the step on the gather-bound convs; 4 epilogue warps lose ~4%.
-constexpr int NPW = NPROD / 32;
-// TMA-only builds: warps whose lane 0 issues the TMA boxes of a K chunk (box b by warp b % NTMAW).  The wgrad chunk is 4
-// (dY^T atoms) + 8 (im2col atoms of 32 columns) small boxes and its K loop runs at 33-37 % of the tensor pipe (ncu call M),
-// so round 2 tried 2 and 3 issuing warps: parity-green and MUCH slower (call Q: step 16.6 ms instead of 12.7, wgrad 5.7 ms
-// instead of 3.1, every other kind slower too) -- the boxes are not limited by the issuing thread but by the TMA unit's
-// per-box cost, and concurrent issuers only interleave the boxes of different stages.  Kept as a build parameter with the
-// measured default of ONE issuer; the remedy is fewer, larger boxes (one 4-D box per MN-major operand tile, below).
+constexpr int NPROD = 256;     // 8 cp.async producer warps = 2 per scheduler, so the address-generation latency of
+                               // one warp hides behind the other
+// TMA-only builds: warps whose lane 0 issues the TMA boxes of a K chunk (box b by warp b % NTMAW).  A build parameter,
+// default one issuer: concurrent issuers only interleave the boxes of different stages; fewer, larger boxes (one 4-D
+// box per MN-major operand tile, below) are the way to cut the per-box cost of the TMA unit.
 #ifndef VLFB_TMA_WARPS
 #define VLFB_TMA_WARPS 1
 #endif
 constexpr int NTMAW = VLFB_TMA_WARPS;
 constexpr int RSTEP = NPROD / 8;   // rows covered by one pass of the K-major loaders
-constexpr int NEPI = 256;          // 8 epilogue warps (two per TMEM lane quarter, splitting the column blocks)
-constexpr int EPC = 16;            // accumulator columns per epilogue step (tcgen05.ld.32x32b.x16)
-constexpr int EPITCH = EPC + 4;    // padded staging row (floats)
-constexpr int EPI_COLV = 2 * 128;     // per-warp column scale + bias of its 128 columns (floats)
-constexpr int EPI_WARP_FLOATS = 32 * EPITCH + EPI_COLV;
+static_assert(NTMAW >= 1 && NTMAW <= 4, "TMA issuers live in the producer warpgroup");
+constexpr int NEPI = 256;          // 2 consumer warpgroups (MMA + epilogue); warp w of a warpgroup owns 16 tile rows
+constexpr int NPROD_TMA = 128;     // producer threads of a TMA-only build: one warpgroup, so the consumers are warpgroup-aligned
+constexpr int EPC = 16;            // accumulator columns per epilogue step
+constexpr int EROWS = 2;           // tile rows per lane in the epilogue: (lane >> 2) + 8 i of the warp's 16
+constexpr int EPITCH = BN_MAX + 4; // padded accumulator staging row (floats): a consumer warp's 16 rows x the tile
+constexpr int EPI_COLV = 2 * BN_MAX;  // per-warp column scale + bias of the tile's columns (floats)
+constexpr int EPI_WARP_FLOATS = 16 * EPITCH + EPI_COLV;
 constexpr int EPI_STAGE_BYTES = (NEPI / 32) * EPI_WARP_FLOATS * 4;
 constexpr int A_TILE_BYTES = BM * KC * 4;  // 16 KB
 constexpr int MAX_STAGES = 8;
@@ -85,7 +81,8 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
   return ok;
 }
 // Bounded wait: a protocol bug traps (kernel error) instead of hanging the GPU.  The clock is only read
-// every 4096 polls so that the spin loop stays 3 instructions long (try_wait suspends in hardware).
+// every 4096 polls so that the spin loop stays 3 instructions long (try_wait suspends in hardware).  No printf:
+// a call inside the consumers' K loop would make ptxas serialize the wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = 0;
@@ -95,7 +92,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       const long long now = clock64();
       if (t0 == 0) t0 = now;
       else if (now - t0 > 8000000000LL) {
-        printf("vlfb gemm_tc: mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
         __trap();
       }
     }
@@ -150,79 +146,52 @@ __device__ __forceinline__ void cp_async_wait_dyn(int n) {
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// the 256 consumer threads (named barrier 1; barrier 0 is __syncthreads)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NEPI) : "memory"); }
+// wgmma m64nNk8, tf32 x tf32 -> f32, both operands K-major SWIZZLE_128B in shared memory; d[0, N/2) accumulates
+// (scale-d = 0 on the first MMA of a tile overwrites it).
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 32) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate));
+  } else if constexpr (N == 64) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
+  } else if constexpr (N == 96) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(da), "l"(db), "r"(accumulate));
+  } else if constexpr (N == 128) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
+  }
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// ---- cta_group::2 (CTA pair) variants.  Protocol (DESIGN.md 4.1): both CTAs of a (2,1,1) cluster allocate TMEM and
-// stage their half of the operands; the barriers that order the pipeline live at the SAME shared-memory offsets in
-// both CTAs; the leader (cluster rank 0) issues the MMAs and publishes their completion to both CTAs with a
-// multicast commit; the peer's TMA loads and epilogue warps signal the LEADER's barriers (mapa address).
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_2(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior MMAs of the pair -> one arrival on the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit2(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-// TMA loads issued by either CTA of the pair; the transaction bytes land on `bar`, which may be the peer's barrier
-__device__ __forceinline__ void tma_load_3d_2(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
-      : "memory");
+// wgmma shared-memory matrix descriptor: K-major SWIZZLE_128B, 8-row groups 1024 B apart (SBO), LBO unused (1).
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                 // [0,14)  start address
+  d |= (uint64_t)1 << 16;                                  // [16,30) leading byte offset (unused by 128B swizzle)
+  d |= (uint64_t)(1024 >> 4) << 32;                        // [32,46) stride byte offset
+  d |= (uint64_t)1 << 62;                                  // [62,64) 1 = SWIZZLE_128B
+  return d;
 }
 __device__ __forceinline__ void red_add_f4(float* p, const float4& v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
@@ -231,19 +200,6 @@ __device__ __forceinline__ float4 ld_cg_f4(const float* p) {
   float4 v;
   asm volatile("ld.global.cg.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
 }
 // residual / accumulate reads: plain (coherent) 128-bit loads -- D may have been written by an earlier launch
 // on the same stream, never by this one
@@ -256,40 +212,29 @@ __device__ __forceinline__ uint32_t ld_nc_u16(const unsigned short* p) {
 __device__ __forceinline__ void prefetch_l2(const void* p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout), SWIZZLE_128B.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                 uint32_t layout_type = 2) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                 // [0,14)  start address
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;        // [16,30) leading byte offset
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;        // [32,46) stride byte offset
-  d |= (uint64_t)1 << 46;                                  // [46,48) descriptor version 1 (sm_100)
-  d |= (uint64_t)layout_type << 61;                        // [61,64) 2 = SWIZZLE_128B, 1 = SWIZZLE_128B_BASE32B
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): tf32 x tf32 -> f32, M=128, N=bn.
-__host__ __device__ inline uint32_t make_idesc(int bn, int a_mn_major, int b_mn_major, int m = BM) {
-  uint32_t d = 0;
-  d |= 1u << 4;                          // c_format  = F32
-  d |= 2u << 7;                          // a_format  = TF32
-  d |= 2u << 10;                         // b_format  = TF32
-  d |= (uint32_t)(a_mn_major & 1) << 15; // a_major
-  d |= (uint32_t)(b_mn_major & 1) << 16; // b_major
-  d |= (uint32_t)(bn >> 3) << 17;        // n_dim
-  d |= (uint32_t)(m >> 4) << 24;         // m_dim (128, or 256 = a CTA pair with cta_group::2)
-  return d;
+// Consumer-side rewrite of an MN-major stage tile into the K-major SWIZZLE_128B image [row][128 B] that wgmma reads
+// (tf32 operands must be K-major).  Source: `rows` x 32 k as [atom of 32 elements][k-row][128 B], 32-byte units XOR
+// (k & 3) (SWIZZLE_128B_ATOM_32B / MNLoader), atoms `atom_stride` bytes apart; k-rows 128 B apart, or, for the conv1
+// wgrad patch tile (row_gap = sH), k-rows 16-31 (the patch's second output row) row_gap 2 KB slabs further.
+// Thread t moves float4 f = t + NEPI j: 16-byte chunk f % 8 of k-row (f / 8) % 32 of atom f / 256 (conflict-free reads).
+__device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int rows, int atom_stride, int row_gap, int ctid) {
+  for (int f = ctid; f < rows * 8; f += NEPI) {
+    const int c = f & 7, k = (f >> 3) & 31, atom = f >> 8;
+    const uint32_t koff = row_gap ? (uint32_t)((k >> 4) * row_gap * 2048 + (k & 15) * 128) : (uint32_t)(k * 128);
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                 : "r"(src + (uint32_t)(atom * atom_stride) + koff + (uint32_t)((c * 16) ^ ((k & 3) << 5)))
+                 : "memory");
+    const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int n = atom * 32 + 4 * c + q;
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (uint32_t)(n * 128 + ((((k >> 2) ^ (n & 7)) << 4) | ((k & 3) << 2)))),
+                   "f"(e[q]) : "memory");
+    }
+  }
 }
 
 __host__ __device__ constexpr bool is_mn(int kind) { return kind == VLFB_OP_DENSE_MN || kind == VLFB_OP_CONV_MN || kind == VLFB_OP_STEM_MN; }
@@ -324,7 +269,7 @@ __device__ __forceinline__ Pos4 decode_pos_fast(uint32_t idx, const PosDiv& pd) 
   return p;
 }
 
-// TMA im2col mode (measured semantics: profiles/r01_im2col_probe.txt): the 5-D map of an NDHWC tensor walks
+// TMA im2col mode: the 5-D map of an NDHWC tensor walks
 // `pixelsPerColumn` window origins in W -> H -> D -> N order inside the bounding box [lower, dim-1+upper] with the
 // convolution strides as traversal strides; {w,h,d} = origin of the first window (= out*stride - pad), the u16
 // offsets select the filter tap (tap*dilation); out-of-range pixels (padding, tensor tail) read as zeros.
@@ -332,16 +277,6 @@ __device__ __forceinline__ void tma_load_im2col(uint32_t dst, const CUtensorMap*
                                                 int ow, int oh, int od, uint32_t bar) {
   asm volatile(
       "cp.async.bulk.tensor.5d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%2, %3, %4, %5, %6}], [%7], {%8, %9, %10};"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "r"(bar),
-        "h"((uint16_t)ow), "h"((uint16_t)oh), "h"((uint16_t)od)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_im2col_2(uint32_t dst, const CUtensorMap* tm, int c, int w, int h, int d, int n,
-                                                  int ow, int oh, int od, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
       "[%0], [%1, {%2, %3, %4, %5, %6}], [%7], {%8, %9, %10};"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "r"(bar),
         "h"((uint16_t)ow), "h"((uint16_t)oh), "h"((uint16_t)od)
@@ -363,8 +298,7 @@ struct KLoader {
   uint32_t rowmask;  // DENSE_K: bit j set when row j is inside the matrix
   // Filter-tap cursor.  Chunks are issued in order, so the tap advances incrementally (no division per
   // chunk) and the gathered element offset / validity of every owned row is recomputed only when the
-  // tap changes (ncu r01: the per-chunk divisions and 64-bit address math made the producers
-  // instruction-bound at ~330 instructions per chunk per warp).
+  // tap changes (per-chunk divisions and 64-bit address math would make the producers instruction-bound).
   int cpt, tc, kt, kh, kw;
   int off[MAXR];
   uint32_t okmask;
@@ -484,18 +418,18 @@ struct KLoader {
 
 // ---------------------------------------------------------------- MN-major loaders
 // Tile = 32 k-rows, each `rows`*4 bytes of the m (or n) extent, stored as
-// [atom of 32 elements][32 k-rows][128 B] (UMMA canonical MN-major SWIZZLE_128B_BASE32B: LBO = 4096 between
-// atoms, SBO = 512 between groups of 4 k-rows).
+// [atom of 32 elements][32 k-rows][128 B] (MN-major SWIZZLE_128B_ATOM_32B; the
+// consumers rewrite it K-major before the MMAs, mn_to_kmajor).
 template <int KIND>
 struct MNLoader {
-  static constexpr int MAXS = (32 * 64) / NPROD;   // copies per thread per chunk at the widest tile (256 cols)
+  static constexpr int MAXS = (32 * (BN_MAX / 4)) / NPROD;   // copies per thread per chunk at the widest tile
   const float* base;
   int64_t ld;
   int tapz, nslot;
   // A thread copies the SAME 16-byte column chunk c of the k-rows kk0, kk0 + kstep, ... (NPROD is a multiple of
   // the chunks per k-row), so everything that depends on the column -- bounds, filter tap (kh,kw), channel,
   // swizzled shared-memory offset -- is one scalar per tile, and the per-chunk work per copy is two shuffles,
-  // a bit test and an add (ncu r01: the previous per-slot arrays cost ~100 instructions per 16-byte copy).
+  // a bit test and an add.
   int mn, kk0, kstep;
   bool colok;
   uint32_t dst0, dstep;
@@ -518,8 +452,7 @@ struct MNLoader {
     mn = row0 + c * 4;
     colok = mn < limit;
     // atom-major tile [atom of 32 elements][32 k-rows][128 B] in the SWIZZLE_128B_BASE32B pattern (32-byte
-    // units XOR (k & 3)); plain SWIZZLE_128B returns zeros for tf32 MN-major operands (measured,
-    // profiles/r01_gemm_layout_diag.txt).  Same image as a TMA box with SWIZZLE_128B_ATOM_32B.
+    // units XOR (k & 3)).  Same image as a TMA box with SWIZZLE_128B_ATOM_32B.
     // kstep is a multiple of 4 whenever a thread owns more than one copy, so the XOR term is per-thread.
     const int r = kk0 & 3, cc8 = c & 7;
     dst0 = (uint32_t)((c >> 3) * 4096 + kk0 * 128 + ((((cc8 >> 1) ^ r) << 5) | ((cc8 & 1) << 4)));
@@ -599,8 +532,8 @@ unsigned long long* g_trace_buf = nullptr;
 #else
 #define TR(slot) do { } while (0)
 #endif
-constexpr int MAX_UNITS = 160;       // >= #SMs: CTAs (or CTA pairs) of the persistent grid
-constexpr int SK_CNT_INTS = 16384;   // arrival counters at the head of the stream-K workspace (tile x rank x epilogue warp)
+constexpr int MAX_UNITS = 160;       // >= #SMs: CTAs of the persistent grid
+constexpr int SK_CNT_INTS = 16384;   // arrival counters at the head of the stream-K workspace (tile x consumer warp)
 
 // the lean epilogue addresses D / residual / sign bits with 32-bit element offsets
 __host__ __device__ inline bool span32_ok(const vlfb_gemm_params_t& p) {
@@ -611,7 +544,7 @@ __host__ __device__ inline bool span32_ok(const vlfb_gemm_params_t& p) {
 struct ParCls { short nh, nw, rh, rw, ph, pw; int nk; };   // taps per dim, first tap, parity, K chunks of the class
 
 struct Launch {
-  int bn;        // tile N (32/64/128/256) = UMMA N = TMEM columns
+  int bn;        // tile N (32/64/96/128) = wgmma N
   int stages;
   PosDiv out;    // fast divisors of the conv OUTPUT extents (Wo, Ho, To)
   PosDiv in;     // ... and of the INPUT extents (W, H, T) for the dgrad row decode
@@ -622,15 +555,14 @@ struct Launch {
                      //     view of a W-padded clip (make_tmap_stem)
   int lag;           // cp.async groups kept in flight before a stage is published (< stages)
   int tiles_m, tiles_n, total_tiles;
-  int tile_rows;     // output rows per tile: 128, or 256 when a CTA pair shares the tile (cta_group::2)
   int stem_patch;    // conv1 forward: an M tile = a 16 (wo) x 8 (ho) patch of one output frame instead of 128 consecutive
                      // positions, so that ONE strided TMA box stages the whole A tile of a K chunk (tile row r =
                      // (ho0 + r / 16, wo0 + r % 16)); the fast epilogue maps rows back (patch_row)
   int patch_wb, patch_hb;   // patches per output row / per frame column: Wo / 16, Ho / 8 (forward), Ho / 2 (wgrad)
                             // conv1 WGRAD (B = STEM_MN) with stem_patch: K chunk = the 32 output positions of a
                             // 16 (wo) x 2 (ho) patch; ONE box stages the sH + kH input rows all kH filter-row atoms need
-                            // ([input row][16 windows][128 B] slabs; atom kh of output row j = slab j*sH + kh, so the UMMA
-                            // descriptor's atom stride is one slab) and one 4-D box per 32 channels stages dY^T
+                            // ([input row][16 windows][128 B] slabs; atom kh of output row j = slab j*sH + kh, so the
+                            // atom stride is one slab) and one 4-D box per 32 channels stages dY^T
   // Strided conv dgrad (A = DGRAD_K, sH / sW = 2) as sH * sW PARITY CLASSES: the input positions (h, w) = (sH h' + ph,
   // sW w' + pw) of one class receive only the filter taps kh = rh + sH j, kw = rw + sW i (rh = (ph + pH) % sH ...), i.e.
   // each class is a unit-stride convolution over dY with nh x nw taps (3x3 stride 2: 1 + 2 + 2 + 4 = 9 taps for the four
@@ -642,13 +574,13 @@ struct Launch {
   int par_lo[2];     // im2col origin offset (w, h) shared by the classes: (p + ph) / s - (taps - 1)
   PosDiv sub;        // fast divisors of the sub-grid extents
   ParCls par_cls[4];
-  // Stream-K: the linear space (tile, K chunk) is cut into one contiguous range per unit (CTA or CTA pair), so every
+  // Stream-K: the linear space (tile, K chunk) is cut into one contiguous range per unit (CTA), so every
   // SM gets the same number of chunks whatever the tile count.  A tile whose chunks span several units is reduced
   // through the workspace by the LAST unit to arrive at its counter (no unit ever waits for another).
   int sk;
   int nkt;           // K chunks per tile
-  float* ws_tiles;   // partial-sum slots: [unit][2][rank][128][bn]
-  int* ws_cnt;       // arrival counters [tile][rank][epilogue warp], zero between launches
+  float* ws_tiles;   // partial-sum slots: [unit][2][128][bn]
+  int* ws_cnt;       // arrival counters [tile][consumer warp], zero between launches
   unsigned long long* trace;   // diagnostic build only
   int bounds[MAX_UNITS + 1];
 };
@@ -668,8 +600,7 @@ struct TileInfo {
 
 // Linear tile index -> (m tile fastest, n tile, z = batch|tap x split): CTAs that run concurrently share the
 // same weight (B) tile in L2.
-__device__ __forceinline__ void decode_tile(const vlfb_gemm_params_t& p, const Launch& L, int t, int rank, int split_k,
-                                            TileInfo& ti) {
+__device__ __forceinline__ void decode_tile(const vlfb_gemm_params_t& p, const Launch& L, int t, int split_k, TileInfo& ti) {
   const int mt = t % L.tiles_m;
   const int r = t / L.tiles_m;
   const int nt = r % L.tiles_n;
@@ -677,7 +608,7 @@ __device__ __forceinline__ void decode_tile(const vlfb_gemm_params_t& p, const L
   const int split = z % split_k, zz = z / split_k;
   ti.batch = (p.taps > 1) ? 0 : zz;
   ti.tap = (p.taps > 1) ? zz : 0;
-  ti.m0 = mt * L.tile_rows + rank * BM;
+  ti.m0 = mt * BM;
   ti.n0 = nt * L.bn;
   int kper = (p.K + split_k - 1) / split_k;
   kper = (kper + KC - 1) / KC * KC;
@@ -707,7 +638,7 @@ __device__ __forceinline__ int patch_row(const vlfb_gemm_params_t& p, const Laun
   return (rest * p.g.Ho + hb * 8 + (r >> 4)) * p.g.Wo + wb * 16 + (r & 15);
 }
 
-// Every role of a CTA (and both CTAs of a pair) walks the same work sequence.  cur/lim = next tile index / tile
+// Every role of a CTA walks the same work sequence.  cur/lim = next tile index / tile
 // count (static loop, stride = #units) or next / end position in the (tile, K chunk) space (stream-K).
 struct Sched { int cur, lim; };
 __device__ __forceinline__ void sched_init(Sched& s, const Launch& L, int unit) {
@@ -715,13 +646,13 @@ __device__ __forceinline__ void sched_init(Sched& s, const Launch& L, int unit) 
   s.lim = L.sk ? L.bounds[unit + 1] : L.total_tiles;
 }
 __device__ __forceinline__ bool sched_next(const vlfb_gemm_params_t& p, const Launch& L, Sched& s, int unit, int nunits,
-                                           int rank, TileInfo& ti) {
+                                           TileInfo& ti) {
   if (L.sk) {
     if (s.cur >= s.lim) return false;
     const int tile = s.cur / L.nkt;
     const int c0 = s.cur - tile * L.nkt;
     const int len = min(L.nkt - c0, s.lim - s.cur);
-    decode_tile(p, L, tile, rank, 1, ti);
+    decode_tile(p, L, tile, 1, ti);
     ti.k_begin = c0 * KC;
     ti.k_end = min(p.K, (c0 + len) * KC);
     ti.nk = len;
@@ -738,49 +669,46 @@ __device__ __forceinline__ bool sched_next(const vlfb_gemm_params_t& p, const La
     return true;
   }
   while (s.cur < s.lim) {
-    decode_tile(p, L, s.cur, rank, p.split_k, ti);
+    decode_tile(p, L, s.cur, p.split_k, ti);
     s.cur += nunits;
     if (ti.nk != 0 || L.par) return true;
   }
   return false;
 }
 
-// Persistent, warp-specialised: grid = min(#tiles, #SMs) CTAs (PAIR: 2 x #pairs in clusters of two); every role walks
-// the same work sequence (Sched).  The smem ring (full/empty) runs continuously across tiles and the TMEM accumulator
-// is double-buffered (tmem_full/tmem_empty), so the epilogue of tile i overlaps the loads and MMAs of tile i+1.
-// PAIR (both operands staged by TMA only): the two CTAs of a cluster own one 256 x bn tile; CTA r stages A rows
-// [m0 + 128 r, +128) and B rows [n0 + (bn/2) r, +bn/2); the leader issues tcgen05.mma.cta_group::2 (M = 256) which
-// reads both CTAs' shared memory and writes 128 accumulator lanes x bn columns into EACH CTA's TMEM, so every SM
-// receives (128 + bn/2) x 128 B per K chunk instead of (128 + bn) x 128 B for the same MACs.
-// CP = false: both operands are staged by TMA, so ONE producer warp suffices and the CTA is 10 warps (producer, MMA
-// issuer, 8 epilogue warps) with up to 168 registers per thread -- the 17-warp CP = true build (8 cp.async gather
-// warps: conv1 stem, strided dgrad, operands TMA cannot address) is capped at 96 and spills in the epilogue.
-template <int AK, int BK, bool MASK, bool PAIR, bool CP>
-__global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm_tc_kernel(const vlfb_gemm_params_t p, const Launch L,
+// Persistent, warp-specialised: grid = min(#tiles, #SMs) CTAs; every role walks the same work sequence (Sched).  The
+// smem ring (full/empty) runs continuously across tiles, so the producers stage the next tile while the consumers
+// run the epilogue of the current one.
+// CP = false: both operands are staged by TMA, so one producer warpgroup (one issuing warp) suffices and the CTA is
+// 12 warps with up to 168 registers per thread; the 16-warp CP = true build (8 cp.async gather warps: conv1 stem,
+// strided dgrad, operands TMA cannot address) is capped at 128.
+// FIX: the stream-K fix-up (a piece of a shared tile through the workspace) is compiled in.  Its last-arriver decision
+// is per warp, so the warps of a warpgroup may diverge there and ptxas then serialises the wgmma of the whole kernel;
+// only the launches that plan fix-ups use these instantiations, every other launch keeps the MMA pipeline.
+template <int AK, int BK, bool MASK, bool CP, bool FIX>
+__global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_kernel(const vlfb_gemm_params_t p, const Launch L,
                                                               const __grid_constant__ CUtensorMap tmA,
                                                               const __grid_constant__ CUtensorMap tmB) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int bn = L.bn, S = L.stages;
-  const int bnh = PAIR ? (bn >> 1) : bn;                    // B rows (columns of D) staged by this CTA
-  const uint32_t b_tile_bytes = (uint32_t)bnh * KC * 4;
+  const int bnh = bn;
+  const uint32_t b_tile_bytes = (uint32_t)bn * KC * 4;
   const uint32_t stage_bytes = A_TILE_BYTES + b_tile_bytes;
-  const uint32_t epi_base = smem_base + S * stage_bytes;                  // per-epilogue-warp transpose tiles
+  // K-major images of the MN-major operands (wgmma reads tf32 operands K-major only)
+  constexpr bool TA = is_mn(AK), TB = is_mn(BK);
+  const uint32_t ka_img = smem_base + S * stage_bytes;
+  const uint32_t kb_img = ka_img + (TA ? (uint32_t)A_TILE_BYTES : 0u);
+  const uint32_t epi_base = kb_img + (TB ? b_tile_bytes : 0u);          // per-consumer-warp transpose tiles
   const uint32_t bar_base = epi_base + EPI_STAGE_BYTES;
   const uint32_t full0 = bar_base, empty0 = bar_base + 8 * MAX_STAGES;
-  const uint32_t tfull0 = bar_base + 16 * MAX_STAGES, tempty0 = tfull0 + 16;
-  const uint32_t tptr_addr = tempty0 + 16;
-  volatile uint32_t* tptr_generic =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tptr_addr - smem_u32(smem_raw)));
 
-  static_assert(!(PAIR && CP), "CTA pairs need both operands staged by TMA");
-  constexpr int NPRODT = CP ? NPROD : 32 * NTMAW;   // producer threads of this build
+  constexpr int NPRODT = CP ? NPROD : NPROD_TMA;   // producer threads of this build
   constexpr int NPWT = NPRODT / 32;
-  constexpr int NTHR = NPRODT + 32 + NEPI;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int rank = PAIR ? (int)cluster_ctarank() : 0;
-  const int unit = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int nunits = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int tid = threadIdx.x;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform role: producer / consumer branches are not divergent
+  const int unit = (int)blockIdx.x;
+  const int nunits = (int)gridDim.x;
   const bool tma_a = L.tma_a != 0, tma_b = L.tma_b != 0;
   const bool cp_any = CP && !(tma_a && tma_b);
 
@@ -795,23 +723,11 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(full0 + 8 * s, (cp_any ? NPROD : 0) + ((tma_a || tma_b) ? 1 : 0));
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, PAIR ? 2 * (NEPI / 32) : NEPI / 32);       // one arrival per epilogue warp
+      mbar_init(empty0 + 8 * s, NEPI / 128);          // one arrival per consumer warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  uint32_t tmem_cols = 32;              // tcgen05.alloc takes a power of two >= 32; two accumulators of bn columns
-  while (tmem_cols < (uint32_t)(2 * bn)) tmem_cols <<= 1;
-  if (warp == NPWT) {
-    if (PAIR) tmem_alloc2(tptr_addr, tmem_cols); else tmem_alloc(tptr_addr, tmem_cols);
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all(); else __syncthreads();     // PAIR: the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem = *tptr_generic;
+  __syncthreads();
   if (tid == 0) TR(2);
 
   if (warp < NPWT) {
@@ -821,11 +737,11 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
     // themselves; issuer `hid` launches the boxes b with b % NISS == hid; issuer 0 posts the expected byte count.
     constexpr int NISS = CP ? 1 : NTMAW;
     const int hid = CP ? 0 : (tid >> 5);
-    const bool issuer = CP ? (tid == 0) : ((tid & 31) == 0);
+    const bool issuer = CP ? (tid == 0) : ((tid & 31) == 0 && hid < NTMAW);
     if (cp_any || issuer) {
       KLoader<is_mn(AK) ? VLFB_OP_DENSE_K : AK, BM / RSTEP> ka;
       MNLoader<is_mn(AK) ? AK : VLFB_OP_DENSE_MN> ma;
-      KLoader<is_mn(BK) ? VLFB_OP_DENSE_K : BK, 256 / RSTEP> kb;
+      KLoader<is_mn(BK) ? VLFB_OP_DENSE_K : BK, BN_MAX / RSTEP> kb;
       MNLoader<is_mn(BK) ? BK : VLFB_OP_DENSE_MN> mb;
       const int LAG = L.lag;
       // compile-time gates keep the im2col state out of the instantiations that cannot use it (registers)
@@ -838,39 +754,29 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
       int ib_c[NATOM], ib_off[NATOM], ib_atoms = 0;
       // conv1 stem rows (tma 3): the 128 tile rows = 8 groups of 16 consecutive output positions (16 | Wo, so a group
       // never crosses an output row): per group the window origin (wo, hi0 = ho sH - pH, ti0 = to sT - pT, n)
-      const bool stem_a = !PAIR && AK == VLFB_OP_STEM_K && L.tma_a == 3;
-      const bool stem_b = !PAIR && BK == VLFB_OP_STEM_MN && L.tma_b == 3;
+      const bool stem_a = AK == VLFB_OP_STEM_K && L.tma_a == 3;
+      const bool stem_b = BK == VLFB_OP_STEM_MN && L.tma_b == 3;
       constexpr int NSG = AK == VLFB_OP_STEM_K ? 8 : 1;
       int sg_w[NSG], sg_ht[NSG], sg_n[NSG];
       // chunk counter over the CTA's whole work sequence; ring slot / phase / lagged slot advance
       // incrementally (S is a run-time value: `it % S` cost three integer divisions per chunk per thread)
       int it = 0, s = 0, sl = 0;
       uint32_t ph = 0;
-      // PAIR: every copy of either CTA completes on the LEADER's stage barrier
-      const uint32_t fullx = PAIR ? mapa_rank(full0, 0) : full0;
-      auto ld3 = [&](uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, uint32_t bar) {
-        if (PAIR) tma_load_3d_2(dst, tm, c0, c1, c2, bar); else tma_load_3d(dst, tm, c0, c1, c2, bar);
-      };
-      auto ldi = [&](uint32_t dst, const CUtensorMap* tm, int c, int w, int h, int d, int n, int ow, int oh, int od,
-                     uint32_t bar) {
-        if (PAIR) tma_load_im2col_2(dst, tm, c, w, h, d, n, ow, oh, od, bar);
-        else tma_load_im2col(dst, tm, c, w, h, d, n, ow, oh, od, bar);
-      };
+      const uint32_t fullx = full0;
       Sched sc;
       sched_init(sc, L, unit);
       TileInfo ti;
       int witem = 0;
-      while (sched_next(p, L, sc, unit, nunits, rank, ti)) {
+      while (sched_next(p, L, sc, unit, nunits, ti)) {
         if (tid == 0 && witem < 4) TR(8 + 2 * witem);
-        const int nb0 = ti.n0 + rank * bnh;              // first D column whose B rows this CTA stages
+        const int nb0 = ti.n0;                           // first D column whose B rows this CTA stages
         if (cp_any) {
           if (!tma_a) { if (is_mn(AK)) ma.init(p, p.a, ti.m0, BM, p.M, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { ka.init(p, p.a, ti.m0, BM, p.M, ti.batch, L.out, L.in, ti.k_begin / KC); ka.kend = ti.k_end; } }
           if (!tma_b) { if (is_mn(BK)) mb.init(p, p.b, ti.n0, bn, p.N, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { kb.init(p, p.b, ti.n0, bn, p.N, ti.batch, L.out, L.in, ti.k_begin / KC); kb.kend = ti.k_end; } }
         }
         const int kc0 = ti.k_begin / KC;
-        // bytes the stage barrier expects: this CTA's copies (PAIR: both CTAs', posted by the leader)
+        // bytes the stage barrier expects
         uint32_t tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + (tma_b ? b_tile_bytes : 0u);
-        if (PAIR) tma_bytes *= 2u;
         if (issuer && stem_a && L.stem_patch) {
           const vlfb_conv_geom_t& g = p.g;
           const int mt = ti.m0 / BM;
@@ -920,7 +826,6 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         if (issuer && im2col_b) {
           const vlfb_conv_geom_t& g = p.g;
           ib_atoms = 0;
-          int peer_atoms = 0;
 #pragma unroll
           for (int a = 0; a < NATOM; ++a) {
             const int ncol = nb0 + a * 32;
@@ -932,9 +837,8 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
               ib_off[a] = ((int)qh * g.dH << 16) | ((int)qw * g.dW);
               ib_atoms = a + 1;
             }
-            if (PAIR && a * 32 < bnh && ti.n0 + (rank ^ 1) * bnh + a * 32 < p.N) peer_atoms = a + 1;
           }
-          tma_bytes = (PAIR ? 2u : 1u) * (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + 4096u * (uint32_t)(ib_atoms + peer_atoms);
+          tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + 4096u * (uint32_t)ib_atoms;
         }
         if (issuer && stem_b) {
           ib_atoms = 0;                                             // atoms = filter rows kh of this N tile
@@ -949,8 +853,7 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         for (int i = 0; i < ti.nk; ++i, ++it) {
           // Helper issuers (hid > 0) wait for the free stage LAZILY, right before their first box of the chunk: an issuer
           // without a box in a chunk (2-box chunks on 3 issuers) must not wait at all -- nothing would depend on it, the
-          // others would lap it by two phases of the stage barrier and its parity wait would then never return (call P:
-          // exactly that hang, 4 s later the watchdog trap, in the full-size captured step).
+          // others would lap it by two phases of the stage barrier and its parity wait would then never return.
           const bool need_wait = it >= S;
           const uint32_t wpar = ph ^ 1u;
           const int s_cur = s;
@@ -960,7 +863,7 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
           const uint32_t b_tile = a_tile + A_TILE_BYTES;
           const uint32_t fbar = fullx + 8 * s_cur;
           if (issuer && tma_bytes) {
-            if (hid == 0 && (!PAIR || rank == 0)) mbar_expect_tx(full0 + 8 * s_cur, tma_bytes);
+            if (hid == 0) mbar_expect_tx(full0 + 8 * s_cur, tma_bytes);
             int box = 0;                                  // boxes of this chunk, in issue order
             bool waited = NISS == 1 || hid == 0;
             auto mine = [&]() {
@@ -986,19 +889,19 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
             } else if (im2col_a) {
               const vlfb_conv_geom_t& g = p.g;
               if (AK == VLFB_OP_CONV_K) {
-                if (mine()) ldi(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, ic_w * g.dW, ic_h * g.dH, ic_t * g.dT, fbar);
+                if (mine()) tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, ic_w * g.dW, ic_h * g.dH, ic_t * g.dT, fbar);
               } else if (AK == VLFB_OP_DGRAD_K && L.par) {
                 // tap (kt, rh + sH ic_h, rw + sW ic_w) of the class: dY offset (taps - 1 - index), weights at the original tap
                 const ParCls& c = L.par_cls[ti.batch];
-                if (mine()) ldi(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, c.nw - 1 - ic_w, c.nh - 1 - ic_h, (g.kT - 1 - ic_t) * g.dT, fbar);
+                if (mine()) tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, c.nw - 1 - ic_w, c.nh - 1 - ic_h, (g.kT - 1 - ic_t) * g.dT, fbar);
                 const int tap = (ic_t * g.kH + c.rh + g.sH * ic_h) * g.kW + c.rw + g.sW * ic_w;
-                if (mine()) ld3(b_tile, &tmB, tap * g.Co + ic_c * KC, nb0, 0, fbar);
+                if (mine()) tma_load_3d(b_tile, &tmB, tap * g.Co + ic_c * KC, nb0, 0, fbar);
                 if (++ic_c == icpt) {
                   ic_c = 0;
                   if (++ic_w == c.nw) { ic_w = 0; if (++ic_h == c.nh) { ic_h = 0; ++ic_t; } }
                 }
               } else {
-                if (mine()) ldi(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, (g.kW - 1 - ic_w) * g.dW,
+                if (mine()) tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, (g.kW - 1 - ic_w) * g.dW,
                     (g.kH - 1 - ic_h) * g.dH, (g.kT - 1 - ic_t) * g.dT, fbar);
               }
               if (!(AK == VLFB_OP_DGRAD_K && L.par) && ++ic_c == icpt) {
@@ -1010,9 +913,9 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
                 if (mine()) tma_load_4d(a_tile, &tmA, 0, ti.k_begin + i * KC, ti.m0 >> 5, ti.batch, fbar);
               } else if (is_mn(AK)) {
                 for (int a = 0; a < BM / 32; ++a)
-                  if (mine()) ld3(a_tile + a * 4096, &tmA, ti.m0 + a * 32, ti.k_begin + i * KC, ti.batch, fbar);
+                  if (mine()) tma_load_3d(a_tile + a * 4096, &tmA, ti.m0 + a * 32, ti.k_begin + i * KC, ti.batch, fbar);
               } else {
-                if (mine()) ld3(a_tile, &tmA, (kc0 + i) * KC, ti.m0, ti.batch, fbar);
+                if (mine()) tma_load_3d(a_tile, &tmA, (kc0 + i) * KC, ti.m0, ti.batch, fbar);
               }
             }
             if (stem_b && L.stem_patch) {
@@ -1055,16 +958,16 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
 #pragma unroll
               for (int a = 0; a < NATOM; ++a)
                 if (a < ib_atoms)
-                  if (mine()) ldi(b_tile + a * 4096, &tmB, ib_c[a], bw, bh, bd, o.n, ib_off[a] & 0xFFFF, ib_off[a] >> 16,
+                  if (mine()) tma_load_im2col(b_tile + a * 4096, &tmB, ib_c[a], bw, bh, bd, o.n, ib_off[a] & 0xFFFF, ib_off[a] >> 16,
                       ti.tap * g.dT, fbar);
             } else if (tma_b && !(AK == VLFB_OP_DGRAD_K && L.par)) {
               if (is_mn(BK) && L.tma_b == 4) {
                 if (mine()) tma_load_4d(b_tile, &tmB, 0, ti.k_begin + i * KC, nb0 >> 5, ti.batch, fbar);
               } else if (is_mn(BK)) {
                 for (int a = 0; a < bnh / 32; ++a)
-                  if (mine()) ld3(b_tile + a * 4096, &tmB, nb0 + a * 32, ti.k_begin + i * KC, ti.batch, fbar);
+                  if (mine()) tma_load_3d(b_tile + a * 4096, &tmB, nb0 + a * 32, ti.k_begin + i * KC, ti.batch, fbar);
               } else {
-                if (mine()) ld3(b_tile, &tmB, (kc0 + i) * KC, nb0, ti.batch, fbar);
+                if (mine()) tma_load_3d(b_tile, &tmB, (kc0 + i) * KC, nb0, ti.batch, fbar);
               }
             }
           }
@@ -1097,76 +1000,22 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         }
       }
     }
-  } else if (warp == NPWT) {
-    // ============================ MMA ISSUER (1 thread; PAIR: the leader CTA's) ============================
-    if ((tid & 31) == 0 && rank == 0) {
-      const uint32_t idesc = make_idesc(bn, is_mn(AK) ? 1 : 0, is_mn(BK) ? 1 : 0, PAIR ? 2 * BM : BM);
-      // K-major tile: SWIZZLE_128B, LBO 16, SBO 1024, K step 32 B; MN-major: SWIZZLE_128B_BASE32B, LBO 4096, SBO 512,
-      // K step 1024 B (4 k-rows of 128 B per 32-element atom)
-      const uint64_t a_d0 = is_mn(AK) ? make_desc(smem_base, 4096, 512, 1) : make_desc(smem_base, 16, 1024);
-      const uint64_t b_d0 = is_mn(BK) ? make_desc(smem_base + A_TILE_BYTES, 4096, 512, 1) : make_desc(smem_base + A_TILE_BYTES, 16, 1024);
-      const uint32_t a_hi = (uint32_t)(a_d0 >> 32), b_hi = (uint32_t)(b_d0 >> 32);
-      const uint32_t a_lo0 = (uint32_t)a_d0, b_lo0 = (uint32_t)b_d0;
-      const uint32_t stage_units = stage_bytes >> 4;
-      // conv1 wgrad patch chunks: atoms (filter rows) are one 2 KB input-row slab apart (LBO 2048), the second output row
-      // of the patch starts sH slabs further
-      const bool stem_pb = !PAIR && BK == VLFB_OP_STEM_MN && L.tma_b == 3 && L.stem_patch != 0;
-      const uint32_t b_lo0_pb = (uint32_t)make_desc(smem_base + A_TILE_BYTES, 2048, 512, 1);     // LBO lives in the low word
-      const uint32_t pb_rowstep = (uint32_t)(p.g.sH * 2048) >> 4;
-      constexpr uint32_t a_kstep = is_mn(AK) ? (1024u >> 4) : (32u >> 4), b_kstep = is_mn(BK) ? (1024u >> 4) : (32u >> 4);
-      int it = 0, tile_iter = 0, s = 0;
-      uint32_t ph = 0;
-      Sched sc;
-      sched_init(sc, L, unit);
-      TileInfo ti;
-      while (sched_next(p, L, sc, unit, nunits, rank, ti)) {
-        const int acc = tile_iter & 1;
-        if (tile_iter >= 2) {                          // wait until the epilogue(s) drained this accumulator
-          mbar_wait(tempty0 + 8 * acc, ((tile_iter >> 1) - 1) & 1);
-          tc_fence_after();
-        }
-        const uint32_t d_tmem = tmem + (uint32_t)(acc * bn);
-        for (int i = 0; i < ti.nk; ++i, ++it) {
-          mbar_wait(full0 + 8 * s, ph);
-          if (i == 0 && tile_iter < 4) TR(16 + 2 * tile_iter);
-          tc_fence_after();
-          // descriptors of the stage: only the 14-bit start-address field moves (by stage, then by the 32-byte /
-          // 1024-byte K step of a K-major / MN-major tile), so each MMA costs one 32-bit add per operand instead of
-          // re-encoding the descriptor (trace r2b: the issue loop, not the tensor pipe, paced tiles narrower than 256)
-          const uint32_t a_lo = a_lo0 + (uint32_t)s * stage_units, b_lo = b_lo0 + (uint32_t)s * stage_units;
-#pragma unroll
-          for (int j = 0; j < KC / 8; ++j) {          // UMMA K = 8 for tf32
-            const uint64_t da = ((uint64_t)a_hi << 32) | (uint64_t)(a_lo + (uint32_t)j * a_kstep);
-            uint64_t db = ((uint64_t)b_hi << 32) | (uint64_t)(b_lo + (uint32_t)j * b_kstep);
-            if (BK == VLFB_OP_STEM_MN && stem_pb)     // k rows 0-15 = output row 0 (slab kh), 16-31 = output row 1 (slab sH + kh)
-              db = ((uint64_t)b_hi << 32) |
-                   (uint64_t)(b_lo0_pb + (uint32_t)s * stage_units + (uint32_t)(j >> 1) * pb_rowstep + (uint32_t)(j & 1) * (1024u >> 4));
-            if (PAIR) umma_tf32_2(d_tmem, da, db, idesc, (i | j) ? 1u : 0u);
-            else umma_tf32(d_tmem, da, db, idesc, (i | j) ? 1u : 0u);
-          }
-          // frees the smem stage (PAIR: in both CTAs) when these MMAs retire
-          if (PAIR) umma_commit2(empty0 + 8 * s); else umma_commit(empty0 + 8 * s);
-          if (++s == S) { s = 0; ph ^= 1u; }
-        }
-        // accumulator complete -> epilogue (PAIR: of both CTAs); a parity class without taps has nothing to wait for
-        if (!PAIR && ti.nk == 0) mbar_arrive(tfull0 + 8 * acc);
-        else if (PAIR) umma_commit2(tfull0 + 8 * acc); else umma_commit(tfull0 + 8 * acc);
-        if (tile_iter < 4) TR(17 + 2 * tile_iter);
-        ++tile_iter;
-      }
-    }
   } else {
-    // ============================ EPILOGUE (8 warps) ============================
-    // TMEM lane quarter = warp % 4 (hardware rule); the two warps of a quarter take alternate 16-column
-    // blocks.  Each 32x16 block is transposed through a padded shared-memory tile so that a warp store /
-    // residual load / atomic covers 8 rows x 64 contiguous bytes (whole 32-byte sectors).
-    const int ew = warp - NPWT - 1;
-    const int quarter = warp & 3;
-    const int half = ew >> 2;
+    // ============================ CONSUMERS (2 warpgroups: wgmma K loop, then the epilogue) ============================
+    // Warp w of warpgroup g holds accumulator rows [64 g + 16 w, +16) of the tile (wgmma fragment layout).  After the K
+    // loop the warp writes them to its padded shared-memory tile (16 x EPITCH), so that the epilogue holds no accumulator
+    // registers and a warp store / residual load / atomic covers 8 rows x 64 contiguous bytes (whole 32-byte sectors).
+    const int ctid = tid - NPRODT;
+    const int wg = ctid >> 7;
+    const int ew = ctid >> 5;            // consumer warp 0-7 = 4 wg + (warp % 4)
+    const int wrow = 16 * ew;            // its first tile row
     const int lane = tid & 31;
+    const bool stem_pb = BK == VLFB_OP_STEM_MN && L.tma_b == 3 && L.stem_patch != 0;
     float* stg = reinterpret_cast<float*>(smem_raw + (epi_base - smem_u32(smem_raw))) + ew * EPI_WARP_FLOATS;
-    float* wsc = stg + 32 * EPITCH;      // column scale of this warp's column blocks, then the bias
-    float* wbi = wsc + 128;
+    float* wsc = stg + 16 * EPITCH;      // column scale of the tile's columns, then the bias
+    float* wbi = wsc + BN_MAX;
+    int s = 0, sprev = 0;
+    uint32_t ph = 0;
     int colv_n0 = -1;
     const bool vec_ok = ((p.ldd & 3) == 0) && ((p.d_batch_stride & 3) == 0) && ((p.d_tap_stride & 3) == 0) &&
                         ((reinterpret_cast<uintptr_t>(p.d) & 15) == 0) &&
@@ -1176,26 +1025,75 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
     const int col = (lane & 3) * 4;
     const bool want_res = (p.residual != nullptr) || (p.flags & VLFB_EPI_ACCUM);
     const float* res_src = p.residual ? p.residual : p.d;
-    const uint32_t tempty_x = (PAIR && rank != 0) ? mapa_rank(tempty0, 0) : tempty0;
-    const int nrank = PAIR ? 2 : 1;
     const size_t ws_tile_floats = (size_t)BM * bn;
     int tile_iter = 0;
     Sched sc;
     sched_init(sc, L, unit);
     TileInfo ti;
-    while (sched_next(p, L, sc, unit, nunits, rank, ti)) {
-      const int acc = tile_iter & 1;
-      const uint32_t lane_addr = tmem + (uint32_t)(acc * bn) + ((uint32_t)(quarter * 32) << 16);
-      const bool par = !PAIR && AK == VLFB_OP_DGRAD_K && L.par != 0;
+    while (sched_next(p, L, sc, unit, nunits, ti)) {
+      // ---- K loop, instantiated per tile width so that the width is a compile-time constant of the MMA loop: the MMAs
+      // of chunk i are in flight while chunk i + 1 is issued; a stage goes back to the producers once the MMAs that
+      // read it have completed (the host keeps the cp.async lag <= stages - 2, so that release never waits on itself)
+      auto mma_tile = [&](auto bn_c) {
+        constexpr int BN = decltype(bn_c)::value;
+        float acc[BN / 2];
+#pragma unroll
+        for (int q = 0; q < BN / 2; ++q) acc[q] = 0.f;
+        for (int i = 0; i < ti.nk; ++i) {
+          mbar_wait(full0 + 8 * s, ph);
+          const uint32_t a_tile = smem_base + s * stage_bytes, b_tile = a_tile + A_TILE_BYTES;
+          if (TA || TB) {
+            wgmma_wait<0>();                     // no MMA still reads the K-major images
+            consumers_sync();
+            if (TA) mn_to_kmajor(a_tile, ka_img, BM, 4096, 0, ctid);
+            if (TB) mn_to_kmajor(b_tile, kb_img, BN, stem_pb ? 2048 : 4096, stem_pb ? p.g.sH : 0, ctid);
+            fence_proxy_async();                 // generic-proxy writes -> visible to the wgmma (async proxy) reads
+            consumers_sync();
+          }
+          const uint32_t a_src = (TA ? ka_img : a_tile) + (uint32_t)wg * (64 * 128);
+          const uint32_t b_src = TB ? kb_img : b_tile;
+          wgmma_fence();
+#pragma unroll
+          for (int j = 0; j < KC / 8; ++j)      // wgmma K = 8 for tf32: 32 bytes along the swizzled 128-byte rows
+            wgmma_tf32<BN>(acc, make_desc(a_src + 32 * j), make_desc(b_src + 32 * j), (i | j) ? 1u : 0u);
+          wgmma_commit();
+          if (i > 0) {
+            wgmma_wait<1>();
+            if ((ctid & 127) == 0) mbar_arrive(empty0 + 8 * sprev);
+          }
+          sprev = s;
+          if (++s == S) { s = 0; ph ^= 1u; }
+        }
+        if (ti.nk > 0) {
+          wgmma_wait<0>();
+          if ((ctid & 127) == 0) mbar_arrive(empty0 + 8 * sprev);
+        }
+        // fragment (n8 group j: rows lane / 4 and lane / 4 + 8, columns 8 j + 2 (lane % 4) + {0, 1}) -> stg
+        float* r = stg + (lane >> 2) * EPITCH + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(r + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(r + 8 * EPITCH + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        __syncwarp();
+      };
+      switch (bn) {
+        case 32: mma_tile(std::integral_constant<int, 32>{}); break;
+        case 64: mma_tile(std::integral_constant<int, 64>{}); break;
+        case 96: mma_tile(std::integral_constant<int, 96>{}); break;
+        default: mma_tile(std::integral_constant<int, 128>{}); break;
+      }
+      if (ew == 0 && lane == 0 && tile_iter < 4) TR(24 + 4 * tile_iter);
+      const bool par = AK == VLFB_OP_DGRAD_K && L.par != 0;
       const int64_t tile_off = par ? 0 : (int64_t)ti.batch * p.d_batch_stride + (int64_t)ti.tap * p.d_tap_stride;
       if ((want_res || MASK) && !par) {
         // pull the NEXT tile's residual / mask rows into L2 while this tile is being written out
         Sched sn = sc;
         TileInfo tn;
-        if (sched_next(p, L, sn, unit, nunits, rank, tn) && tn.npieces() == 1) {
+        if (sched_next(p, L, sn, unit, nunits, tn) && tn.npieces() == 1) {
           const int64_t noff = (int64_t)tn.batch * p.d_batch_stride + (int64_t)tn.tap * p.d_tap_stride;
           const int segs = bn >> 5;
-          for (int idx = tid - (NPRODT + 32); idx < BM * segs; idx += NEPI) {
+          for (int idx = ctid; idx < BM * segs; idx += NEPI) {
             const int row = idx / segs, seg = idx - row * segs;
             const int m = tn.m0 + row, n = tn.n0 + seg * 32;
             if (m < p.M && n < p.N) {
@@ -1209,17 +1107,17 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         // per-column affine of this warp's blocks -> shared memory, once per N tile (not per block: the
         // global-load latency used to sit in front of every block's first FFMA)
         colv_n0 = ti.n0;
-        for (int i = lane; i < (bn >> 1); i += 32) {
-          const int n = ti.n0 + half * EPC + (i >> 4) * (2 * EPC) + (i & 15);
+        for (int i = lane; i < bn; i += 32) {
+          const int n = ti.n0 + i;
           wsc[i] = (p.col_scale && n < p.N) ? p.col_scale[n] : 1.f;
           wbi[i] = (p.col_bias && n < p.N) ? p.col_bias[n] : 0.f;
         }
         __syncwarp();
       }
-      float rs[4];
+      float rs[EROWS];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int m = ti.m0 + quarter * 32 + (lane >> 2) + 8 * i;
+      for (int i = 0; i < EROWS; ++i) {
+        const int m = ti.m0 + wrow + (lane >> 2) + 8 * i;
         rs[i] = (p.row_scale && m < p.M) ? p.row_scale[m] : 1.f;
       }
       // One pass over this warp's column blocks.  mode 0: accumulator -> fused epilogue -> D (whole tile here);
@@ -1235,22 +1133,21 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
           const int n = ti.n0 + c0 + col;
           const bool ok = wres && vec_ok && c0 < bn && n + 3 < p.N;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int m = ti.m0 + quarter * 32 + (lane >> 2) + 8 * i;
+          for (int i = 0; i < EROWS; ++i) {
+            const int m = ti.m0 + wrow + (lane >> 2) + 8 * i;
             r[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (ok && m < p.M) r[i] = ld_nc_f4(res_src + tile_off + (int64_t)m * p.ldd + n);
           }
         };
         // ReLU mask (backward of the ReLU that produced this GEMM's D-shaped input): fetched one block ahead like
         // the residual, but AFTER the accumulator block has left the registers and packed to 16 bits as soon as
-        // it arrives, so that it never coexists with v[] / both residual buffers (register budget of 17 warps;
-        // holding it as 4 more float4 spilled the whole epilogue loop -- measured 1.5-2.8x slower).
+        // it arrives, so that it never coexists with both residual buffers (register budget).
         auto load_mask = [&](int c0, float4* mk) {
           const int n = ti.n0 + c0 + col;
           const bool ok = mode != 1 && vec_ok && c0 < bn && n + 3 < p.N;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int m = ti.m0 + quarter * 32 + (lane >> 2) + 8 * i;
+          for (int i = 0; i < EROWS; ++i) {
+            const int m = ti.m0 + wrow + (lane >> 2) + 8 * i;
             mk[i] = make_float4(1.f, 1.f, 1.f, 1.f);
             if (ok && m < p.M) {
               const int64_t e = tile_off + (int64_t)m * p.ldd + n;
@@ -1266,67 +1163,52 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         auto pack_mask = [](const float4* mk) {
           uint32_t b = 0;
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
+          for (int i = 0; i < EROWS; ++i)
             b |= ((mk[i].x > 0.f ? 1u : 0u) | (mk[i].y > 0.f ? 2u : 0u) | (mk[i].z > 0.f ? 4u : 0u) |
                   (mk[i].w > 0.f ? 8u : 0u)) << (4 * i);
           return b;
         };
         uint32_t mbits = 0xFFFFu;
         if (MASK) {
-          float4 mk[4];
-          load_mask(half * EPC, mk);
+          float4 mk[EROWS];
+          load_mask(0, mk);
           mbits = pack_mask(mk);
         }
         // MASK instantiations keep one residual buffer (register budget)
         constexpr bool DB = !MASK;
-        float4 rr[4], rn[4];
-        if (DB) load_res(half * EPC, rr);          // independent of the accumulator: issued before the wait
-        if (mode != 2) {
-          mbar_wait(tfull0 + 8 * acc, (tile_iter >> 1) & 1);
-          tc_fence_after();
-          if (ew == 0 && lane == 0 && tile_iter < 4) TR(24 + 4 * tile_iter);
-        }
-        for (int c0 = half * EPC; c0 < bn; c0 += 2 * EPC) {
+        float4 rr[EROWS], rn[EROWS];
+        if (DB) load_res(0, rr);          // independent of the accumulator: issued before the wait
+        for (int c0 = 0; c0 < bn; c0 += EPC) {
           if (ti.n0 + c0 >= p.N) break;            // warp-uniform
-          if (DB) load_res(c0 + 2 * EPC, rn);
-          else load_res(c0, rr);                   // L2-resident (tile-ahead prefetch); overlaps the TMEM load
-          if (mode != 2) {
-            float v[EPC];
-            tmem_ld16(lane_addr + c0, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < EPC / 4; ++q)
-              *reinterpret_cast<float4*>(stg + lane * EPITCH + q * 4) =
-                  make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            __syncwarp();
-          }
-          float4 mk[4];
-          if (MASK) load_mask(c0 + 2 * EPC, mk);
+          if (DB) load_res(c0 + EPC, rn);
+          else load_res(c0, rr);                   // L2-resident (tile-ahead prefetch)
+          float4 mk[EROWS];
+          if (MASK) load_mask(c0 + EPC, mk);
           const int n = ti.n0 + c0 + col;
           const bool nfull = n + 3 < p.N;
-          const int cvi = ((c0 - half * EPC) >> 1) + col;
+          const int cvi = c0 + col;
           const float4 cs = *reinterpret_cast<const float4*>(wsc + cvi);
           float4 cb = *reinterpret_cast<const float4*>(wbi + cvi);
           if (mode == 0 && ti.k_begin != 0) cb = make_float4(0.f, 0.f, 0.f, 0.f);      // split-K: bias from the first K slice only
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
+          for (int i = 0; i < EROWS; ++i) {
             const int row = (lane >> 2) + 8 * i;
-            const int m = ti.m0 + quarter * 32 + row;
+            const int m = ti.m0 + wrow + row;
             float4 a4;
             if (mode == 2) {
-              const size_t wso = (size_t)(quarter * 32 + row) * bn + c0 + col;
+              const size_t wso = (size_t)(wrow + row) * bn + c0 + col;
               a4 = make_float4(0.f, 0.f, 0.f, 0.f);
               for (int j = 0; j < ti.npieces(); ++j) {
                 const int sl = (j == 0) ? ti.first_slot() : 0;
-                const float4 w4 = ld_cg_f4(L.ws_tiles + ((size_t)((ti.ufirst() + j) * 2 + sl) * nrank + rank) * ws_tile_floats + wso);
+                const float4 w4 = ld_cg_f4(L.ws_tiles + ((size_t)((ti.ufirst() + j) * 2 + sl) ) * ws_tile_floats + wso);
                 a4.x += w4.x; a4.y += w4.y; a4.z += w4.z; a4.w += w4.w;
               }
             } else {
-              a4 = *reinterpret_cast<const float4*>(stg + row * EPITCH + col);
+              a4 = *reinterpret_cast<const float4*>(stg + row * EPITCH + c0 + col);
             }
             if (mode == 1) {
-              float* const ws_mine = L.ws_tiles + ((size_t)(unit * 2 + ti.slot()) * nrank + rank) * ws_tile_floats;
-              *reinterpret_cast<float4*>(ws_mine + (size_t)(quarter * 32 + row) * bn + c0 + col) = a4;
+              float* const ws_mine = L.ws_tiles + ((size_t)(unit * 2 + ti.slot()) ) * ws_tile_floats;
+              *reinterpret_cast<float4*>(ws_mine + (size_t)(wrow + row) * bn + c0 + col) = a4;
               continue;
             }
             if (m >= p.M || n >= p.N) continue;
@@ -1364,39 +1246,38 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
           if (MASK) mbits = pack_mask(mk);
           if (DB) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) rr[i] = rn[i];
+            for (int i = 0; i < EROWS; ++i) rr[i] = rn[i];
           }
         }
       };
       // The same pass, lean: for tiles whose rows are 16-byte addressable and whose N extent is a whole number of
-      // 16-column blocks (every layer of the networks).  run_blocks spends ~830 instructions per 32 x 16 block
-      // (ncu r2b: per-float4 flag tests, 64-bit address arithmetic and bounds checks) -- 6.3 us for a 128 x 256 tile,
-      // longer than the K loop of most res2 / res3 / res4 layers; here every run-time switch is tested once per tile
-      // (warp-uniform), rows are four precomputed pointers and the column offset is one add per block.
+      // 16-column blocks (every layer of the networks).  run_blocks pays per-float4 flag tests, 64-bit address
+      // arithmetic and bounds checks; here every run-time switch is tested once per tile (warp-uniform), rows are
+      // precomputed 32-bit offsets and the column offset is one add per block.
       auto run_fast = [&](auto mode_c, auto atomic_c, auto wres_c, auto bits_c) {
         constexpr int mode = decltype(mode_c)::value;
         constexpr bool ATOMIC = decltype(atomic_c)::value && mode != 1;
         constexpr bool WRES = decltype(wres_c)::value && mode != 1;
         constexpr bool BITS = decltype(bits_c)::value && mode != 1 && !ATOMIC;      // emit the ReLU sign bits of the result
-        const int r0 = quarter * 32 + (lane >> 2);                         // tile rows r0 + 8 i of this lane
-        const int cbase = half * EPC + col;
-        const bool patch = !PAIR && AK == VLFB_OP_STEM_K && L.stem_patch != 0;
+        const int r0 = wrow + (lane >> 2);                         // tile rows r0 + 8 i of this lane
+        const int cbase = 0 + col;
+        const bool patch = AK == VLFB_OP_STEM_K && L.stem_patch != 0;
         const int mrows = par ? L.par_m : p.M;
         uint32_t rowok = 0;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) rowok |= (patch || ti.m0 + r0 + 8 * i < mrows) ? (1u << i) : 0u;
+        for (int i = 0; i < EROWS; ++i) rowok |= (patch || ti.m0 + r0 + 8 * i < mrows) ? (1u << i) : 0u;
         const int ncols = min(bn, p.N - ti.n0);                            // multiple of 16
         // ONE 32-bit element offset per row, shared by every stream (D, residual, sign bits: same addressing), advanced by
         // one block (32 columns) per step; 64-bit row pointers per stream cost 24 registers, which the look-ahead
         // buffers need (the host / fast_tile test guarantees offsets < 2^32)
-        uint32_t eo[4];
+        uint32_t eo[EROWS];
         float* wsp = nullptr;                  // mode 1: this unit's workspace slot (rows 8 bn apart)
         unsigned short* bout = nullptr;        // relu_bits_out group of tile row r0 + 8 (lane & 3) (this lane stores that row's)
         constexpr bool emit_bits = BITS;
         if (mode == 1)
-          wsp = L.ws_tiles + ((size_t)(unit * 2 + ti.slot()) * nrank + rank) * ws_tile_floats + (size_t)r0 * bn + cbase;
+          wsp = L.ws_tiles + ((size_t)(unit * 2 + ti.slot()) ) * ws_tile_floats + (size_t)r0 * bn + cbase;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < EROWS; ++i) {
           int64_t row = ti.m0 + r0 + 8 * i;
           if (patch) row = patch_row(p, L, ti.m0 / BM, r0 + 8 * i);      // conv1 patch tile: row -> (ho, wo) of the patch
           if (par && ((rowok >> i) & 1u)) row = par_row(p, L, ti.batch, ti.m0 + r0 + 8 * i);   // parity class: sub-grid row -> dX row
@@ -1406,7 +1287,7 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
           const int rb = r0 + 8 * (lane & 3);
           int64_t row = ti.m0 + rb;
           if (patch) row = patch_row(p, L, ti.m0 / BM, rb);
-          bout = reinterpret_cast<unsigned short*>(p.relu_bits_out) + ((tile_off + row * p.ldd + ti.n0 + half * EPC) >> 4);
+          bout = reinterpret_cast<unsigned short*>(p.relu_bits_out) + ((tile_off + row * p.ldd + ti.n0 + 0) >> 4);
         }
         const unsigned short* mbase = reinterpret_cast<const unsigned short*>(p.relu_mask_bits);
         const bool relu = (p.flags & VLFB_EPI_RELU) != 0, tf32 = (p.flags & VLFB_EPI_TF32) != 0;
@@ -1417,8 +1298,8 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         // (MASK builds): the sign bits of the activation that gates this gradient, one 16-bit group per row and block.
         auto load_ahead = [&](bool valid, int ahead, float4* r, uint32_t* m) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint32_t e = eo[i] + (uint32_t)(ahead * 2 * EPC);
+          for (int i = 0; i < EROWS; ++i) {
+            const uint32_t e = eo[i] + (uint32_t)(ahead * EPC);
             if (WRES) {
               r[i] = make_float4(0.f, 0.f, 0.f, 0.f);
               if (valid && ((rowok >> i) & 1u)) r[i] = ld_nc_f4(res_src + e);
@@ -1431,48 +1312,35 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         };
         // Residual / mask operands are fetched VLFB_EPI_DEPTH blocks ahead into a ring of register buffers; the loop is
         // unrolled over the ring so that no buffer is ever copied (a `cur = next` move at the end of an iteration waits
-        // for the load it copies: the first version's look-ahead was worth less than one block, call G).
+        // for the load it copies).
         constexpr int NBUF = VLFB_EPI_DEPTH + 1;
-        float4 rbuf[NBUF][4];
-        uint32_t mbuf[NBUF][4];
-        load_ahead(half * EPC < ncols, 0, rbuf[0], mbuf[0]);
-        if (NBUF == 3) load_ahead(half * EPC + 2 * EPC < ncols, 1, rbuf[1], mbuf[1]);
-        if (mode != 2) {
-          mbar_wait(tfull0 + 8 * acc, (tile_iter >> 1) & 1);
-          tc_fence_after();
-          if (ew == 0 && lane == 0 && tile_iter < 4) TR(24 + 4 * tile_iter);
-        }
+        float4 rbuf[NBUF][EROWS];
+        uint32_t mbuf[NBUF][EROWS];
+        load_ahead(0 < ncols, 0, rbuf[0], mbuf[0]);
+        if (NBUF == 3) load_ahead(0 + EPC < ncols, 1, rbuf[1], mbuf[1]);
         // one 32 x 16 block: operands of block c0 in (rc, mc); the block VLFB_EPI_DEPTH ahead is fetched into (rl, ml)
         auto step = [&](int c0, int cofs, const float4* rc, const uint32_t* mc, float4* rl, uint32_t* ml) {
-          load_ahead(c0 + 2 * EPC * VLFB_EPI_DEPTH < ncols, VLFB_EPI_DEPTH, rl, ml);
-          float4 a4[4];
+          load_ahead(c0 + EPC * VLFB_EPI_DEPTH < ncols, VLFB_EPI_DEPTH, rl, ml);
+          float4 a4[EROWS];
           uint32_t obits = 0;
           if (mode != 2) {
-            float v[EPC];
-            tmem_ld16(lane_addr + c0, v);
-            tmem_ld_wait();
 #pragma unroll
-            for (int q = 0; q < EPC / 4; ++q)
-              *reinterpret_cast<float4*>(stg + lane * EPITCH + q * 4) =
-                  make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              a4[i] = *reinterpret_cast<const float4*>(stg + ((lane >> 2) + 8 * i) * EPITCH + col);
+            for (int i = 0; i < EROWS; ++i)
+              a4[i] = *reinterpret_cast<const float4*>(stg + ((lane >> 2) + 8 * i) * EPITCH + c0 + col);
             __syncwarp();
             if (par && ti.nk == 0) {                                        // class without taps: dX = finish(0)
 #pragma unroll
-              for (int i = 0; i < 4; ++i) a4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+              for (int i = 0; i < EROWS; ++i) a4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
           } else {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) a4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int i = 0; i < EROWS; ++i) a4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             for (int j = 0; j < ti.npieces(); ++j) {                        // piece order: deterministic sum
               const int sl = (j == 0) ? ti.first_slot() : 0;
-              const float* w = L.ws_tiles + ((size_t)((ti.ufirst() + j) * 2 + sl) * nrank + rank) * ws_tile_floats +
+              const float* w = L.ws_tiles + ((size_t)((ti.ufirst() + j) * 2 + sl) ) * ws_tile_floats +
                                (size_t)r0 * bn + cbase + cofs;
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
+              for (int i = 0; i < EROWS; ++i) {
                 const float4 w4 = ld_cg_f4(w + (size_t)i * 8 * bn);
                 a4[i].x += w4.x; a4[i].y += w4.y; a4[i].z += w4.z; a4[i].w += w4.w;
               }
@@ -1480,17 +1348,17 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
           }
           if (mode == 1) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(wsp + (size_t)i * 8 * bn) = a4[i];
-            wsp += 2 * EPC;
+            for (int i = 0; i < EROWS; ++i) *reinterpret_cast<float4*>(wsp + (size_t)i * 8 * bn) = a4[i];
+            wsp += EPC;
             return;
           }
-          const int cvi = ((c0 - half * EPC) >> 1) + col;
+          const int cvi = c0 + col;
           float4 cs = *reinterpret_cast<const float4*>(wsc + cvi);
           float4 cb = *reinterpret_cast<const float4*>(wbi + cvi);
           cs.x *= alpha; cs.y *= alpha; cs.z *= alpha; cs.w *= alpha;
           if (nobias) cb = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
+          for (int i = 0; i < EROWS; ++i) {
             float4 o;
             o.x = fmaf(a4[i].x, cs.x, cb.x); o.y = fmaf(a4[i].y, cs.y, cb.y);
             o.z = fmaf(a4[i].z, cs.z, cb.z); o.w = fmaf(a4[i].w, cs.w, cb.w);
@@ -1507,7 +1375,7 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
               if (ATOMIC) red_add_f4(p.d + eo[i], o);
               else *reinterpret_cast<float4*>(p.d + eo[i]) = o;
             }
-            eo[i] += 2 * EPC;
+            eo[i] += EPC;
             if (emit_bits) {             // the row's 16 sign bits: 4 lanes x 4 columns (warp-uniform branch)
               uint32_t nb = (o.x > 0.f ? 1u : 0u) | (o.y > 0.f ? 2u : 0u) | (o.z > 0.f ? 4u : 0u) | (o.w > 0.f ? 8u : 0u);
               nb <<= (lane & 3) * 4;
@@ -1517,17 +1385,17 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
             }
           }
           if (emit_bits) {
-            if ((rowok >> (lane & 3)) & 1u) *bout = (unsigned short)obits;
-            bout += 2 * EPC / 16;
+            if ((lane & 3) < EROWS && ((rowok >> (lane & 3)) & 1u)) *bout = (unsigned short)obits;
+            bout += EPC / 16;
           }
         };
         {
-          int c0 = half * EPC, cofs = 0;                                    // cofs: column offset of the block from cbase (mode 2)
+          int c0 = 0, cofs = 0;                                    // cofs: column offset of the block from cbase (mode 2)
           while (c0 < ncols) {
 #pragma unroll
             for (int b = 0; b < NBUF; ++b) {
               if (c0 < ncols) step(c0, cofs, rbuf[b], mbuf[b], rbuf[(b + NBUF - 1) % NBUF], mbuf[(b + NBUF - 1) % NBUF]);
-              c0 += 2 * EPC; cofs += 2 * EPC;
+              c0 += EPC; cofs += EPC;
             }
           }
         }
@@ -1543,7 +1411,7 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         else { if (want_res) run_fast(mode_c, F{}, T{}, F{}); else run_fast(mode_c, F{}, F{}, F{}); }
       };
       // (the 17-warp cp.async builds never take the fix-up path: the host plans stream-K fix-ups for TMA-fed launches only)
-      const bool split_tile = !CP && ti.npieces() > 1;
+      const bool split_tile = FIX && !CP && ti.npieces() > 1;
       // (MASK builds: the lean path reads the mask as sign bits; a float mask takes the general path)
       const bool bits_ok = (p.ldd & 15) == 0 && (p.d_batch_stride & 15) == 0 && (p.d_tap_stride & 15) == 0;
       const bool fast_tile = !CP && vec_ok && (p.N & 15) == 0 && span32_ok(p) && !(MASK && (p.relu_mask != nullptr || !bits_ok));
@@ -1559,19 +1427,12 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
         run_blocks(std::integral_constant<int, 0>{});
       }
       if (ew == 0 && lane == 0 && tile_iter < 4) TR(25 + 4 * tile_iter);
-      // every TMEM read of this accumulator has completed (tcgen05.wait::ld above): hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (PAIR && rank != 0) mbar_arrive_cluster(tempty_x + 8 * acc);
-        else mbar_arrive(tempty0 + 8 * acc);
-      }
       ++tile_iter;
-      if constexpr (!CP) if (split_tile) {
+      if constexpr (FIX && !CP) if (split_tile) {
         // publish this piece, count it; the warp that arrives last owns the reduction of its sub-blocks
         __threadfence();
         __syncwarp();
-        int* cnt = L.ws_cnt + ((size_t)ti.tile * nrank + rank) * (NEPI / 32) + ew;
+        int* cnt = L.ws_cnt + (size_t)ti.tile * (NEPI / 32) + ew;
         int old = 0;
         if (lane == 0) old = atomicAdd(cnt, 1);
         old = __shfl_sync(0xffffffffu, old, 0);
@@ -1587,12 +1448,6 @@ __global__ void __launch_bounds__((CP ? NPROD : 32 * NTMAW) + 32 + NEPI, 1) gemm
     }
   }
   if (tid == 0) TR(3);
-  tc_fence_before();
-  if (PAIR) cluster_sync_all(); else __syncthreads();       // PAIR: no CTA exits (or frees TMEM) while its peer can still signal it
-  if (warp == NPWT) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc2(tmem, tmem_cols); else tmem_dealloc(tmem, tmem_cols);
-  }
 }
 
 // ---------------------------------------------------------------- host dispatch
@@ -1633,7 +1488,7 @@ static bool make_tmap(CUtensorMap* tm, const vlfb_operand_t& op, int rows, int K
 }
 
 // Dense MN-major fp32 matrix [K rows][extent] (+batch): box = {32 elements, 32 k-rows, 1} written in the
-// SWIZZLE_128B_ATOM_32B pattern = one UMMA MN-major atom column (4 KB) per copy.
+// SWIZZLE_128B_ATOM_32B pattern = one MN-major atom column (4 KB) per copy.
 static bool make_tmap_mn(CUtensorMap* tm, const vlfb_operand_t& op, int extent, int K, int batch) {
   EncodeTiledFn enc = encode_fn();
   if (!enc || op.kind != VLFB_OP_DENSE_MN || K < KC || extent < 32) return false;
@@ -1650,8 +1505,7 @@ static bool make_tmap_mn(CUtensorMap* tm, const vlfb_operand_t& op, int extent, 
 // The same operand as ONE box per tile: a 4-D view {32 elements of an atom, K rows, atom index, batch} -- the atom
 // dimension has the SMALLEST stride (128 B), which a tiled map may have -- with box {32, 32 k-rows, natoms, 1}: the copy
 // writes atom after atom, i.e. exactly the [atom][k][32] layout the per-atom copies produce, in one instruction instead
-// of 4 (A) / 8 (B).  The TMA unit's cost is per BOX: the 12 small boxes of a wgrad K chunk took 0.72 us against 0.27 us
-// of MMAs (tensor pipe 33-37 % active in every wgrad launch, ncu call M).  Needs whole atoms (extent % 32 == 0).
+// of one per atom.  The TMA unit's cost is per BOX, so fewer boxes per K chunk.  Needs whole atoms (extent % 32 == 0).
 static bool make_tmap_mn4(CUtensorMap* tm, const vlfb_operand_t& op, int extent, int K, int batch, int natoms) {
   EncodeTiledFn enc = encode_fn();
   if (!enc || op.kind != VLFB_OP_DENSE_MN || K < KC || extent < 32 || (extent & 31) || natoms < 1 || natoms > 8) return false;
@@ -1753,14 +1607,13 @@ static bool make_tmap_dy4(CUtensorMap* tm, const float* dy, const vlfb_conv_geom
 }
 
 // tuning overrides, read once (scripts/tune_gemm.py); the per-call fields of vlfb_gemm_params_t take precedence
-struct Env { int bn, stages, lag, pair, sk, debug, no_patch, no_par; bool tma_mn, im2col, fuse_atoms; };
+struct Env { int bn, stages, lag, sk, debug, no_patch, no_par; bool tma_mn, im2col, fuse_atoms; };
 static Env read_env() {
   Env e;
   auto geti = [](const char* name, int dflt) { const char* v = getenv(name); return v ? atoi(v) : dflt; };
   e.bn = geti("VLFB_BN", 0);
   e.stages = geti("VLFB_STAGES", 0);
   e.lag = geti("VLFB_LAG", 0);
-  e.pair = geti("VLFB_PAIR", 0);
   e.sk = geti("VLFB_SK", 0);
   e.debug = geti("VLFB_DEBUG", 0);
   e.no_patch = geti("VLFB_NO_PATCH", 0);
@@ -1775,76 +1628,67 @@ static const Env& env() {
   return e;
 }
 
-// ---- plan: tile width x CTA pairing x schedule, chosen together by a cycle model of one SM -----------------
+// ---- plan: tile width x schedule, chosen together by a cycle model of one SM -----------------------------------
 // A K chunk (32 fp32 of K) of a 128 x bn tile costs max(tensor pipe, operand delivery):
-//   tensor   = 4 MMAs x (128 x bn x 8 MACs) / 2048 MAC/clk = 2 bn clocks (kind::tf32 issues at half the bf16 rate);
-//   delivery = (128 + bn) x 128 B, or (128 + bn/2) x 128 B for a CTA pair, at ~58 B/clk through the SM's
-//              L2 port (ncu r01: 694 MB -> 98 SMs in 70.9 us on res5 branch2b).
+//   tensor   = 128 x bn x 32 MACs / 1024 tf32 MAC/clk (dense H100 SM) = 4 bn clocks;
+//   delivery = (128 + bn) x 128 B through the SM's L2 port at a model rate of 64 B/clk.
 // A tile adds a fixed fill + epilogue cost (~8 chunks' worth); a stream-K launch adds the fix-up of the shared tiles.
-static double chunk_cost(int bn, bool pair) {
-  const double tensor = 2.0 * bn;
-  const double port = (16384.0 + (pair ? 64.0 : 128.0) * bn) / 58.0;
+// The constants rank tile widths against each other; they are model values, not measurements.
+static double chunk_cost(int bn) {
+  const double tensor = 4.0 * bn;
+  const double port = (16384.0 + 128.0 * bn) / 64.0;
   return tensor > port ? tensor : port;
 }
 
 struct Plan { int bn, split_k, pair, sk; int tiles, units; double cost; };
 
-static constexpr bool kind_pair_capable(int kind) { return kind != VLFB_OP_STEM_K && kind != VLFB_OP_STEM_MN; }
-static constexpr bool kind_tma_capable(int) { return true; }
-
-// `pairs` = co-resident CTA pairs (0: pairing unavailable); pair_ok / sk_ok = what the operands / workspace allow.
-static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, int pairs, bool pair_ok, bool sk_ok) {
+// sk_ok = what the workspace allows; pow2_only: a 96-wide request becomes 64 (the cp.async MN-major loader needs a
+// power-of-two tile width).  p.pair is accepted and ignored: Hopper has no CTA-pair MMA (pair is always 0).
+static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool pow2_only = false) {
   const int zbase = p.taps > 1 ? p.taps : p.batch;
   const bool atomic = (p.flags & VLFB_EPI_ATOMIC) != 0;
-  const int want_bn = p.tile_n > 0 ? p.tile_n : env().bn;
-  const int want_pair = p.pair != 0 ? p.pair : env().pair;
+  int want_bn = p.tile_n > 0 ? p.tile_n : env().bn;
+  if (want_bn > BN_MAX) want_bn = BN_MAX;                                      // wider requests get the widest tile
+  if (pow2_only && (want_bn & (want_bn - 1))) want_bn = 64;
   const int want_sk = p.stream_k != 0 ? p.stream_k : env().sk;
   Plan best, best_sk;
   best.cost = 1e30; best.bn = 32; best.split_k = p.split_k > 0 ? p.split_k : 1; best.pair = 0; best.sk = 0;
   best.tiles = 0; best.units = 0;
   best_sk = best;
-  static const int kWidths[] = {256, 192, 128, 96, 64, 32};
-  for (int pr = 0; pr < 2; ++pr) {
-    // CTA pairs and stream-K are opt-in (p.pair / p.stream_k = 1, VLFB_PAIR / VLFB_SK): measured on B200 (profiles/
-    // r02_gemm_variants.txt, r02_trace_*.txt) the K loop of a 128 x 256 tf32 tile already runs at the tensor-pipe
-    // rate (0.287 us per 32-deep chunk = 4 x 128-cycle MMAs), so halving the operand bytes per SM buys nothing, and
-    // the stream-K fix-up costs more than the idle SMs of a 98-tile launch.
-    const bool can_pair = pair_ok && pairs >= 1 && p.M > BM;
-    if (pr == 1 && (!can_pair || want_pair <= 0)) continue;
-    if (pr == 0 && want_pair > 0 && can_pair) continue;
-    const int U = pr ? pairs : num_sms;
-    for (int wi = 0; wi < 6; ++wi) {
-      const int bn = kWidths[wi];
-      if (want_bn > 0 ? bn != want_bn : ((bn & (bn - 1)) != 0)) continue;       // 96 / 192 only on request
-      if (pr && (bn & 63)) continue;                                            // each CTA of a pair stages whole 32-column atoms
-      if (want_bn <= 0 && bn > 32 && p.N <= bn / 2) continue;                   // do not pad N by 2x
-      const int tiles_m = ceil_div(p.M, pr ? 2 * BM : BM);
-      const int64_t T = (int64_t)tiles_m * ceil_div(p.N, bn) * zbase;
-      const int nkt = ceil_div(p.K, KC);
-      const double cc = chunk_cost(bn, pr != 0);
-      const double fixed = 8.0 * cc;
-      // (a) static tile loop, optional plain split-K (atomic epilogues only)
-      const int smax = p.split_k > 0 ? p.split_k : (atomic && p.K >= 512 ? (p.K / 256 < 128 ? p.K / 256 : 128) : 1);
-      for (int sp = (p.split_k > 0 ? p.split_k : 1); sp <= smax; ++sp) {
-        const int64_t tiles = T * sp;
-        const double rounds = (double)((tiles + U - 1) / U);
-        const double cost = rounds * (ceil_div(ceil_div(p.K, sp), KC) * cc + fixed);
-        if (cost < best.cost * 0.999) {
-          best.cost = cost; best.bn = bn; best.split_k = sp; best.pair = pr; best.sk = 0;
-          best.tiles = (int)tiles; best.units = (int)(tiles < U ? tiles : U);
-        }
+  static const int kWidths[] = {128, 96, 64, 32};
+  // Stream-K is opt-in (p.stream_k = 1, VLFB_SK): its fix-up pass costs more than it saves unless the tile count
+  // leaves many SMs idle.
+  const int U = num_sms;
+  for (int wi = 0; wi < 4; ++wi) {
+    const int bn = kWidths[wi];
+    if (want_bn > 0 ? bn != want_bn : ((bn & (bn - 1)) != 0)) continue;       // 96 only on request
+    if (want_bn <= 0 && bn > 32 && p.N <= bn / 2) continue;                   // do not pad N by 2x
+    const int tiles_m = ceil_div(p.M, BM);
+    const int64_t T = (int64_t)tiles_m * ceil_div(p.N, bn) * zbase;
+    const int nkt = ceil_div(p.K, KC);
+    const double cc = chunk_cost(bn);
+    const double fixed = 8.0 * cc;
+    // (a) static tile loop, optional plain split-K (atomic epilogues only)
+    const int smax = p.split_k > 0 ? p.split_k : (atomic && p.K >= 512 ? (p.K / 256 < 128 ? p.K / 256 : 128) : 1);
+    for (int sp = (p.split_k > 0 ? p.split_k : 1); sp <= smax; ++sp) {
+      const int64_t tiles = T * sp;
+      const double rounds = (double)((tiles + U - 1) / U);
+      const double cost = rounds * (ceil_div(ceil_div(p.K, sp), KC) * cc + fixed);
+      if (cost < best.cost * 0.999) {
+        best.cost = cost; best.bn = bn; best.split_k = sp; best.pair = 0; best.sk = 0;
+        best.tiles = (int)tiles; best.units = (int)(tiles < U ? tiles : U);
       }
-      // (b) stream-K: equal chunk ranges; shared tiles reduced through the workspace (or by atomics)
-      const int64_t total = T * nkt;
-      const bool sk_legal = (atomic ? p.split_k != 1 : (sk_ok && p.split_k <= 1)) && want_sk > 0 && nkt >= 2 &&
-                            total >= 2 * (int64_t)U && T * (pr ? 2 : 1) * (NEPI / 32) <= SK_CNT_INTS && U <= MAX_UNITS;
-      if (sk_legal && (T % U) != 0) {
-        const double per_unit = (double)((total + U - 1) / U);
-        const double cost = per_unit * cc + fixed * (double)((T + U - 1) / U) + (atomic ? 1.0 : 2.0) * fixed;
-        if (cost < best_sk.cost * 0.999) {
-          best_sk.cost = cost; best_sk.bn = bn; best_sk.split_k = 1; best_sk.pair = pr; best_sk.sk = 1;
-          best_sk.tiles = (int)T; best_sk.units = U;
-        }
+    }
+    // (b) stream-K: equal chunk ranges; shared tiles reduced through the workspace (or by atomics)
+    const int64_t total = T * nkt;
+    const bool sk_legal = (atomic ? p.split_k != 1 : (sk_ok && p.split_k <= 1)) && want_sk > 0 && nkt >= 2 &&
+                          total >= 2 * (int64_t)U && T * (NEPI / 32) <= SK_CNT_INTS && U <= MAX_UNITS;
+    if (sk_legal && (T % U) != 0) {
+      const double per_unit = (double)((total + U - 1) / U);
+      const double cost = per_unit * cc + fixed * (double)((T + U - 1) / U) + (atomic ? 1.0 : 2.0) * fixed;
+      if (cost < best_sk.cost * 0.999) {
+        best_sk.cost = cost; best_sk.bn = bn; best_sk.split_k = 1; best_sk.pair = 0; best_sk.sk = 1;
+        best_sk.tiles = (int)T; best_sk.units = U;
       }
     }
   }
@@ -1874,46 +1718,20 @@ size_t gemm_tc_workspace_bytes() {
   return (size_t)SK_CNT_INTS * 4 + (size_t)MAX_UNITS * 2 * BM * 256 * 4;
 }
 
-template <int AK, int BK, bool MASK>
-static int max_pairs() {
-  static int cached = -1;
-  if constexpr (!(kind_pair_capable(AK) && kind_pair_capable(BK))) return 0;
-  else if (cached < 0) {
-    cached = 0;
-    if (cudaFuncSetAttribute(gemm_tc_kernel<AK, BK, MASK, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             227 * 1024) == cudaSuccess) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(2 * MAX_UNITS);
-      cfg.blockDim = dim3(32 + 32 + NEPI);
-      cfg.dynamicSmemBytes = 200 * 1024;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<AK, BK, MASK, true, false>, &cfg) == cudaSuccess && n > 0)
-        cached = n < MAX_UNITS ? n : MAX_UNITS;
-    }
-    cudaGetLastError();
-  }
-  return cached;
-}
-
-template <int AK, int BK, bool MASK, bool PAIR, bool CP>
+template <int AK, int BK, bool MASK, bool CP, bool FIX>
 static int launch_variant(const cudaLaunchConfig_t& cfg, const vlfb_gemm_params_t& p, const Launch& L, const CUtensorMap& tmA,
                           const CUtensorMap& tmB) {
   static bool attr_done = false;
   cudaError_t e;
   if (!attr_done) {
-    e = cudaFuncSetAttribute(gemm_tc_kernel<AK, BK, MASK, PAIR, CP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    e = cudaFuncSetAttribute(gemm_tc_kernel<AK, BK, MASK, CP, FIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(smem): %s", cudaGetErrorString(e));
       return VLFB_E_CUDA;
     }
     attr_done = true;
   }
-  e = cudaLaunchKernelEx(&cfg, gemm_tc_kernel<AK, BK, MASK, PAIR, CP>, p, L, tmA, tmB);
+  e = cudaLaunchKernelEx(&cfg, gemm_tc_kernel<AK, BK, MASK, CP, FIX>, p, L, tmA, tmB);
   if (e != cudaSuccess) {
     set_error("gemm_tc launch: %s", cudaGetErrorString(e));
     return VLFB_E_CUDA;
@@ -1939,16 +1757,12 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   if (num_sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+    if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
     if (num_sms > MAX_UNITS) num_sms = MAX_UNITS;
   }
   const Env& ev = env();
   const vlfb_conv_geom_t& g = p.g;
   const bool unit_dgrad = g.sT == 1 && g.sH == 1 && g.sW == 1;
-  // can both operands be staged by TMA (the precondition of CTA pairs)?  Decided on the cheap conditions here; the
-  // tensor maps themselves are encoded after the plan (their boxes depend on it) and a failure falls back below.
-  bool pair_ok = kind_pair_capable(AK) && kind_pair_capable(BK) && encode_fn() != nullptr && ev.im2col &&
-                 (ev.tma_mn || !(is_mn(AK) || is_mn(BK))) && !(AK == VLFB_OP_DGRAD_K && !unit_dgrad) && p.K >= KC;
   bool sk_ws = p.workspace != nullptr && p.workspace_bytes >= gemm_tc_workspace_bytes() &&
                      (reinterpret_cast<uintptr_t>(p.workspace) & 15) == 0;
   alignas(64) CUtensorMap tmA, tmB;
@@ -1994,23 +1808,23 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       L.sub.w = make_fastdiv(Ws); L.sub.h = make_fastdiv(Hs); L.sub.t = make_fastdiv(g.T);
       par_lo[2] = g.pT - (g.kT - 1);
       par_hi[0] = par_lo[0] + Ws - g.Wo; par_hi[1] = par_lo[1] + Hs - g.Ho; par_hi[2] = par_lo[2] + g.T - g.To;
-      pair_ok = false;
       sk_ws = false;
     }
   }
   Plan plan;
-  for (int attempt = 0; attempt < 2; ++attempt) {
+  bool pow2_only = false;
+  for (int attempt = 0; attempt < 4; ++attempt) {
     if (L.par) {                       // plan for the class sub-problems: M' rows, one z slice per class
       vlfb_gemm_params_t pp = p;
       pp.M = L.par_m; pp.batch = L.par; pp.K = L.par_cls[0].nk * KC;
-      plan = make_plan(pp, num_sms, 0, false, false);
+      plan = make_plan(pp, num_sms, false, pow2_only);
       plan.split_k = 1;
     } else {
-      plan = make_plan(p, num_sms, pair_ok ? max_pairs<AK, BK, MASK>() : 0, pair_ok, sk_ws);
+      plan = make_plan(p, num_sms, sk_ws, pow2_only);
     }
     L.bn = plan.bn;
     p.split_k = plan.split_k;
-    const int bnh = plan.pair ? L.bn / 2 : L.bn;
+    const int bnh = L.bn;
     memset(&tmA, 0, sizeof(tmA));
     memset(&tmB, 0, sizeof(tmB));
     const bool mn_tma = ev.tma_mn;
@@ -2019,7 +1833,7 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
     L.tma_b = (BK == VLFB_OP_DENSE_K && make_tmap(&tmB, p.b, p.N, p.K, p.batch, bnh)) ||
               (BK == VLFB_OP_DENSE_MN && mn_tma && make_tmap_mn(&tmB, p.b, p.N, p.K, p.batch)) ? 1 : 0;
     // MN-major tiles as ONE box (all atoms of the tile) instead of one box per 32-element atom
-    if (ev.fuse_atoms && !plan.pair) {
+    if (ev.fuse_atoms) {
       if (AK == VLFB_OP_DENSE_MN && L.tma_a == 1 && make_tmap_mn4(&tmA, p.a, p.M, p.K, p.batch, BM / 32)) L.tma_a = 4;
       if (BK == VLFB_OP_DENSE_MN && L.tma_b == 1 && make_tmap_mn4(&tmB, p.b, p.N, p.K, p.batch, bnh / 32)) L.tma_b = 4;
     }
@@ -2083,27 +1897,30 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
                            CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
         L.tma_b = 2;
       // ... and without spatial taps the whole B tile of a chunk is one dense box (make_tmap_conv_flat)
-      if (BK == VLFB_OP_CONV_MN && L.tma_b == 2 && ev.fuse_atoms && !plan.pair &&
+      if (BK == VLFB_OP_CONV_MN && L.tma_b == 2 && ev.fuse_atoms &&
           make_tmap_conv_flat(&tmB, p.b.ptr, g, bnh / 32))
         L.tma_b = 5;
     }
+    if (is_mn(BK) && !L.tma_b && (L.bn & (L.bn - 1)) && !pow2_only) { pow2_only = true; continue; }
     const bool fixup = plan.sk && !(p.flags & VLFB_EPI_ATOMIC);
-    if (!(plan.pair || fixup) || (L.tma_a && L.tma_b)) break;
-    pair_ok = false;                   // an operand fell back to cp.async: plan again without pairing / fix-ups
-    sk_ws = false;
+    if (!fixup || (L.tma_a && L.tma_b)) break;
+    sk_ws = false;                     // an operand fell back to cp.async: plan again without fix-ups
   }
   const int zbase = L.par ? L.par : (p.taps > 1 ? p.taps : p.batch);
-  L.tile_rows = plan.pair ? 2 * BM : BM;
-  L.tiles_m = ceil_div(L.par ? L.par_m : p.M, L.tile_rows);
+  L.tiles_m = ceil_div(L.par ? L.par_m : p.M, BM);
   L.tiles_n = ceil_div(p.N, L.bn);
   L.total_tiles = (int)((int64_t)L.tiles_m * L.tiles_n * zbase * p.split_k);
-  const int stage_bytes = A_TILE_BYTES + (plan.pair ? L.bn / 2 : L.bn) * KC * 4;
-  L.stages = (227 * 1024 - EPI_STAGE_BYTES - 2048) / stage_bytes;
-  if (L.stages > (plan.pair ? 7 : 6)) L.stages = plan.pair ? 7 : 6;
-  if (ev.stages >= 2 && ev.stages <= L.stages) L.stages = ev.stages;
-  L.lag = L.stages - 1 < 2 ? L.stages - 1 : 2;
-  if (ev.lag >= 1 && ev.lag < L.stages && ev.lag <= 5) L.lag = ev.lag;
-  const int cap = plan.pair ? max_pairs<AK, BK, MASK>() : num_sms;
+  const int stage_bytes = A_TILE_BYTES + L.bn * KC * 4;
+  const int img_bytes = (is_mn(AK) ? A_TILE_BYTES : 0) + (is_mn(BK) ? L.bn * KC * 4 : 0);     // K-major images
+  L.stages = (227 * 1024 - EPI_STAGE_BYTES - img_bytes - 2048) / stage_bytes;
+  if (L.stages > 6) L.stages = 6;
+  if (ev.stages >= 3 && ev.stages <= L.stages) L.stages = ev.stages;
+  // The consumers release chunk c's stage after they have waited for chunk c + 1, and a cp.async producer publishes
+  // chunk c only after the free-stage wait of chunk c + lag - stages.  lag <= stages - 2 keeps that wait behind a
+  // release that does not depend on chunk c itself (no cycle); stages >= 3 always (the smem budget above gives >= 3).
+  L.lag = L.stages - 2 < 2 ? L.stages - 2 : 2;
+  if (ev.lag >= 1 && ev.lag <= L.stages - 2 && ev.lag <= 5) L.lag = ev.lag;
+  const int cap = num_sms;
   int units = L.total_tiles < cap ? L.total_tiles : cap;
 #ifdef VLFB_TRACE
   L.trace = g_trace_buf;
@@ -2119,34 +1936,25 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       L.ws_tiles = reinterpret_cast<float*>(reinterpret_cast<char*>(p.workspace) + (size_t)SK_CNT_INTS * 4);
     }
   }
-  const int smem = L.stages * stage_bytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  const int smem = L.stages * stage_bytes + img_bytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
   const bool cp = !(L.tma_a && L.tma_b);
   if (ev.debug)
-    fprintf(stderr, "vlfb gemm_tc: kinds %d,%d M=%d N=%d K=%d z=%d | bn=%d pair=%d sk=%d split=%d tiles=%d units=%d stages=%d tma=%d,%d cap=%d patch=%d par=%d\n",
-            AK, BK, p.M, p.N, p.K, zbase, L.bn, plan.pair, L.sk, p.split_k, L.total_tiles, units, L.stages, L.tma_a, L.tma_b, cap, L.stem_patch, L.par);
+    fprintf(stderr, "vlfb gemm_tc: kinds %d,%d M=%d N=%d K=%d z=%d | bn=%d sk=%d split=%d tiles=%d units=%d stages=%d tma=%d,%d cap=%d patch=%d par=%d\n",
+            AK, BK, p.M, p.N, p.K, zbase, L.bn, L.sk, p.split_k, L.total_tiles, units, L.stages, L.tma_a, L.tma_b, cap, L.stem_patch, L.par);
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(plan.pair ? 2 * units : units));
-  cfg.blockDim = dim3((unsigned)((cp ? NPROD : 32 * NTMAW) + 32 + NEPI));
+  cfg.gridDim = dim3((unsigned)units);
+  cfg.blockDim = dim3((unsigned)((cp ? NPROD : NPROD_TMA) + NEPI));
   cfg.dynamicSmemBytes = (size_t)smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = plan.pair ? 1 : 0;
   // ReLU sign bits are emitted by the lean epilogue; any other path writes them in a second pass over the dense output
   const bool lean = !cp && (p.ldd & 3) == 0 && (p.N & 15) == 0 && span32_ok(p) && (reinterpret_cast<uintptr_t>(p.d) & 15) == 0 &&
                     (!p.residual || ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && !(p.flags & VLFB_EPI_ACCUM)));
   uint32_t* bits_after = nullptr;
   if (p.relu_bits_out && (!lean || MASK)) { bits_after = p.relu_bits_out; p.relu_bits_out = nullptr; }
   int rc = VLFB_OK;
-  bool done = false;
-  if constexpr (kind_pair_capable(AK) && kind_pair_capable(BK)) {
-    if (plan.pair) { rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB); done = true; }
-  }
-  if (done) {}
-  else if (!cp) rc = launch_variant<AK, BK, MASK, false, false>(cfg, p, L, tmA, tmB);
-  else rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
+  if (cp) rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);     // (fix-ups are planned for TMA-fed launches only)
+  else if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
+  else rc = launch_variant<AK, BK, MASK, false, false>(cfg, p, L, tmA, tmB);
   if (rc == VLFB_OK && bits_after) rc = relu_bits(p.d, bits_after, (int64_t)p.M * p.N, stream);
   return rc;
 }
@@ -2154,10 +1962,9 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
 }  // namespace tc
 
 void gemm_tc_plan(const vlfb_gemm_params_t& p, int num_sms, vlfb_gemm_plan_t* out) {
-  // host-only view of the plan: pairing assumes both operands are TMA-addressable and one pair per two SMs
-  const bool pair_ok = tc::kind_pair_capable(p.a.kind) && tc::kind_pair_capable(p.b.kind) && p.K >= tc::KC;
+  // host-only view of the plan
   bool sk_ws = p.workspace != nullptr && p.workspace_bytes >= tc::gemm_tc_workspace_bytes();
-  const tc::Plan pl = tc::make_plan(p, num_sms, num_sms / 2, pair_ok, sk_ws);
+  const tc::Plan pl = tc::make_plan(p, num_sms, sk_ws);
   out->tile_n = pl.bn; out->split_k = pl.split_k; out->pair = pl.pair; out->stream_k = pl.sk;
   out->tiles = pl.tiles; out->units = pl.units;
 }

@@ -1,7 +1,7 @@
 // Streaming (HBM-bound) kernels of the hot path: pooling, RoIAlign, softmax, LayerNorm,
 // elementwise, layout changes, losses, optimizer, fused FBO attention core.
 // All activations fp32 channels-last; 128-bit loads/stores wherever the channel extent allows;
-// grids are sized in multiples of the 148 SMs (common.cuh: stream_grid).
+// grids are sized in multiples of the 132 SMs (common.cuh: stream_grid).
 #include <float.h>
 
 #include "common.cuh"
@@ -516,7 +516,7 @@ __global__ void colsum_k(const float* __restrict__ x, int64_t ld, float* __restr
 // src [N][C][inner] <-> dst [N][inner][Cpad]; tiled 32x32 transposes through shared memory.
 // Clip feeding (C <= 4 planes -> 4-channel pixels): one thread converts 4 consecutive positions: C coalesced 16-byte
 // plane loads -> four 16-byte pixel stores (64 contiguous bytes per thread), optional TF32 rounding of the conv1 operand.
-// The generic 32x32 tile kernel below moves only 3 of its 32 tile rows for a clip (0.39 TB/s measured).
+// The generic 32x32 tile kernel below would move only 3 of its 32 tile rows for a clip.
 __global__ void nc_to_cl4_k(const float* __restrict__ src, float4* __restrict__ dst, int C, int64_t inner4,
                             int64_t total, int tf32) {
   for (int64_t q = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
@@ -630,7 +630,7 @@ __global__ void weight_transpose_k(const float* __restrict__ w, float* __restric
 __global__ void weight_transpose_multi_k(const vlfb_wt_job_t* __restrict__ jobs, int njobs) {
   __shared__ float tile[32][33];
   // block -> job: the table's block_begin column is fetched by ONE coalesced load into shared memory and searched
-  // there (the search over global memory was ~6 dependent L2 round trips per 4 KB tile: call J, 185 us for 238 MB)
+  // there (a search over global memory costs ~6 dependent L2 round trips per 4 KB tile)
   __shared__ int begins[256];
   const int tid = threadIdx.y * 32 + threadIdx.x;
   const bool in_smem = njobs <= 256;
@@ -956,7 +956,7 @@ int vlfb_colsum(const float* x, int64_t ld, float* out, int64_t rows, int cols, 
   }
   if (rows == 0) return VLFB_OK;
   const int cb = ceil_div(cols, 32);
-  int slabs = (int)((2 * 148 + cb - 1) / cb);                 // ~2 waves of blocks on 148 SMs
+  int slabs = (int)((2 * 132 + cb - 1) / cb);                 // ~2 waves of blocks on 132 SMs
   const int64_t max_slabs = (rows + 63) / 64;
   if (slabs > max_slabs) slabs = (int)max_slabs;
   if (slabs < 1) slabs = 1;

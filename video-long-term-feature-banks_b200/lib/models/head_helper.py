@@ -1,4 +1,4 @@
-"""Output heads (B200 re-implementation of the reference's lib/models/head_helper.py).
+"""Output heads (CUDA re-implementation of the reference's lib/models/head_helper.py).
 
 `add_roi_head` (AVA, box-level; reference :61-85 with `roi_pool` :88-123): temporal average
 pool -> Squeeze -> legacy RoIAlign 7x7 -> 7x7 max pool -> `box_pooled` (R, 2048, 1, 1, 1),

@@ -1,4 +1,4 @@
-"""Feature-bank operators (B200 re-implementation of the reference's lib/models/lfb_helper.py).
+"""Feature-bank operators (CUDA re-implementation of the reference's lib/models/lfb_helper.py).
 
 FBO-NL (`add_fbo_nl_head`, reference :78-103): the RoI / clip feature A attends over the L
 long-term bank features B with `FBO_NL.NUM_LAYERS` stacked single-query non-local layers

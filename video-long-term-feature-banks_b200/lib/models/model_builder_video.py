@@ -1,9 +1,9 @@
-"""Model builder abstraction (B200 re-implementation of the reference's
+"""Model builder abstraction (CUDA re-implementation of the reference's
 lib/models/model_builder_video.py).
 
 `ModelBuilder` keeps the reference's constructor kwargs, methods and attributes (:66-314) but
 derives from vlfb.cnn.CNNModelHelper, so the builder functions record a net that vlfb.executor
-lowers onto sm_100a kernels.  The data loader side (`get_input_db` / `DataLoader`, :98-117) is
+lowers onto sm_90a kernels.  The data loader side (`get_input_db` / `DataLoader`, :98-117) is
 out of scope: inputs are fed with workspace.FeedBlob under the reference's blob names.
 """
 import logging

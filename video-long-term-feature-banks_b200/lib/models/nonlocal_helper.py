@@ -1,4 +1,4 @@
-"""Space-time non-local block (B200 re-implementation of the reference's
+"""Space-time non-local block (CUDA re-implementation of the reference's
 lib/models/nonlocal_helper.py; arXiv:1711.07971).
 
 `spacetime_nonlocal` (reference :29-160) records theta/phi/g 1x1x1 convs, the 1x2x2 max pool

@@ -1,9 +1,9 @@
-"""Residual stages (B200 re-implementation of the reference's lib/models/resnet_helper.py).
+"""Residual stages (CUDA re-implementation of the reference's lib/models/resnet_helper.py).
 
 Signatures, blob names and semantics follow the reference (bottleneck :35-72, shortcut :75-89,
 residual block :92-119, stages :122-194): temporal conv in branch2a, stride/dilation on the
 1x3x3 branch2b, in-place Sum + ReLU into `{prefix}_branch2c_bn`.  vlfb.executor fuses each
-conv -> affine -> (sum) -> relu chain into a single tcgen05 GEMM epilogue.
+conv -> affine -> (sum) -> relu chain into a single tensor-core GEMM epilogue.
 """
 import logging
 

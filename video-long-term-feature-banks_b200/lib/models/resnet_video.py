@@ -1,11 +1,11 @@
-"""Full-model builder (B200 re-implementation of the reference's lib/models/resnet_video.py).
+"""Full-model builder (CUDA re-implementation of the reference's lib/models/resnet_video.py).
 
 Same public surface -- `obtain_arc(arc_type)`, `create_model(model, data, labels, split,
 lfb_infer_only, suffix='')`, `BLOCK_CONFIG` -- same blob names and YAML keys, so the graph a
 driver obtains is the one the reference builds (stem conv1 5x7x7 -> pool1 -> res2 -> pool2 ->
 res3(+grouped NL) -> res4(+NL) -> res5(dilated) -> head -> dropout -> pred -> loss; reference
 lib/models/resnet_video.py:133-351).  The ops are recorded on a vlfb model helper and later
-lowered onto fused sm_100a kernels by vlfb.executor.
+lowered onto fused sm_90a kernels by vlfb.executor.
 """
 import logging
 

@@ -1,4 +1,4 @@
-"""Precise batch-norm statistics (B200 re-implementation of the reference's lib/utils/bn_helper.py:60-221).
+"""Precise batch-norm statistics (CUDA re-implementation of the reference's lib/utils/bn_helper.py:60-221).
 
 Before testing / checkpointing a SpatialBN model (`MODEL.USE_AFFINE False`), the running statistics kept by the
 momentum update are replaced by the exact population statistics of `TRAIN.ITER_COMPUTE_PRECISE_BN` training batches:

@@ -1,7 +1,7 @@
 """CNNModelHelper stand-in: the op-emitter object the reference's builders call
 (`model.ConvNd`, `model.MaxPool`, `model.net.Sum`, ... -- the list is in SURVEY.md
 section 8b).  Emitters only RECORD ops and parameter initialisers; the executor
-(vlfb/executor.py) lowers the recorded net onto the B200 kernels.
+(vlfb/executor.py) lowers the recorded net onto the sm_90a kernels.
 
 Argument conventions follow the Caffe2 python helpers at the reference's call sites
 (e.g. lib/models/resnet_video.py:169-179 for ConvNd, :190-196 for MaxPool).

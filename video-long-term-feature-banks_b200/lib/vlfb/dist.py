@@ -32,8 +32,8 @@ def init_from_env(backend=None):
 def shutdown(timeout_s=20.0):
     """Leave the process group.  The captured training step holds NCCL kernels (overlapped all-reduce inside the graph) and
     ncclCommDestroy waits for every CUDA graph that captured the communicator: the graphs are released first (the nets of
-    the workspace are dropped), and the teardown runs under a watchdog -- call N: `bench.py --gpus 2` printed its line and
-    then sat in destroy_process_group() until the driver's timeout.  Returns False if the teardown had to be abandoned."""
+    the workspace are dropped), and the teardown runs under a watchdog, so that a benchmark that has printed its line
+    never sits in destroy_process_group().  Returns False if the teardown had to be abandoned."""
     if not dist.is_initialized():
         return True
     import gc

@@ -1,4 +1,4 @@
-"""Lowers a recorded net (vlfb.net.Net) onto the B200 kernels and runs forward / backward /
+"""Lowers a recorded net (vlfb.net.Net) onto the sm_90a kernels and runs forward / backward /
 optimizer.  Replaces the Caffe2 `dag` executor behind `workspace.RunNet`
 (reference tools/train_net.py:152) for the hot path.
 
@@ -27,10 +27,8 @@ DTYPE = torch.float32      # the CUDA kernels are fp32-only; the CPU test stand-
 STATS = {'fused_grad_finish': 0}
 LAZY_GRAD_SUM = os.environ.get('VLFB_LAZY_GRAD_SUM', '1') != '0'   # defer residual + dgrad sums into the consumer's mask/round pass
 # Fold the ReLU backward + TF32 rounding of a conv's incoming gradient (and the sum of its earlier contributions)
-# into the epilogue of the dgrad GEMM that delivers the last contribution.  Exact (tests run both ways).  Round 1
-# measured it 2-3% SLOWER (the 96-register epilogue spilled on the extra operand streams); with the 10-warp TMA-only
-# builds and the lean epilogue of round 2 (mask + residual prefetched into registers) it is 1% faster and removes 44
-# streaming launches per step (13.58 vs 13.72 ms, profiles/r02_perf_log.md): ON by default, VLFB_FUSE_GRAD_FINISH=0 disables.
+# into the epilogue of the dgrad GEMM that delivers the last contribution.  Exact (tests run both ways); removes 44
+# streaming launches per step.  ON by default, VLFB_FUSE_GRAD_FINISH=0 disables.
 FUSE_GRAD_FINISH = os.environ.get('VLFB_FUSE_GRAD_FINISH', '1') == '1'
 # ... with the mask read as sign bits written by the producing conv's epilogue instead of the fp32 activation
 RELU_BITS = os.environ.get('VLFB_RELU_BITS', '1') == '1'
@@ -1263,7 +1261,7 @@ class CompiledNet(object):
             else:
                 cls = STEP_TYPES.get(op.type)
                 if cls is None:
-                    raise NotImplementedError('op type %s has no B200 lowering' % op.type)
+                    raise NotImplementedError('op type %s has no GPU lowering' % op.type)
                 steps.append(cls(op, self.in_keys[i], self.out_keys[i]))
         return steps
 

@@ -10,7 +10,7 @@ import torch
 
 from . import libvlfb as L
 
-NUM_SMS = 148
+NUM_SMS = 132
 
 
 LAUNCHES = 0            # kernels launched through this module (bench.py reports it as gpu_launches)
@@ -79,7 +79,8 @@ _GEMM_WS = {}                                             # device index -> stre
 
 
 def set_gemm_backend(name):
-    """'tcgen05' (default) or 'simt' (debug cross-check engine)."""
+    """'tcgen05' (default: the tensor-core wgmma engine, csrc/gemm_tc.cu; the name is historical) or 'simt'
+    (debug cross-check engine)."""
     global _ENGINE
     _ENGINE = {'tcgen05': L.ENGINE_TCGEN05, 'simt': L.ENGINE_SIMT}[name]
 
@@ -318,7 +319,7 @@ def _mat_operand(t, rows_dim, k_dim):
     if t.shape[0] == 1:
         sb = 0
     k_ok, mn_ok = _dim_ok(sk, K), _dim_ok(sr, R)
-    k_al = (R == 1 or sr % 4 == 0) and K % 4 == 0 and sb % 4 == 0       # 16-byte addressable for tcgen05
+    k_al = (R == 1 or sr % 4 == 0) and K % 4 == 0 and sb % 4 == 0       # 16-byte addressable for the tensor-core engine
     mn_al = (K == 1 or sk % 4 == 0) and R % 4 == 0 and sb % 4 == 0
     if k_ok and (k_al or not (mn_ok and mn_al)):
         return L.OP_DENSE_K, (sr if R > 1 else K), sb
@@ -333,7 +334,7 @@ def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32
     Each matrix needs unit stride along one of its two dims (16-byte aligned rows).  Returns whether d was stored
     TF32-rounded: with `tf32_optional` a product that qualifies for split-K (atomic accumulation cannot round) keeps
     the split and leaves the rounding to the consumer -- the split is worth 2x on the K = 3136 non-local gradient
-    products, the saved rounding pass ~5 us (call J/K: 0.046 vs 0.022 ms per launch)."""
+    products."""
     assert a.dim() == 3 and b.dim() == 3 and d.dim() == 3
     Bt, M, K = a.shape
     N = b.shape[2]
@@ -356,7 +357,7 @@ def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32
         tf32_out = False
     if tiles <= NUM_SMS // 2 and K >= 1024 and not tf32_out:
         # few output tiles with a long reduction (the 4 x 80 x 2560 classifier ran 0.19 ms on ONE CTA; the non-local
-        # affinity products fill 28-56 of 148 SMs): split K over the SMs -- atomic accumulation into a zeroed / kept
+        # affinity products fill 28-56 of 132 SMs): split K over the SMs -- atomic accumulation into a zeroed / kept
         # D, bias from the first slice; the library picks the split together with the tile width
         if not accumulate:
             fill(d, 0.0) if d.is_contiguous() else d.zero_()
