@@ -83,7 +83,8 @@ enum { VLFB_EPI_RELU = 1, VLFB_EPI_ACCUM = 2, VLFB_EPI_ATOMIC = 4, VLFB_EPI_TF32
 typedef struct {
   vlfb_operand_t a, b;
   vlfb_conv_geom_t g;         /* used by the CONV_ / DGRAD_ / STEM_ kinds    */
-  int M, N, K;                /* logical GEMM extent (K per z-slice for wgrad) */
+  int M, N, K;                /* logical GEMM extent (K per z-slice for wgrad), all > 0: an empty sum (K = 0) is
+                               * rejected with VLFB_E_BADARG, not evaluated as D = epi(0) */
   int batch;                  /* >= 1 (DENSE only)                           */
   int taps;                   /* wgrad: number of temporal taps kT (z-slices), else 1 */
   int split_k;                /* >= 1 (>1 needs VLFB_EPI_ATOMIC); 0 = the library picks it with the tile width */

@@ -1,0 +1,736 @@
+"""Path matrix of the tensor-core GEMM (csrc/gemm_tc.cu): a table of seeded, self-describing cases, each ONE vlfb_gemm call
+whose result is checked elementwise against an fp64 PyTorch reference, and whose path record (the VLFB_DEBUG line of
+launch()) is compared with the path the case declares.
+
+The loader / schedule switches of the library (VLFB_TMA, VLFB_IM2COL, ...) are read once per process, so every
+configuration runs in its own process:
+
+    python tests/gemm_paths.py --config NAME --out FILE
+
+writes one JSON record per case that lists NAME among its configurations.  tests/test_gpu_gemm_paths.py drives it;
+tests/test_gemm_paths_cpu.py checks the table and the comparison itself without a GPU.
+
+Every output lives inside a NaN-filled buffer with a guard band (a lead-in, rows past M, ldd > N where the caller
+controls ldd, gaps between batches): after the call each in-range element must be finite and within the bound of
+`compare`, and every other element must still be the NaN it was filled with, bit for bit.
+"""
+import argparse
+import json
+import os
+import re
+import sys
+import tempfile
+
+import torch
+import torch.nn.functional as F
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+for _p in (os.path.join(ROOT, 'video-long-term-feature-banks_b200', 'lib'), HERE):
+    if _p not in sys.path:
+        sys.path.insert(0, _p)
+
+from util import tf32_round  # noqa: E402
+
+# Tolerance of the accumulation, relative to sum_k |A[m,k]| |B[n,k]| (the operands are TF32-exact, so every product
+# is exact and only the fp32 additions err).  The wgmma accumulator adds each k8 step to the running fp32 sum with at
+# most one ulp (2^-23, truncation allowed) of a partial sum bounded by sum |A||B|, so over ceil(K/8) steps plus the
+# in-MMA reduction the error is below (ceil(K/8) + 8) 2^-23 sum |A||B|.  tau(K) is that bound times TAU_SAFETY (the
+# split-K / stream-K partial sums add a few more roundings of the same size).  A missing 32-wide K chunk of a random
+# tile shifts an element by ~sqrt(32) times a typical |A||B| term, far above tau(K) sum |A||B| (test_gemm_paths_cpu.py
+# shows the check rejects it at the largest K of the table).
+TAU_SAFETY = 4.0
+KMAX = 16000                   # the table's K stays in the range the worker's fp64 references handle quickly
+
+
+def tau(K):
+    return TAU_SAFETY * (-(-K // 8) + 8) * 2.0 ** -23
+
+# the fp32 epilogue (scale, bias, residual, accumulate) rounds a few times: 2^-22 of the magnitudes it adds
+EPS32 = 2.0 ** -22
+NAN_BITS = 0x7FC00000          # torch.full(..., nan) fills this pattern
+GUARD = 64                     # lead-in guard floats (keeps d 16-byte aligned)
+
+CONFIGS = {
+    'default': {},
+    'tma0': {'VLFB_TMA': '0'},
+    'im2col0': {'VLFB_IM2COL': '0'},
+    'tmamn0': {'VLFB_TMA_MN': '0'},
+    'fuse0': {'VLFB_FUSE_ATOMS': '0'},
+    'nopatch': {'VLFB_NO_PATCH': '1'},
+    'nopar': {'VLFB_NO_PAR': '1'},
+}
+# every environment override of the GEMM (a configuration sets some of them; the rest must be unset)
+SWITCHES = ('VLFB_TMA', 'VLFB_IM2COL', 'VLFB_TMA_MN', 'VLFB_FUSE_ATOMS', 'VLFB_NO_PATCH', 'VLFB_NO_PAR', 'VLFB_BN',
+            'VLFB_STAGES', 'VLFB_LAG', 'VLFB_SK', 'VLFB_DEBUG')
+
+OP_DENSE_K, OP_DENSE_MN, OP_CONV_K, OP_DGRAD_K, OP_CONV_MN, OP_STEM_K, OP_STEM_MN = range(7)
+
+
+# ----------------------------------------------------------------------------------------------- path records
+def parse_record(line):
+    """One VLFB_DEBUG line of gemm_tc launch() -> dict (None if the line is not one).  Values are ints; 'kinds' and
+    'tma' are (a, b) tuples."""
+    m = re.search(r'vlfb gemm_tc:\s*(.*)$', line.strip())
+    if not m:
+        return None
+    rec = {}
+    for tok in m.group(1).split():
+        if '=' not in tok:
+            continue
+        k, v = tok.split('=', 1)
+        rec[k] = tuple(int(x) for x in v.split(',')) if ',' in v else int(v)
+    return rec
+
+
+def matches(rec, expect):
+    """Fields of `expect` that the record contradicts ([] = it took the declared path).  An expected value '>N'
+    means greater than N."""
+    bad = []
+    for k, want in expect.items():
+        got = rec.get(k)
+        if isinstance(want, str) and want.startswith('>'):
+            ok = got is not None and got > int(want[1:])
+        else:
+            ok = tuple(got) == tuple(want) if isinstance(want, (tuple, list)) else got == want
+        if not ok:
+            bad.append('%s=%r (declared %r)' % (k, got, want))
+    return bad
+
+
+# ----------------------------------------------------------------------------------------------- the case table
+def G(N, T, H, W, C, Co, ker, st=(1, 1, 1), pd=(0, 0, 0), dil=(1, 1, 1)):
+    return dict(N=N, T=T, H=H, W=W, C=C, Co=Co, ker=ker, st=st, pd=pd, dil=dil)
+
+
+def _case(name, op, seed, runs, **kw):
+    c = dict(name=name, op=op, seed=seed, runs=runs, opts=kw.pop('opts', {}))
+    c.update(kw)
+    return c
+
+
+# runs: configuration -> the path fields the case must take there (kinds / mask / tma / cp / bn / sk / fix / lean /
+# bits2 / patch / par / split as printed by VLFB_DEBUG).  Kinds: 0 DENSE_K, 1 DENSE_MN, 2 CONV_K, 3 DGRAD_K, 4 CONV_MN,
+# 5 STEM_K, 6 STEM_MN.  tma_a: 0 cp.async, 1 TMA tiled, 2 im2col, 3 stem, 4 fused MN atoms; tma_b adds 5 = conv_flat.
+CASES = []
+
+
+def _add(*a, **kw):
+    CASES.append(_case(*a, **kw))
+
+
+# ---- convolution forward (kernels.conv_fwd): CONV_K x DENSE_K
+_add('fwd_3x3_res_relu_bits', 'conv_fwd', 1, geom=G(2, 3, 9, 10, 32, 64, (1, 3, 3), pd=(0, 1, 1)),
+     epi=dict(scale=True, bias=True, residual=True, relu=True, bits=True),
+     runs={'default': dict(kinds=(2, 0), mask=0, tma=(2, 1), cp=0, lean=1, bits2=0),
+           'im2col0': dict(kinds=(2, 0), tma=(0, 1), cp=1, lean=0, bits2=1),
+           'tma0': dict(kinds=(2, 0), tma=(0, 0), cp=1, bits2=1)})
+_add('fwd_dilated_t96', 'conv_fwd', 2, geom=G(1, 2, 14, 14, 64, 112, (1, 3, 3), pd=(0, 2, 2), dil=(1, 2, 2)),
+     epi=dict(bias=True, tf32=True), opts=dict(tile_n=96),
+     runs={'default': dict(kinds=(2, 0), tma=(2, 1), cp=0, bn=96),
+           'im2col0': dict(kinds=(2, 0), tma=(0, 1), cp=1, bn=96)})
+_add('fwd_strided_t32_ntail', 'conv_fwd', 3, geom=G(2, 2, 14, 14, 32, 80, (1, 3, 3), st=(1, 2, 2), pd=(0, 1, 1)),
+     epi=dict(scale=True, relu=True), opts=dict(tile_n=32),
+     runs={'default': dict(kinds=(2, 0), tma=(2, 1), cp=0, bn=32),
+           'im2col0': dict(kinds=(2, 0), tma=(0, 1), cp=1, bn=32)})
+_add('fwd_temporal_t128', 'conv_fwd', 4, geom=G(1, 4, 7, 7, 256, 288, (3, 1, 1), pd=(1, 0, 0)),
+     epi=dict(bias=True), opts=dict(tile_n=128),
+     runs={'default': dict(kinds=(2, 0), tma=(2, 1), cp=0, bn=128),
+           'tma0': dict(kinds=(2, 0), tma=(0, 0), cp=1, bn=128)})
+# ---- conv1 stem forward (STEM_K x DENSE_K): patch tiles, TMA rows without patches, cp.async on a dense clip
+_add('stem_fwd_patch', 'conv_fwd', 5, geom=G(1, 4, 32, 32, 4, 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3)), pitched=True,
+     epi=dict(scale=True, bias=True, relu=True, bits=True),
+     runs={'default': dict(kinds=(5, 0), tma=(3, 1), patch=1, cp=0, lean=1, bits2=0),
+           'nopatch': dict(kinds=(5, 0), tma=(3, 1), patch=0, cp=0),
+           'tma0': dict(kinds=(5, 0), tma=(0, 0), patch=0, cp=1, bits2=1)})
+_add('stem_fwd_rows_ho18', 'conv_fwd', 6, geom=G(1, 4, 36, 64, 4, 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3)),
+     pitched=True, epi=dict(bias=True),
+     runs={'default': dict(kinds=(5, 0), tma=(3, 1), patch=0, cp=0)})
+_add('stem_fwd_dense_clip', 'conv_fwd', 7, geom=G(2, 3, 20, 20, 4, 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3)),
+     epi=dict(relu=True),
+     runs={'default': dict(kinds=(5, 0), tma=(0, 1), patch=0, cp=1)})
+# ---- convolution dgrad (kernels.conv_dgrad): DGRAD_K x DENSE_K, parity classes, strided gather, ReLU masks
+_add('dgrad_unit_accum', 'conv_dgrad', 8, geom=G(1, 3, 9, 10, 64, 32, (1, 3, 3), pd=(0, 1, 1)),
+     epi=dict(accum=True),
+     runs={'default': dict(kinds=(3, 0), mask=0, tma=(2, 1), cp=0, par=0),
+           'im2col0': dict(kinds=(3, 0), mask=0, tma=(0, 1), cp=1),
+           'tma0': dict(kinds=(3, 0), mask=0, tma=(0, 0), cp=1)})
+_add('dgrad_parity_bits_tf32', 'conv_dgrad', 9, geom=G(2, 2, 30, 30, 64, 128, (1, 3, 3), st=(1, 2, 2), pd=(0, 1, 1)),
+     epi=dict(residual=True, mask_bits=True, tf32=True),
+     runs={'default': dict(kinds=(3, 0), mask=1, tma=(2, 1), cp=0, par='>0'),
+           'nopar': dict(kinds=(3, 0), mask=1, tma=(0, 1), cp=1, par=0),
+           'im2col0': dict(kinds=(3, 0), mask=1, tma=(0, 1), cp=1, par=0)})
+_add('dgrad_parity_plain', 'conv_dgrad', 10, geom=G(3, 2, 20, 12, 128, 64, (1, 1, 1), st=(1, 2, 2)),
+     epi=dict(),
+     runs={'default': dict(kinds=(3, 0), mask=0, tma=(2, 1), cp=0, par='>0')})
+_add('dgrad_strided_gather', 'conv_dgrad', 11, geom=G(1, 2, 15, 15, 32, 64, (1, 3, 3), st=(1, 2, 2), pd=(0, 1, 1)),
+     epi=dict(residual=True),
+     runs={'default': dict(kinds=(3, 0), tma=(0, 1), cp=1, par=0)})
+_add('dgrad_pointwise_float_mask', 'conv_dgrad', 12, geom=G(2, 3, 6, 6, 64, 160, (1, 1, 1)),
+     epi=dict(residual=True, mask_float=True, tf32=True),
+     runs={'default': dict(kinds=(0, 0), mask=1, tma=(1, 1), cp=0, lean=1),
+           'tma0': dict(kinds=(0, 0), mask=1, tma=(0, 0), cp=1)})
+# ---- convolution wgrad (kernels.conv_wgrad): DENSE_MN x CONV_MN / STEM_MN, atomic, split or stream-K.  On sm_90a every
+# MN-major operand is staged by cp.async: the tensor maps of the MN-major TMA paths (make_tmap_mn / _mn4, the wgrad
+# im2col and conv_flat maps, the conv1 wgrad rows and patches) use CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, which the H100
+# driver does not encode, so launch() falls back to the gather loaders (UNREACHABLE_SM90 in test_gpu_gemm_paths.py).
+_add('wgrad_3x3', 'conv_wgrad', 13, geom=G(2, 3, 9, 10, 32, 64, (1, 3, 3), pd=(0, 1, 1)),
+     epi=dict(row_scale=True),
+     runs={'default': dict(kinds=(1, 4), tma=(0, 0), cp=1),
+           'tma0': dict(kinds=(1, 4), tma=(0, 0), cp=1)})
+_add('wgrad_temporal_pointwise_taps', 'conv_wgrad', 14, geom=G(2, 4, 8, 8, 64, 64, (3, 1, 1), pd=(1, 0, 0)),
+     epi=dict(row_scale=True),
+     runs={'default': dict(kinds=(1, 4), tma=(0, 0), cp=1, z=3)})
+_add('wgrad_c36', 'conv_wgrad', 15, geom=G(1, 2, 6, 6, 36, 64, (1, 3, 3), pd=(0, 1, 1)),
+     epi=dict(),
+     runs={'default': dict(kinds=(1, 4), tma=(0, 0), cp=1)})
+_add('wgrad_stream_k_atomic', 'conv_wgrad', 16, geom=G(2, 8, 14, 14, 64, 64, (1, 3, 3), pd=(0, 1, 1)),
+     epi=dict(), opts=dict(stream_k=1),
+     runs={'default': dict(kinds=(1, 4), cp=1, sk=1, fix=0)})
+# conv1 wgrad 1x3x3 / stride (1, 2, 2) on a W-padded clip with Wo = 16 and Ho even: the only geometry whose N = 32 kH
+# fits one tile (the patch-chunk form needs it); the requested 96-wide tile is re-planned to 64 (pow2_only) because
+# the MN-major B operand falls back to cp.async
+_add('stem_wgrad_1x3x3_t128', 'conv_wgrad', 17, geom=G(1, 2, 32, 32, 4, 64, (1, 3, 3), st=(1, 2, 2), pd=(0, 1, 1)),
+     pitched=True, epi=dict(row_scale=True), opts=dict(tile_n=128),
+     runs={'default': dict(kinds=(1, 6), tma=(0, 0), patch=0, cp=1, bn=128),
+           'nopatch': dict(kinds=(1, 6), tma=(0, 0), patch=0, cp=1, bn=128)})
+_add('stem_wgrad_1x3x3_t96', 'conv_wgrad', 18, geom=G(1, 2, 32, 32, 4, 64, (1, 3, 3), st=(1, 2, 2), pd=(0, 1, 1)),
+     pitched=True, epi=dict(), opts=dict(tile_n=96),
+     runs={'default': dict(kinds=(1, 6), tma=(0, 0), patch=0, cp=1, bn=64)})
+_add('stem_wgrad_7x7', 'conv_wgrad', 19, geom=G(1, 4, 36, 64, 4, 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3)),
+     pitched=True, epi=dict(),
+     runs={'default': dict(kinds=(1, 6), tma=(0, 0), patch=0, cp=1)})
+_add('stem_wgrad_dense_clip', 'conv_wgrad', 20, geom=G(2, 3, 20, 20, 4, 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3)),
+     epi=dict(),
+     runs={'default': dict(kinds=(1, 6), tma=(0, 0), cp=1)})
+# ---- dense GEMMs through kernels.matmul
+# the Charades classifier: 4 x 157 x 2048, B = the transposed view of a contiguous [157, 2048] weight (K-major), split-K
+# atomic into an output whose ldd (159) and N are not multiples of 4: the scalar epilogue of run_blocks
+_add('fc_157_split_scalar', 'matmul', 21, Z=1, M=4, N=157, K=2048, a_mn=False, b_mn=False, b_weight=True, lib_split=True,
+     gn=2, epi=dict(bias=True),
+     runs={'default': dict(kinds=(0, 0), tma=(0, 1), cp=1, split='>1', sk=0, lean=0)})      # 4 rows: no 128-row TMA box
+_add('mm_stream_k_fix_general', 'matmul', 22, Z=1, M=1000, N=200, K=1024, a_mn=False, b_mn=False, gn=4,
+     epi=dict(tf32=True), opts=dict(stream_k=1),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, sk=1, fix=1, lean=0),
+           'tma0': dict(kinds=(0, 0), tma=(0, 0), cp=1, sk=0, fix=0)})
+# ---- dense GEMMs with every field set directly (vlfb_gemm_params_t)
+_add('raw_kk_t32_tails', 'raw', 23, Z=2, M=129, N=100, K=300, a_mn=False, b_mn=False, gn=3, gm=5,
+     epi=dict(alpha=0.5, bias=True), opts=dict(tile_n=32),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, bn=32),
+           'tma0': dict(kinds=(0, 0), tma=(0, 0), cp=1, bn=32)})
+_add('raw_kmn_t96', 'raw', 24, Z=1, M=192, N=160, K=256, a_mn=False, b_mn=True, gn=4, gm=3,
+     epi=dict(scale=True, bias=True, relu=True), opts=dict(tile_n=96),
+     runs={'default': dict(kinds=(0, 1), tma=(1, 0), cp=1, bn=64),          # pow2_only re-plan: MN-major cp.async
+           'tmamn0': dict(kinds=(0, 1), tma=(1, 0), cp=1, bn=64)})
+_add('raw_mnk_t64_k32', 'raw', 25, Z=3, M=236, N=72, K=32, a_mn=True, b_mn=False, gn=4, gm=2,
+     epi=dict(bias=True, residual=True), opts=dict(tile_n=64),
+     runs={'default': dict(kinds=(1, 0), tma=(0, 1), cp=1, bn=64),
+           'tmamn0': dict(kinds=(1, 0), tma=(0, 1), cp=1, bn=64)})
+_add('raw_mnmn_t128_accum', 'raw', 26, Z=2, M=256, N=200, K=200, a_mn=True, b_mn=True, gn=4, gm=1,
+     epi=dict(accum=True), opts=dict(tile_n=128),
+     runs={'default': dict(kinds=(1, 1), tma=(0, 0), cp=1, bn=128),
+           'fuse0': dict(kinds=(1, 1), tma=(0, 0), cp=1, bn=128)})
+_add('raw_k16_big_bias', 'raw', 27, Z=1, M=127, N=48, K=16, a_mn=False, b_mn=False, gn=4, gm=1,
+     epi=dict(bias=True, bias_scale=64.0),
+     runs={'default': dict(kinds=(0, 0), tma=(0, 0), cp=1)})
+_add('raw_split3_row_scale', 'raw', 28, Z=1, M=300, N=96, K=1000, a_mn=False, b_mn=False, gn=4, gm=2, split_k=3,
+     epi=dict(atomic=True, scale=True, bias=True, row_scale=True),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, split=3, sk=0),
+           'tma0': dict(kinds=(0, 0), tma=(0, 0), cp=1, split=3, sk=0)})
+_add('raw_accum_residual_tf32', 'raw', 29, Z=1, M=130, N=64, K=96, a_mn=False, b_mn=False, gn=4, gm=2,
+     epi=dict(accum=True, residual=True, relu=True, tf32=True),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, lean=0)})
+_add('raw_float_mask', 'raw', 30, Z=1, M=200, N=64, K=128, a_mn=False, b_mn=False, gn=4, gm=2,
+     epi=dict(mask_float=True, bias=True),
+     runs={'default': dict(kinds=(0, 0), mask=1, tma=(1, 1), cp=0),
+           'tma0': dict(kinds=(0, 0), mask=1, tma=(0, 0), cp=1)})
+_add('raw_stream_k_fix_lean', 'raw', 31, Z=1, M=1000, N=256, K=1024, a_mn=False, b_mn=False, gn=4, gm=2,
+     epi=dict(bias=True, relu=True), opts=dict(stream_k=1),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, sk=1, fix=1, lean=1)})
+_add('raw_stream_k_fix_accum', 'raw', 32, Z=1, M=1000, N=256, K=1024, a_mn=False, b_mn=False, gn=4, gm=2,
+     epi=dict(accum=True), opts=dict(stream_k=1),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, sk=1, fix=1, lean=1)})
+
+_add('raw_stream_k_atomic', 'raw', 33, Z=1, M=1000, N=256, K=1024, a_mn=False, b_mn=False, gn=4, gm=2, split_k=0,
+     epi=dict(atomic=True, bias=True), opts=dict(stream_k=1),
+     runs={'default': dict(kinds=(0, 0), tma=(1, 1), cp=0, sk=1, fix=0),
+           'tma0': dict(kinds=(0, 0), tma=(0, 0), cp=1, sk=1, fix=0)})
+
+def case_by_name(name):
+    return next(c for c in CASES if c['name'] == name)
+
+
+# ----------------------------------------------------------------------------------------------- GEMM view of a case
+def out_dims(g):
+    To = (g['T'] + 2 * g['pd'][0] - g['dil'][0] * (g['ker'][0] - 1) - 1) // g['st'][0] + 1
+    Ho = (g['H'] + 2 * g['pd'][1] - g['dil'][1] * (g['ker'][1] - 1) - 1) // g['st'][1] + 1
+    Wo = (g['W'] + 2 * g['pd'][2] - g['dil'][2] * (g['ker'][2] - 1) - 1) // g['st'][2] + 1
+    return To, Ho, Wo
+
+
+def _pointwise(g):
+    return tuple(g['ker']) == (1, 1, 1) and tuple(g['st']) == (1, 1, 1) and tuple(g['pd']) == (0, 0, 0)
+
+
+def describe(c):
+    """The vlfb_gemm call a case makes, as (kinds, M, N, K, batch, taps, flags): what kernels.py builds for the conv /
+    matmul wrappers and what _run_raw sets.  The GPU worker checks the launch's record against it."""
+    e = c.get('epi', {})
+    if c['op'] in ('matmul', 'raw'):
+        # lib_split: kernels.matmul itself picks split-K with atomic accumulation (few tiles, long K) and zero-fills d
+        flags = dict(accum=bool(e.get('accum')), atomic=bool(e.get('atomic') or c.get('lib_split')),
+                     residual=bool(e.get('residual')), relu=bool(e.get('relu')), tf32=bool(e.get('tf32')),
+                     mask=bool(e.get('mask_float')), split_k=0 if c.get('lib_split') else c.get('split_k', 1))
+        return dict(kinds=(OP_DENSE_MN if c['a_mn'] else OP_DENSE_K, OP_DENSE_MN if c['b_mn'] else OP_DENSE_K),
+                    M=c['M'], N=c['N'], K=c['K'], batch=c['Z'], taps=1, flags=flags)
+    g = c['geom']
+    To, Ho, Wo = out_dims(g)
+    kT, kH, kW = g['ker']
+    stem = g['C'] == 4
+    flags = dict(accum=bool(e.get('accum')), atomic=c['op'] == 'conv_wgrad', residual=bool(e.get('residual')),
+                 relu=bool(e.get('relu')), tf32=bool(e.get('tf32')),
+                 mask=bool(e.get('mask_float') or e.get('mask_bits')), split_k=0 if c['op'] == 'conv_wgrad' else 1)
+    if c['op'] == 'conv_fwd':
+        ak = OP_STEM_K if stem else (OP_DENSE_K if _pointwise(g) else OP_CONV_K)
+        K = kT * kH * 32 if stem else kT * kH * kW * g['C']
+        return dict(kinds=(ak, OP_DENSE_K), M=g['N'] * To * Ho * Wo, N=g['Co'], K=K, batch=1, taps=1, flags=flags)
+    if c['op'] == 'conv_dgrad':
+        ak = OP_DENSE_K if _pointwise(g) else OP_DGRAD_K
+        return dict(kinds=(ak, OP_DENSE_K), M=g['N'] * g['T'] * g['H'] * g['W'], N=g['C'], K=kT * kH * kW * g['Co'],
+                    batch=1, taps=1, flags=flags)
+    bk = OP_STEM_MN if stem else (OP_DENSE_MN if _pointwise(g) else OP_CONV_MN)
+    n = kH * 32 if stem else (g['C'] if _pointwise(g) else kH * kW * g['C'])
+    return dict(kinds=(OP_DENSE_MN, bk), M=g['Co'], N=n, K=g['N'] * To * Ho * Wo, batch=1,
+                taps=1 if _pointwise(g) else kT, flags=flags)
+
+
+# ----------------------------------------------------------------------------------------------- comparison
+def ulp_tf32(x):
+    """One TF32 ulp (10 explicit mantissa bits) of |x|, elementwise; 0 at 0."""
+    m, e = torch.frexp(x.abs())
+    return torch.where(x == 0, torch.zeros_like(x), torch.ldexp(torch.ones_like(x), e - 11))
+
+
+def finish(acc, mag, epi, K):
+    """fp64 epilogue of vlfb_gemm (common.cuh epilogue_store, element by element) and the error bound of each element.
+    acc / mag: [Z, M, N] sum_k A B and sum_k |A| |B| over the call's K; epi: alpha, cs [N], cb [N], rs [M],
+    res / prev / keep [Z, M, N], relu, tf32.  Returns (ref, bound)."""
+    Z, M, N = acc.shape
+    one = torch.ones((), dtype=torch.float64, device=acc.device)
+    cs = epi.get('cs', one).view(1, 1, -1) if epi.get('cs') is not None else one
+    cb = epi.get('cb').view(1, 1, -1) if epi.get('cb') is not None else 0 * one
+    rs = epi.get('rs').view(1, -1, 1) if epi.get('rs') is not None else one
+    s = epi.get('alpha', 1.0) * cs * rs
+    v = acc * s + cb * rs
+    extra = (cb * rs).abs()
+    for k in ('res', 'prev'):
+        if epi.get(k) is not None:
+            v = v + epi[k]
+            extra = extra + epi[k].abs()
+    if epi.get('relu'):
+        v = v.clamp(min=0)
+    if epi.get('keep') is not None:
+        v = torch.where(epi['keep'], v, torch.zeros_like(v))
+    bound = tau(K) * s.abs() * mag + EPS32 * (s.abs() * mag + extra)
+    if epi.get('tf32'):
+        bound = bound + ulp_tf32(v)
+    return v, bound.expand_as(v)
+
+
+def compare(d, ref, bound):
+    """Elementwise check: d finite and |d - ref| <= bound everywhere; plus the suite's global max|d-ref| / max|ref| <
+    2e-5 (looser where the result is stored TF32-rounded).  Returns a dict: ok, worst ratio |d-ref|/bound, where, and
+    the global relative error."""
+    d = d.double()
+    diff = (d - ref).abs()
+    finite = torch.isfinite(d)
+    ratio = torch.where(finite, diff / bound.clamp(min=1e-300), torch.full_like(diff, float('inf')))
+    ratio = torch.where(diff == 0, torch.zeros_like(ratio), ratio)
+    worst = int(ratio.reshape(-1).argmax())
+    rel = float(diff[finite].max() / (ref.abs().max() + 1e-30)) if bool(finite.any()) else float('inf')
+    nbad = int((ratio > 1).sum())
+    at = [int(i) for i in torch.unravel_index(torch.tensor(worst), tuple(ref.shape))]
+    return dict(ok=nbad == 0 and bool(finite.all()), nbad=nbad, nonfinite=int((~finite).sum()),
+                worst_ratio=float(ratio.reshape(-1)[worst]), worst_at=at, rel_err=rel)
+
+
+def guard_intact(buf, index):
+    """Every element of the fp32 buffer `buf` outside the flat offsets `index` still holds the NaN fill, bit for bit.
+    Returns the number of touched guard elements."""
+    bits = buf.reshape(-1).view(torch.int32)
+    guard = torch.ones(bits.numel(), dtype=torch.bool, device=buf.device)
+    guard[index.reshape(-1)] = False
+    return int((bits[guard] != NAN_BITS).sum())
+
+
+def pack_sign_bits(x):
+    """bit e & 31 of word e >> 5 = x.flat[e] > 0 (vlfb_gemm_params_t.relu_bits_out / relu_mask_bits)."""
+    b = (x.reshape(-1, 32) > 0).to(torch.int64)
+    v = (b << torch.arange(32, dtype=torch.int64, device=x.device)).sum(1)
+    return torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32)
+
+
+# ----------------------------------------------------------------------------------------------- case inputs / references
+def rnd(shape, gen, scale=1.0):
+    return tf32_round(torch.randn(shape, generator=gen) * scale)
+
+
+def _to_cl(x):
+    return x.permute(0, 2, 3, 4, 1).contiguous()
+
+
+def _stem_ext_input(x, g, To, Ho, Wo):
+    """conv1 as the library defines it: every K row spans 8 pixels x 4 channels, so the reference is a (kT, kH, 8)
+    convolution over the zero-padded clip, trimmed to the extents the To x Ho x Wo outputs read."""
+    kT, kH, _ = g['ker']
+    (sT, sH, sW), (pT, pH, pW) = g['st'], g['pd']
+    nt, nh, nw = (To - 1) * sT + kT, (Ho - 1) * sH + kH, (Wo - 1) * sW + 8
+    xp = F.pad(x, (pW, max(0, nw - pW - g['W']), pH, max(0, nh - pH - g['H']), pT, max(0, nt - pT - g['T'])))
+    return xp[:, :, :nt, :nh, :nw]
+
+
+def conv_refs(c, x, w, dy, dev):
+    """fp64 (acc, mag) of the case's convolution GEMM in its output layout [Z, M, N] (independent of libvlfb): x NCTHW,
+    w [Co, C, kT, kH, kW] (stem: [Co, 4, kT, kH, 8]), dy [N, Co, To, Ho, Wo]."""
+    g = c['geom']
+    To, Ho, Wo = out_dims(g)
+    stem = g['C'] == 4
+    x, w, dy = x.to(dev).double(), w.to(dev).double(), dy.to(dev).double()
+    res = []
+    for sgn in (False, True):
+        xs, ws, dys = (x.abs(), w.abs(), dy.abs()) if sgn else (x, w, dy)
+        if stem:                                                     # (no conv1 dgrad: the clip needs no gradient)
+            xi = _stem_ext_input(xs, g, To, Ho, Wo)
+            wi = ws.clone().requires_grad_(True)
+            y = F.conv3d(xi, wi, None, g['st'])
+        else:
+            xi = xs.clone().requires_grad_(True)
+            wi = ws.clone().requires_grad_(True)
+            y = F.conv3d(xi, wi, None, g['st'], g['pd'], g['dil'])
+        if c['op'] == 'conv_fwd':
+            r = y.detach().permute(0, 2, 3, 4, 1).reshape(1, -1, g['Co'])
+        elif c['op'] == 'conv_dgrad':
+            y.backward(dys)
+            r = xi.grad.permute(0, 2, 3, 4, 1).reshape(1, -1, g['C'])
+        else:
+            y.backward(dys)
+            kT = g['ker'][0]
+            r = wi.grad.permute(2, 0, 3, 4, 1)                       # [kT, Co, kH, kW(8), C]
+            r = r.reshape(kT, g['Co'], -1)
+        res.append(r.detach())
+    return res[0], res[1]
+
+
+class Prepared:
+    """Inputs, output buffers, the call and the fp64 reference of one case."""
+
+
+def prepare(c, dev):
+    """Build the case on `dev` (the kernel call needs CUDA; the reference and bound work on any device)."""
+    gen = torch.Generator().manual_seed(1000 + c['seed'])
+    P = Prepared()
+    P.case = c
+    e = c.get('epi', {})
+    if c['op'] in ('matmul', 'raw'):
+        Z, M, N, K = c['Z'], c['M'], c['N'], c['K']
+        A = rnd((Z, M, K), gen)
+        B = rnd((Z, N, K), gen)
+        P.A, P.B = A, B
+        acc = torch.bmm(A.double(), B.double().transpose(1, 2))
+        mag = torch.bmm(A.double().abs(), B.double().abs().transpose(1, 2))
+        gm, gn = c.get('gm', 0), c.get('gn', 0)
+        ldd = N + gn
+        dbs = (M + gm) * ldd + (8 if Z > 1 else 0)              # a gap between batches
+        size = GUARD + Z * dbs + gm * ldd + 64
+        zz, mm, nn = torch.meshgrid(torch.arange(Z), torch.arange(M), torch.arange(N), indexing='ij')
+        P.index = GUARD + zz * dbs + mm * ldd + nn
+        P.layout = dict(ldd=ldd, dbs=dbs if Z > 1 else 0, size=size)
+    else:
+        g = c['geom']
+        To, Ho, Wo = out_dims(g)
+        kT, kH, kW = g['ker']
+        stem = g['C'] == 4
+        Ci = 3 if stem else g['C']
+        x = rnd((g['N'], Ci, g['T'], g['H'], g['W']), gen)
+        if stem:
+            x = torch.cat([x, torch.zeros_like(x[:, :1])], 1)           # the fourth (pad) channel is zero
+            w = torch.zeros((g['Co'], 4, kT, kH, 8))
+            w[:, :3, :, :, :kW] = rnd((g['Co'], 3, kT, kH, kW), gen, 0.1)
+        else:
+            w = rnd((g['Co'], g['C'], kT, kH, kW), gen, 0.1)
+        dy = rnd((g['N'], g['Co'], To, Ho, Wo), gen)
+        P.x, P.w, P.dy = x, w, dy
+        acc, mag = conv_refs(c, x, w, dy, dev)
+        Z, M, N = acc.shape
+        P.layout = dict(size=GUARD + Z * M * N + 96)
+        P.index = GUARD + torch.arange(Z * M * N).view(Z, M, N)
+        if c['op'] == 'conv_wgrad':                                     # dw [Co][kT][n]: tap z at column z * n
+            zz, mm, nn = torch.meshgrid(torch.arange(Z), torch.arange(M), torch.arange(N), indexing='ij')
+            P.index = GUARD + mm * (Z * N) + zz * N + nn
+    Z, M, N = acc.shape
+    epi = dict(alpha=e.get('alpha', 1.0), relu=e.get('relu', False), tf32=e.get('tf32', False))
+    if e.get('scale'):
+        epi['cs'] = (torch.rand(N, generator=gen) + 0.5).double()
+    if e.get('bias'):
+        epi['cb'] = (torch.randn(N, generator=gen) * e.get('bias_scale', 1.0)).double()
+    if e.get('row_scale'):
+        epi['rs'] = (torch.rand(M, generator=gen) + 0.5).double()
+    if e.get('residual'):
+        epi['res'] = torch.randn((Z, M, N), generator=gen).double()
+    if e.get('accum') or e.get('atomic') or c['op'] == 'conv_wgrad':
+        # calls that add to d (ACCUM, atomic split / stream-K, the wgrad): d starts at prev; every other output starts
+        # as the NaN fill, so an element the kernel never writes stays NaN
+        epi['prev'] = torch.randn((Z, M, N), generator=gen).double()
+    if e.get('mask_float') or e.get('mask_bits'):
+        epi['maskv'] = torch.randn((Z, M, N), generator=gen)
+        epi['keep'] = epi['maskv'] > 0
+    P.epi = dict((k, (v.to(dev) if torch.is_tensor(v) else v)) for k, v in epi.items())
+    P.acc, P.mag = acc.to(dev), mag.to(dev)
+    P.K = describe(c)['K']
+    P.ref, P.bound = finish(P.acc, P.mag, P.epi, P.K)
+    P.index = P.index.to(dev)
+    return P
+
+
+# ----------------------------------------------------------------------------------------------- running a case (GPU)
+def _opts(K, c):
+    K.GEMM_OPTS.update(dict(tile_n=0, pair=0, stream_k=0))
+    K.GEMM_OPTS.update(c.get('opts', {}))
+
+
+def _stem_input(K, P, dev):
+    """[N,T,H,W,4] conv1 operand: dense, or a view of a W-padded zero buffer (the TMA stem path)."""
+    c = P.case
+    g = c['geom']
+    x_cl = _to_cl(P.x).to(dev)
+    if not c.get('pitched'):
+        return x_cl
+    pW = g['pd'][2]
+    To, Ho, Wo = out_dims(g)
+    pitch = max(pW + g['W'], (Wo - 1) * g['st'][2] + 8)
+    pitch = (pitch + 3) // 4 * 4
+    buf = torch.zeros((g['N'], g['T'], g['H'], pitch, 4), device=dev)
+    buf[:, :, :, pW:pW + g['W'], :] = x_cl
+    return buf[:, :, :, pW:pW + g['W'], :]
+
+
+def run_case(K, P, dev):
+    """Runs the case's one vlfb_gemm call; returns (buffer, bits or None, bits guard info)."""
+    from vlfb import libvlfb as L
+    import ctypes
+    c = P.case
+    e = c.get('epi', {})
+    Z, M, N = P.ref.shape
+    buf = torch.full((P.layout['size'],), float('nan'), device=dev)
+    flat = buf.view(-1)
+    if 'prev' in P.epi:
+        flat[P.index.reshape(-1)] = P.epi['prev'].reshape(-1).float()
+    cs = P.epi['cs'].float() if 'cs' in P.epi else None
+    cb = P.epi['cb'].float() if 'cb' in P.epi else None
+    rs = P.epi['rs'].float() if 'rs' in P.epi else None
+    bits = None
+    _opts(K, c)
+    try:
+        if c['op'] in ('conv_fwd', 'conv_dgrad', 'conv_wgrad'):
+            g = c['geom']
+            geo = K.conv_geom((g['N'], g['T'], g['H'], g['W'], g['C']), g['Co'], g['ker'], g['st'], g['pd'], g['dil'])
+            n_out = Z * M * N
+            out = flat[GUARD:GUARD + n_out]
+            res = None
+            if 'res' in P.epi:
+                rbuf = torch.zeros_like(flat)
+                rbuf[P.index.reshape(-1)] = P.epi['res'].reshape(-1).float()
+                res = rbuf[GUARD:GUARD + n_out]
+            if c['op'] == 'conv_fwd':
+                x = _stem_input(K, P, dev) if g['C'] == 4 else _to_cl(P.x).to(dev)
+                w = P.w.permute(0, 2, 3, 4, 1).contiguous().to(dev)      # [Co, kT, kH, kW(8), C]
+                y = out.view(K.out_shape(geo))
+                if e.get('bits'):
+                    bits = torch.full((n_out // 32 + 8,), 0x5A5A5A5A, dtype=torch.int32, device=dev)
+                K.conv_fwd(x, w, y, geo, scale=cs, bias=cb, residual=None if res is None else res.view(y.shape),
+                           relu=bool(e.get('relu')), tf32_out=bool(e.get('tf32')),
+                           relu_bits=None if bits is None else bits[:n_out // 32])
+            elif c['op'] == 'conv_dgrad':
+                taps = g['ker'][0] * g['ker'][1] * g['ker'][2]
+                w_cl = P.w.permute(0, 2, 3, 4, 1).contiguous().to(dev)
+                wt = torch.empty((g['C'], taps, g['Co']), device=dev)
+                K.weight_transpose(w_cl, wt)
+                dx = out.view(g['N'], g['T'], g['H'], g['W'], g['C'])
+                mask = mbits = None
+                if 'maskv' in P.epi:
+                    mv = P.epi['maskv'].reshape(dx.shape).float().contiguous()
+                    if e.get('mask_bits'):
+                        mbits = pack_sign_bits(mv)
+                    else:
+                        mask = mv
+                K.conv_dgrad(_to_cl(P.dy).to(dev), wt, dx, geo, accumulate=bool(e.get('accum')),
+                             residual=None if res is None else res.view(dx.shape), relu_mask=mask,
+                             tf32_out=bool(e.get('tf32')), relu_mask_bits=mbits)
+            else:
+                x = _stem_input(K, P, dev) if g['C'] == 4 else _to_cl(P.x).to(dev)
+                dw = out.view((g['Co'],) + tuple(g['ker'][:2]) + (8 if g['C'] == 4 else g['ker'][2], g['C']))
+                K.conv_wgrad(_to_cl(P.dy).to(dev), x, dw, geo, row_scale=rs)
+        elif c['op'] == 'matmul':
+            A = P.A.to(dev)
+            if c.get('b_weight'):
+                Bm = P.B[0].contiguous().to(dev).t().unsqueeze(0)              # [1, K, N] view of a [N, K] weight
+            else:
+                Bm = P.B.to(dev).transpose(1, 2)
+            ldd, dbs = P.layout['ldd'], P.layout['dbs']
+            d = torch.as_strided(flat, (Z, M, N), (dbs if Z > 1 else M * ldd, ldd, 1), GUARD)
+            K.matmul(A, Bm, d, bias=cb, tf32_out=bool(e.get('tf32')))
+        else:
+            _run_raw(K, L, ctypes, P, flat, cs, cb, rs, dev)
+        torch.cuda.synchronize()
+    finally:
+        _opts(K, {'opts': {}})
+    return buf, bits
+
+
+def _run_raw(K, L, ctypes, P, flat, cs, cb, rs, dev):
+    c = P.case
+    e = c.get('epi', {})
+    Z, M, N, Kd = c['Z'], c['M'], c['N'], c['K']
+    keep = []
+
+    def operand(X, mn, rows):                                  # X logical [Z, rows, K]
+        o = L.Operand()
+        if mn:
+            s = X.transpose(1, 2).contiguous().to(dev)          # [Z, K, rows]: rows contiguous
+            o.kind, o.ld = L.OP_DENSE_MN, rows
+        else:
+            s = X.contiguous().to(dev)
+            o.kind, o.ld = L.OP_DENSE_K, Kd
+        o.batch_stride = rows * Kd if Z > 1 else 0
+        o.ptr = s.data_ptr()
+        keep.append(s)
+        return o
+
+    p = L.GemmParams()
+    p.a = operand(P.A, c['a_mn'], M)
+    p.b = operand(P.B, c['b_mn'], N)
+    p.M, p.N, p.K, p.batch, p.taps = M, N, Kd, Z, 1
+    p.split_k = c.get('split_k', 1)
+    p.d = flat.data_ptr() + GUARD * 4
+    p.ldd, p.d_batch_stride, p.d_tap_stride = P.layout['ldd'], P.layout['dbs'], 0
+    p.alpha = float(e.get('alpha', 1.0))
+    for name, t in (('col_scale', cs), ('col_bias', cb), ('row_scale', rs)):
+        if t is not None:
+            t = t.contiguous().to(dev)
+            keep.append(t)
+            setattr(p, name, t.data_ptr())
+    if 'res' in P.epi:
+        rbuf = torch.zeros_like(flat)
+        rbuf[P.index.reshape(-1)] = P.epi['res'].reshape(-1).float()
+        keep.append(rbuf)
+        p.residual = rbuf.data_ptr() + GUARD * 4
+    if 'maskv' in P.epi:
+        mbuf = torch.zeros_like(flat)
+        mbuf[P.index.reshape(-1)] = P.epi['maskv'].reshape(-1).float()
+        keep.append(mbuf)
+        p.relu_mask = mbuf.data_ptr() + GUARD * 4
+    p.flags = ((L.EPI_RELU if e.get('relu') else 0) | (L.EPI_ACCUM if e.get('accum') else 0) |
+               (L.EPI_ATOMIC if e.get('atomic') else 0) | (L.EPI_TF32 if e.get('tf32') else 0))
+    ws = K.gemm_workspace(flat.device)
+    p.workspace, p.workspace_bytes = ws.data_ptr(), ws.numel() * 4
+    p.engine = L.ENGINE_TCGEN05
+    p.tile_n, p.pair, p.stream_k = K.GEMM_OPTS['tile_n'], K.GEMM_OPTS['pair'], K.GEMM_OPTS['stream_k']
+    L.check(L.load().vlfb_gemm(ctypes.byref(p), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'vlfb_gemm')
+    torch.cuda.synchronize()
+
+
+def capture_fd2(fn):
+    """Runs fn() with file descriptor 2 redirected to a temporary file (the library writes its VLFB_DEBUG records with
+    fprintf(stderr)); returns (fn's result, the captured text)."""
+    sys.stderr.flush()
+    with tempfile.TemporaryFile() as tmp:
+        saved = os.dup(2)
+        os.dup2(tmp.fileno(), 2)
+        try:
+            out = fn()
+        finally:
+            sys.stderr.flush()
+            os.dup2(saved, 2)
+            os.close(saved)
+        tmp.seek(0)
+        text = tmp.read().decode('utf-8', 'replace')
+    return out, text
+
+
+def check_case(K, c, config, dev):
+    """Runs one case under the current process's configuration; returns its JSON record."""
+    rec = dict(case=c['name'], config=config, errors=[])
+    P = prepare(c, dev)
+    (buf, bits), text = capture_fd2(lambda: run_case(K, P, dev))
+    paths = [r for r in (parse_record(l) for l in text.splitlines()) if r is not None]
+    rec['paths'] = [dict((k, list(v) if isinstance(v, tuple) else v) for k, v in r.items()) for r in paths]
+    rec['flags'] = describe(c)['flags']
+    if len(paths) != 1:
+        rec['errors'].append('expected one tensor-core launch record, got %d' % len(paths))
+    else:
+        r = paths[0]
+        want = describe(c)
+        for k in ('M', 'N', 'K'):
+            if r[k] != want[k]:
+                rec['errors'].append('record %s=%d, case describes %d' % (k, r[k], want[k]))
+        if tuple(r['kinds']) != tuple(want['kinds']):
+            rec['errors'].append('record kinds=%r, case describes %r' % (r['kinds'], want['kinds']))
+        bad = matches(r, c['runs'][config])
+        if bad:
+            rec['errors'].append('path: ' + ', '.join(bad))
+    d = buf.view(-1)[P.index.reshape(-1)].view(P.ref.shape)
+    cmp = compare(d, P.ref, P.bound)
+    rec.update(worst_ratio=cmp['worst_ratio'], worst_at=cmp['worst_at'], rel_err=cmp['rel_err'], tau=tau(P.K))
+    if not cmp['ok']:
+        rec['errors'].append('values: %d elements outside the bound, %d not finite, worst %.3g x bound at %s' % (
+            cmp['nbad'], cmp['nonfinite'], cmp['worst_ratio'], cmp['worst_at']))
+    tol = 6e-4 if c.get('epi', {}).get('tf32') else 2e-5
+    if not cmp['rel_err'] < tol:
+        rec['errors'].append('global rel_err %.3g >= %g' % (cmp['rel_err'], tol))
+    touched = guard_intact(buf, P.index)
+    if touched:
+        rec['errors'].append('%d guard elements overwritten' % touched)
+    if bits is not None:
+        n = P.ref.numel() // 32
+        want_bits = pack_sign_bits(d.float())
+        if not torch.equal(bits[:n], want_bits):
+            rec['errors'].append('sign bits differ from the output in %d words' % int((bits[:n] != want_bits).sum()))
+        if not bool((bits[n:] == 0x5A5A5A5A).all()):
+            rec['errors'].append('sign-bit words past the output overwritten')
+    cnt = K.gemm_workspace(buf.device)[:16384].view(torch.int32)
+    if int(cnt.abs().sum()) != 0:
+        rec['errors'].append('stream-K arrival counters not zero after the launch')
+        cnt.zero_()
+    rec['ok'] = not rec['errors']
+    return rec
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
+    ap.add_argument('--config', required=True, choices=sorted(CONFIGS))
+    ap.add_argument('--out', required=True)
+    args = ap.parse_args(argv)
+    for k, v in CONFIGS[args.config].items():
+        if os.environ.get(k) != v:
+            raise SystemExit('configuration %s needs %s=%s in the environment' % (args.config, k, v))
+    if os.environ.get('VLFB_DEBUG') != '1':
+        raise SystemExit('the path records need VLFB_DEBUG=1')
+    from vlfb import kernels as K
+    dev = torch.device('cuda')
+    K.set_gemm_backend('tcgen05')
+    with open(args.out, 'w') as f:
+        for c in CASES:
+            if args.config not in c['runs']:
+                continue
+            print('[gemm_paths] config=%s case=%s' % (args.config, c['name']), flush=True)
+            try:
+                rec = check_case(K, c, args.config, dev)
+            except Exception as ex:                       # a failing call is a result of the case, not of the run
+                rec = dict(case=c['name'], config=args.config, ok=False, paths=[], errors=['%s: %s' % (type(ex).__name__, ex)])
+            f.write(json.dumps(rec) + '\n')
+            f.flush()
+    print('[gemm_paths] config=%s done' % args.config, flush=True)
+
+
+if __name__ == '__main__':
+    main()

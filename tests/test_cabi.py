@@ -35,6 +35,13 @@ def test_argument_validation_without_gpu():
     assert lib.vlfb_gemm(ctypes.byref(p), None) == -1 and b'tile_n' in lib.vlfb_last_error()
     p.tile_n, p.flags, p.relu_bits_out = 0, 0, 256                    # sign bits without VLFB_EPI_RELU
     assert lib.vlfb_gemm(ctypes.byref(p), None) == -1 and b'relu_bits_out' in lib.vlfb_last_error()
+    # K = 0 (an empty sum): rejected by the ABI for both engines, as by the plan query
+    p.relu_bits_out, p.K = None, 0
+    for engine in (0, 1):
+        p.engine = engine
+        assert lib.vlfb_gemm(ctypes.byref(p), None) == -1 and b'p.K > 0' in lib.vlfb_last_error()
+    plan = libvlfb.GemmPlan()
+    assert lib.vlfb_gemm_plan(ctypes.byref(p), 132, ctypes.byref(plan)) == -1
     assert lib.vlfb_relu_fwd(None, None, 4, None) == -1
 
 

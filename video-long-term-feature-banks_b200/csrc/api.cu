@@ -22,7 +22,7 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 static int validate_gemm(const vlfb_gemm_params_t& p, bool& tc_ok) {
   tc_ok = true;
   VLFB_CHECK_ARG(p.a.ptr && p.b.ptr && p.d);
-  VLFB_CHECK_ARG(p.M > 0 && p.N > 0 && p.K >= 0);
+  VLFB_CHECK_ARG(p.M > 0 && p.N > 0 && p.K > 0);      // K = 0 (an empty sum) is rejected by both engines alike
   VLFB_CHECK_ARG(p.batch >= 1 && p.taps >= 1 && p.split_k >= 0);          // split_k 0 = chosen by the library
   VLFB_CHECK_ARG(!(p.taps > 1 && p.batch > 1));
   VLFB_CHECK_ARG(p.engine == VLFB_ENGINE_TCGEN05 || p.engine == VLFB_ENGINE_SIMT);

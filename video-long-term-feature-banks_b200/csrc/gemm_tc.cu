@@ -1938,9 +1938,6 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   }
   const int smem = L.stages * stage_bytes + img_bytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
   const bool cp = !(L.tma_a && L.tma_b);
-  if (ev.debug)
-    fprintf(stderr, "vlfb gemm_tc: kinds %d,%d M=%d N=%d K=%d z=%d | bn=%d sk=%d split=%d tiles=%d units=%d stages=%d tma=%d,%d cap=%d patch=%d par=%d\n",
-            AK, BK, p.M, p.N, p.K, zbase, L.bn, L.sk, p.split_k, L.total_tiles, units, L.stages, L.tma_a, L.tma_b, cap, L.stem_patch, L.par);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)units);
   cfg.blockDim = dim3((unsigned)((cp ? NPROD : NPROD_TMA) + NEPI));
@@ -1951,6 +1948,12 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
                     (!p.residual || ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && !(p.flags & VLFB_EPI_ACCUM)));
   uint32_t* bits_after = nullptr;
   if (p.relu_bits_out && (!lean || MASK)) { bits_after = p.relu_bits_out; p.relu_bits_out = nullptr; }
+  // VLFB_DEBUG: one record per launch, space-separated key=value (tests/gemm_paths.py parses it; keep the keys stable)
+  if (ev.debug)
+    fprintf(stderr, "vlfb gemm_tc: kinds=%d,%d mask=%d M=%d N=%d K=%d z=%d bn=%d sk=%d split=%d tiles=%d units=%d stages=%d "
+            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d\n",
+            AK, BK, MASK ? 1 : 0, p.M, p.N, p.K, zbase, L.bn, L.sk, p.split_k, L.total_tiles, units, L.stages, L.lag, L.tma_a,
+            L.tma_b, cap, L.stem_patch, L.par, cp ? 1 : 0, L.ws_tiles != nullptr ? 1 : 0, lean ? 1 : 0, bits_after ? 1 : 0);
   int rc = VLFB_OK;
   if (cp) rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);     // (fix-ups are planned for TMA-fed launches only)
   else if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
