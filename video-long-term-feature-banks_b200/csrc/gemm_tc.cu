@@ -214,25 +214,37 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 }
 
 // Consumer-side rewrite of an MN-major stage tile into the K-major SWIZZLE_128B image [row][128 B] that wgmma reads
-// (tf32 operands must be K-major).  Source: `rows` x 32 k as [atom of 32 elements][k-row][128 B], 32-byte units XOR
-// (k & 3) (SWIZZLE_128B_ATOM_32B / MNLoader), atoms `atom_stride` bytes apart; k-rows 128 B apart, or, for the conv1
-// wgrad patch tile (row_gap = sH), k-rows 16-31 (the patch's second output row) row_gap 2 KB slabs further.
-// Thread t moves float4 f = t + NEPI j: 16-byte chunk f % 8 of k-row (f / 8) % 32 of atom f / 256 (conflict-free reads).
+// (tf32 operands in shared memory must be K-major).  Source: `rows` x 32 k as [atom of 32 elements][k-row][128 B],
+// 16-byte chunk c of k-row k at byte (16 c) ^ (32 (k & 3)) (SWIZZLE_128B_ATOM_32B / MNLoader), atoms `atom_stride`
+// bytes apart; k-rows 128 B apart, or, for the conv1 wgrad patch tile (row_gap = sH), k-rows 16-31 (the patch's second
+// output row) row_gap 2 KB slabs further.  Image: element (n, k) at n * 128 + 16 ((k / 4) ^ (n % 8)) + 4 (k % 4).
+// Unit u = t + NEPI j moves a 4 n x 4 k block: k-quad kq = u % 8, source chunk c = kq ^ ((u / 8) % 8) of atom u / 64.
+// It reads chunk c of k-rows 4 kq .. 4 kq + 3 (four v4 loads), transposes in registers and writes rows n = 32 atom +
+// 4 c + q, q = 0..3, at k-quad kq (four v4 stores).  A 16-byte access is served in four phases of 8 lanes, and a phase
+// is conflict-free when its 8 addresses fall in 8 distinct 16-byte slots of the 128-byte bank window.  The 8 lanes of
+// a phase have kq = 0..7 and one value of (u / 8) % 8 = b:
+//   loads:  slot = c ^ 2 (k & 3) = kq ^ b ^ 2 r for load r  -> 8 distinct slots;
+//   stores: slot = kq ^ (n % 8) = kq ^ 4 ((kq ^ b) & 1) ^ q  -> kq ^ const on even kq, kq ^ (const ^ 4) on odd kq, a
+//           bijection of 0..7 (bit 0 is kept) -> 8 distinct slots.
 __device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int rows, int atom_stride, int row_gap, int ctid) {
-  for (int f = ctid; f < rows * 8; f += NEPI) {
-    const int c = f & 7, k = (f >> 3) & 31, atom = f >> 8;
-    const uint32_t koff = row_gap ? (uint32_t)((k >> 4) * row_gap * 2048 + (k & 15) * 128) : (uint32_t)(k * 128);
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                 : "r"(src + (uint32_t)(atom * atom_stride) + koff + (uint32_t)((c * 16) ^ ((k & 3) << 5)))
-                 : "memory");
-    const float e[4] = {v.x, v.y, v.z, v.w};
+  for (int u = ctid; u < rows * 2; u += NEPI) {
+    const int kq = u & 7, c = kq ^ ((u >> 3) & 7), atom = u >> 6;
+    float v[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int k = 4 * kq + r;
+      const uint32_t koff = row_gap ? (uint32_t)((k >> 4) * row_gap * 2048 + (k & 15) * 128) : (uint32_t)(k * 128);
+      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                   : "=f"(v[r][0]), "=f"(v[r][1]), "=f"(v[r][2]), "=f"(v[r][3])
+                   : "r"(src + (uint32_t)(atom * atom_stride) + koff + (uint32_t)((c * 16) ^ (r << 5)))
+                   : "memory");
+    }
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int n = atom * 32 + 4 * c + q;
-      asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (uint32_t)(n * 128 + ((((k >> 2) ^ (n & 7)) << 4) | ((k & 3) << 2)))),
-                   "f"(e[q]) : "memory");
+      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};"
+                   ::"r"(dst + (uint32_t)(n * 128 + ((kq ^ (n & 7)) << 4))), "f"(v[0][q]), "f"(v[1][q]), "f"(v[2][q]), "f"(v[3][q])
+                   : "memory");
     }
   }
 }
@@ -682,9 +694,9 @@ __device__ __forceinline__ bool sched_next(const vlfb_gemm_params_t& p, const La
 // CP = false: both operands are staged by TMA, so one producer warpgroup (one issuing warp) suffices and the CTA is
 // 12 warps with up to 168 registers per thread; the 16-warp CP = true build (8 cp.async gather warps: conv1 stem,
 // strided dgrad, operands TMA cannot address) is capped at 128.
-// FIX: the stream-K fix-up (a piece of a shared tile through the workspace) is compiled in.  Its last-arriver decision
-// is per warp, so the warps of a warpgroup may diverge there and ptxas then serialises the wgmma of the whole kernel;
-// only the launches that plan fix-ups use these instantiations, every other launch keeps the MMA pipeline.
+// FIX: the stream-K fix-up (a piece of a shared tile through the workspace) is compiled in; only the launches that plan
+// fix-ups use these instantiations.  Its last-arriver decision is per warp, so the K loop must leave no MMA in flight
+// when it ends on any path (ptxas would otherwise serialise every wgmma of the kernel, tests/test_gemm_pipeline_cpu.py).
 template <int AK, int BK, bool MASK, bool CP, bool FIX>
 __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_kernel(const vlfb_gemm_params_t p, const Launch L,
                                                               const __grid_constant__ CUtensorMap tmA,
@@ -695,11 +707,12 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
   const int bnh = bn;
   const uint32_t b_tile_bytes = (uint32_t)bn * KC * 4;
   const uint32_t stage_bytes = A_TILE_BYTES + b_tile_bytes;
-  // K-major images of the MN-major operands (wgmma reads tf32 operands K-major only)
+  // K-major images of the MN-major operands (wgmma reads tf32 operands K-major only): one for A, two for B (chunk i
+  // uses B image i % 2)
   constexpr bool TA = is_mn(AK), TB = is_mn(BK);
   const uint32_t ka_img = smem_base + S * stage_bytes;
   const uint32_t kb_img = ka_img + (TA ? (uint32_t)A_TILE_BYTES : 0u);
-  const uint32_t epi_base = kb_img + (TB ? b_tile_bytes : 0u);          // per-consumer-warp transpose tiles
+  const uint32_t epi_base = kb_img + (TB ? 2 * b_tile_bytes : 0u);      // per-consumer-warp transpose tiles
   const uint32_t bar_base = epi_base + EPI_STAGE_BYTES;
   const uint32_t full0 = bar_base, empty0 = bar_base + 8 * MAX_STAGES;
 
@@ -1039,19 +1052,23 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         float acc[BN / 2];
 #pragma unroll
         for (int q = 0; q < BN / 2; ++q) acc[q] = 0.f;
+        // chunk i: at its start this warpgroup's MMAs of chunk i - 2 have completed (the wait<1> that ends chunk i - 1),
+        // so B image i % 2, which chunk i - 2 read, may be rewritten once both warpgroups are there; the MMAs of chunk
+        // i - 1, which read the other image, stay in flight meanwhile.  The single A image waits for all MMAs.
         for (int i = 0; i < ti.nk; ++i) {
           mbar_wait(full0 + 8 * s, ph);
           const uint32_t a_tile = smem_base + s * stage_bytes, b_tile = a_tile + A_TILE_BYTES;
+          const uint32_t b_img = kb_img + (uint32_t)((i & 1) * BN * 128);
           if (TA || TB) {
-            wgmma_wait<0>();                     // no MMA still reads the K-major images
-            consumers_sync();
+            if (TA) wgmma_wait<0>();             // no MMA still reads the A image
+            consumers_sync();                    // both warpgroups are done with chunk i - 2 (TA: i - 1)
             if (TA) mn_to_kmajor(a_tile, ka_img, BM, 4096, 0, ctid);
-            if (TB) mn_to_kmajor(b_tile, kb_img, BN, stem_pb ? 2048 : 4096, stem_pb ? p.g.sH : 0, ctid);
+            if (TB) mn_to_kmajor(b_tile, b_img, BN, stem_pb ? 2048 : 4096, stem_pb ? p.g.sH : 0, ctid);
             fence_proxy_async();                 // generic-proxy writes -> visible to the wgmma (async proxy) reads
-            consumers_sync();
+            consumers_sync();                    // images complete
           }
           const uint32_t a_src = (TA ? ka_img : a_tile) + (uint32_t)wg * (64 * 128);
-          const uint32_t b_src = TB ? kb_img : b_tile;
+          const uint32_t b_src = TB ? b_img : b_tile;
           wgmma_fence();
 #pragma unroll
           for (int j = 0; j < KC / 8; ++j)      // wgmma K = 8 for tf32: 32 bytes along the swizzled 128-byte rows
@@ -1064,10 +1081,10 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           sprev = s;
           if (++s == S) { s = 0; ph ^= 1u; }
         }
-        if (ti.nk > 0) {
-          wgmma_wait<0>();
-          if ((ctid & 127) == 0) mbar_arrive(empty0 + 8 * sprev);
-        }
+        // unconditional: a path that skips this wait (nk == 0) would let ptxas see accumulators in flight after the
+        // loop, and it then serialises every wgmma of the kernel
+        wgmma_wait<0>();
+        if (ti.nk > 0 && (ctid & 127) == 0) mbar_arrive(empty0 + 8 * sprev);
         // fragment (n8 group j: rows lane / 4 and lane / 4 + 8, columns 8 j + 2 (lane % 4) + {0, 1}) -> stg
         float* r = stg + (lane >> 2) * EPITCH + 2 * (lane & 3);
 #pragma unroll
@@ -1911,7 +1928,7 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   L.tiles_n = ceil_div(p.N, L.bn);
   L.total_tiles = (int)((int64_t)L.tiles_m * L.tiles_n * zbase * p.split_k);
   const int stage_bytes = A_TILE_BYTES + L.bn * KC * 4;
-  const int img_bytes = (is_mn(AK) ? A_TILE_BYTES : 0) + (is_mn(BK) ? L.bn * KC * 4 : 0);     // K-major images
+  const int img_bytes = (is_mn(AK) ? A_TILE_BYTES : 0) + (is_mn(BK) ? 2 * L.bn * KC * 4 : 0);   // K-major images: A, 2 x B
   L.stages = (227 * 1024 - EPI_STAGE_BYTES - img_bytes - 2048) / stage_bytes;
   if (L.stages > 6) L.stages = 6;
   if (ev.stages >= 3 && ev.stages <= L.stages) L.stages = ev.stages;
