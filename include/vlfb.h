@@ -215,6 +215,7 @@ int vlfb_layernorm_bwd(const float* dy, const float* y, const float* std, float*
                        int cols, void* stream);
 
 /* ---- elementwise ------------------------------------------------------------------------ */
+/* n == 0 launches nothing and accepts NULL pointers (an empty tensor has no storage); n < 0 is VLFB_E_BADARG. */
 int vlfb_relu_fwd(const float* x, float* y, int64_t n, void* stream);
 int vlfb_relu_bwd(const float* dy, const float* y, float* dx, int64_t n, void* stream); /* dx = dy*(y>0) */
 int vlfb_axpby(const float* x, float a, const float* y, float b, float* out, int64_t n, void* stream);

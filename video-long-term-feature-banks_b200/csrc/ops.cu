@@ -419,7 +419,8 @@ __global__ void ew_k(const float* __restrict__ a, const float* __restrict__ b, f
 
 template <int OP>
 int ew_launch(const float* a, const float* b, float* o, int64_t n, float s0, float s1, cudaStream_t st) {
-  if (n <= 0) return VLFB_OK;
+  VLFB_CHECK_ARG(n >= 0);
+  if (n == 0) return VLFB_OK;          // nothing to touch: the pointers may be NULL (empty tensors have no storage)
   const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(o)) & 15) == 0;
   launch_k(ew_k<OP>, stream_grid(n, TPB, 4), TPB, 0, st, a, b, o, n, s0, s1, vec ? 1 : 0);
   VLFB_CHECK_LAUNCH();
@@ -904,31 +905,31 @@ int vlfb_layernorm_bwd(const float* dy, const float* y, const float* std, float*
 }
 
 int vlfb_relu_fwd(const float* x, float* y, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && y && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (x && y));
   return ew_launch<EW_RELU>(x, nullptr, y, n, 0.f, 0.f, ST(stream));
 }
 int vlfb_relu_bwd(const float* dy, const float* y, float* dx, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(dy && y && dx && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (dy && y && dx));
   return ew_launch<EW_RELU_BWD>(dy, y, dx, n, 0.f, 0.f, ST(stream));
 }
 int vlfb_axpby(const float* x, float a, const float* y, float b, float* out, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && out && n >= 0 && (y || b == 0.f));
+  VLFB_CHECK_ARG(n == 0 || (x && out && (y || b == 0.f)));
   return ew_launch<EW_AXPBY>(x, y, out, n, a, b, ST(stream));
 }
 int vlfb_fill(float* x, float v, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || x);
   return ew_launch<EW_FILL>(nullptr, nullptr, x, n, v, 0.f, ST(stream));
 }
 int vlfb_round_tf32(const float* x, float* y, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && y && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (x && y));
   return ew_launch<EW_TF32>(x, nullptr, y, n, 0.f, 0.f, ST(stream));
 }
 int vlfb_add_tf32(const float* x, const float* y, float* out, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && y && out && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (x && y && out));
   return ew_launch<EW_ADD_TF32>(x, y, out, n, 0.f, 0.f, ST(stream));
 }
 int vlfb_relu_tf32(const float* x, float* y, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && y && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (x && y));
   return ew_launch<EW_RELU_TF32>(x, nullptr, y, n, 0.f, 0.f, ST(stream));
 }
 int vlfb_relu_bits(const float* x, uint32_t* bits, int64_t n, void* stream) {
@@ -936,12 +937,13 @@ int vlfb_relu_bits(const float* x, uint32_t* bits, int64_t n, void* stream) {
   return relu_bits(x, bits, n, ST(stream));
 }
 int vlfb_relu_bwd_tf32(const float* dy, const float* y, float* dx, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(dy && y && dx && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (dy && y && dx));
   return ew_launch<EW_RELU_BWD_TF32>(dy, y, dx, n, 0.f, 0.f, ST(stream));
 }
 int vlfb_add_relu_bwd_tf32(const float* a, const float* b, const float* y, float* out, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(a && b && out && n >= 0);
+  VLFB_CHECK_ARG(n >= 0);
   if (n == 0) return VLFB_OK;
+  VLFB_CHECK_ARG(a && b && out);
   const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(y) |
                      reinterpret_cast<uintptr_t>(out)) & 15) == 0;
   launch_k(add_mask_tf32_k, stream_grid(n, TPB, 4), TPB, 0, ST(stream), a, b, y, out, n, vec ? 1 : 0);
@@ -966,7 +968,7 @@ int vlfb_colsum(const float* x, int64_t ld, float* out, int64_t rows, int cols, 
   return VLFB_OK;
 }
 int vlfb_sigmoid_fwd(const float* x, float* y, int64_t n, void* stream) {
-  VLFB_CHECK_ARG(x && y && n >= 0);
+  VLFB_CHECK_ARG(n == 0 || (x && y));
   return ew_launch<EW_SIGMOID>(x, nullptr, y, n, 0.f, 0.f, ST(stream));
 }
 
