@@ -115,11 +115,23 @@ typedef struct {
                                * backward at 1/32 of the bytes of the activation itself. */
   uint32_t* relu_bits_out;    /* or NULL: with VLFB_EPI_RELU, bit = (stored value > 0).  Dense outputs only: ldd == N,
                                * N % 32 == 0, batch == taps == split_k == 1, no VLFB_EPI_ATOMIC; M * N / 32 words. */
+  /* ---- grouped convolution (Caffe2 Conv `group`, the ResNeXt branch2b conv) ----
+   * 0 or 1: an ungrouped GEMM, exactly as above.  G > 1: output channel co reads only the input channels of group
+   * co / Cog (Cig = C / G, Cog = Co / G, each a multiple of 4 in [4, 64]).  Three forms, run on CUDA cores
+   * (csrc/gconv.cu; `engine`, `tile_n`, `pair`, `stream_k` and the workspace are ignored):
+   *   fwd   a = CONV_K x,  b = DENSE_K w [Co][kT*kH*kW*Cig] (ld >= K); M = N*To*Ho*Wo, N = Co, K = taps*Cig
+   *   dgrad a = DGRAD_K dy, b = DENSE_K wt [C][taps*Cog], group g's rows = vlfb_weight_transpose of its [Cog][taps][Cig]
+   *         slab of w (one vlfb_weight_transpose_multi job per group); M = N*T*H*W, N = C, K = taps*Cog
+   *   wgrad a = DENSE_MN dy (ld = Co), b = CONV_MN x; M = Co, N = kH*kW*Cig, taps = kT, K = N*To*Ho*Wo; needs
+   *         VLFB_EPI_ATOMIC; epilogue alpha, col_scale, row_scale only
+   * fwd / dgrad take every epilogue field except VLFB_EPI_ATOMIC, with ldd % 4 == 0 and 16-byte aligned d / residual /
+   * relu_mask.  batch and split_k must be 1 (split_k 0 is accepted as 1).  vlfb_gemm_plan returns VLFB_E_UNSUPPORTED. */
+  int groups;
 } vlfb_gemm_params_t;
 
 enum { VLFB_ENGINE_TCGEN05 = 0, VLFB_ENGINE_SIMT = 1 };
 
-/* What vlfb_gemm would do for `p` (host-only, no launch). */
+/* What vlfb_gemm would do for `p` (host-only, no launch; not defined for groups > 1). */
 typedef struct {
   int tile_n;                 /* output-tile width */
   int split_k;                /* plain split-K factor (atomic epilogues) */

@@ -89,6 +89,82 @@ static int validate_gemm(const vlfb_gemm_params_t& p, bool& tc_ok) {
   return VLFB_OK;
 }
 
+// groups > 1: the grouped-convolution forms of include/vlfb.h (fwd, dgrad, wgrad), run by gconv.cu.
+#define GCONV_REQUIRE(cond, code, ...)  \
+  do {                                  \
+    if (!(cond)) {                      \
+      set_error(__VA_ARGS__);           \
+      return code;                      \
+    }                                   \
+  } while (0)
+
+static int validate_gconv(const vlfb_gemm_params_t& p) {
+  const vlfb_conv_geom_t& g = p.g;
+  const int G = p.groups;
+  VLFB_CHECK_ARG(p.a.ptr && p.b.ptr && p.d);
+  VLFB_CHECK_ARG(p.M > 0 && p.N > 0 && p.K > 0);
+  GCONV_REQUIRE(p.batch == 1, VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 needs batch == 1");
+  GCONV_REQUIRE(p.split_k == 0 || p.split_k == 1, VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 needs split_k <= 1");
+  GCONV_REQUIRE(p.a.kind != VLFB_OP_STEM_K && p.a.kind != VLFB_OP_STEM_MN && p.b.kind != VLFB_OP_STEM_K &&
+                    p.b.kind != VLFB_OP_STEM_MN,
+                VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 is not defined for the STEM_* operands");
+  GCONV_REQUIRE(!(p.a.kind == VLFB_OP_DENSE_K), VLFB_E_UNSUPPORTED,
+                "vlfb_gemm: groups > 1 with a DENSE_K A operand (a pointwise conv) is not supported");
+  GCONV_REQUIRE(g.C > 0 && g.Co > 0 && g.C % G == 0 && g.Co % G == 0, VLFB_E_BADARG,
+                "vlfb_gemm: groups = %d must divide C = %d and Co = %d", G, g.C, g.Co);
+  const int Cig = g.C / G, Cog = g.Co / G;
+  GCONV_REQUIRE(Cig % 4 == 0 && Cig >= 4 && Cig <= 64 && Cog % 4 == 0 && Cog >= 4 && Cog <= 64, VLFB_E_UNSUPPORTED,
+                "vlfb_gemm: grouped conv widths Cig = %d, Cog = %d must be multiples of 4 in [4, 64]", Cig, Cog);
+  VLFB_CHECK_ARG(g.N > 0 && g.T > 0 && g.H > 0 && g.W > 0 && g.To > 0 && g.Ho > 0 && g.Wo > 0);
+  VLFB_CHECK_ARG(g.kT > 0 && g.kH > 0 && g.kW > 0 && g.sT > 0 && g.sH > 0 && g.sW > 0);
+  VLFB_CHECK_ARG(g.pT >= 0 && g.pH >= 0 && g.pW >= 0 && g.dT > 0 && g.dH > 0 && g.dW > 0);
+  const int64_t in_elems = (int64_t)g.N * g.T * g.H * g.W * g.C;
+  const int64_t out_elems = (int64_t)g.N * g.To * g.Ho * g.Wo * g.Co;
+  GCONV_REQUIRE(in_elems < (1ll << 31) && out_elems < (1ll << 31), VLFB_E_BADARG,
+                "vlfb_gemm: conv tensors of >= 2^31 elements are not supported (split the batch)");
+  const int taps = g.kT * g.kH * g.kW;
+  const int64_t in_pos = (int64_t)g.N * g.T * g.H * g.W, out_pos = (int64_t)g.N * g.To * g.Ho * g.Wo;
+  const uintptr_t mis = reinterpret_cast<uintptr_t>(p.a.ptr) | reinterpret_cast<uintptr_t>(p.b.ptr);
+  VLFB_CHECK_ARG(!(p.relu_mask && p.relu_mask_bits));
+  if (p.a.kind == VLFB_OP_DENSE_MN) {          // wgrad
+    GCONV_REQUIRE(p.b.kind == VLFB_OP_CONV_MN && p.a.ld == g.Co && p.M == g.Co && p.N == g.kH * g.kW * Cig &&
+                      p.taps == g.kT && (int64_t)p.K == out_pos,
+                  VLFB_E_BADARG, "vlfb_gemm: grouped wgrad needs a = DENSE_MN dy (ld = Co), b = CONV_MN x, M = Co, "
+                  "N = kH*kW*Cig, taps = kT, K = N*To*Ho*Wo");
+    GCONV_REQUIRE((p.flags & VLFB_EPI_ATOMIC) && !(p.flags & (VLFB_EPI_RELU | VLFB_EPI_ACCUM | VLFB_EPI_TF32)) &&
+                      !p.col_bias && !p.residual && !p.relu_mask && !p.relu_mask_bits && !p.relu_bits_out,
+                  VLFB_E_BADARG, "vlfb_gemm: grouped wgrad accumulates (VLFB_EPI_ATOMIC) with alpha, col_scale and "
+                  "row_scale only");
+    GCONV_REQUIRE((mis & 15) == 0, VLFB_E_BADARG, "vlfb_gemm: grouped conv operands must be 16-byte aligned");
+    return VLFB_OK;
+  }
+  const bool dgrad = p.a.kind == VLFB_OP_DGRAD_K;
+  GCONV_REQUIRE(p.a.kind == VLFB_OP_CONV_K || dgrad, VLFB_E_BADARG,
+                "vlfb_gemm: groups > 1 needs A = CONV_K (fwd), DGRAD_K (dgrad) or DENSE_MN (wgrad)");
+  GCONV_REQUIRE(p.b.kind == VLFB_OP_DENSE_K && p.b.ld >= p.K, VLFB_E_BADARG,
+                "vlfb_gemm: grouped fwd / dgrad needs b = DENSE_K weights with ld >= K");
+  if (dgrad)
+    GCONV_REQUIRE(p.N == g.C && p.K == taps * Cog && (int64_t)p.M == in_pos, VLFB_E_BADARG,
+                  "vlfb_gemm: grouped dgrad needs M = N*T*H*W, N = C, K = taps*Cog");
+  else
+    GCONV_REQUIRE(p.N == g.Co && p.K == taps * Cig && (int64_t)p.M == out_pos, VLFB_E_BADARG,
+                  "vlfb_gemm: grouped fwd needs M = N*To*Ho*Wo, N = Co, K = taps*Cig");
+  GCONV_REQUIRE(!(p.flags & VLFB_EPI_ATOMIC), VLFB_E_UNSUPPORTED,
+                "vlfb_gemm: grouped fwd / dgrad store their output (no VLFB_EPI_ATOMIC)");
+  const uintptr_t out_mis = reinterpret_cast<uintptr_t>(p.a.ptr) | reinterpret_cast<uintptr_t>(p.d) |
+                            reinterpret_cast<uintptr_t>(p.residual) | reinterpret_cast<uintptr_t>(p.relu_mask) |
+                            reinterpret_cast<uintptr_t>(p.col_scale) | reinterpret_cast<uintptr_t>(p.col_bias);
+  GCONV_REQUIRE((out_mis & 15) == 0 && p.ldd >= p.N && (p.ldd & 3) == 0, VLFB_E_BADARG,
+                "vlfb_gemm: grouped fwd / dgrad need 16-byte aligned x / dy, d, residual, relu_mask, col_scale, "
+                "col_bias and ldd %% 4 == 0");
+  if (p.relu_bits_out)
+    GCONV_REQUIRE((p.flags & VLFB_EPI_RELU) && p.ldd == p.N && (p.N & 31) == 0 &&
+                      (reinterpret_cast<uintptr_t>(p.relu_bits_out) & 3) == 0,
+                  VLFB_E_BADARG, "vlfb_gemm: relu_bits_out needs VLFB_EPI_RELU and a dense output with N %% 32 == 0");
+  return VLFB_OK;
+}
+#undef GCONV_REQUIRE
+
 }  // namespace vlfb
 
 using namespace vlfb;
@@ -99,6 +175,10 @@ int vlfb_version(void) { return 100; }
 const char* vlfb_last_error(void) { return g_err; }
 int vlfb_gemm_plan(const vlfb_gemm_params_t* p, int num_sms, vlfb_gemm_plan_t* plan) {
   VLFB_CHECK_ARG(p && plan && p->M > 0 && p->N > 0 && p->K > 0);
+  if (p->groups > 1) {
+    set_error("vlfb_gemm_plan: grouped convolutions (groups > 1) run on CUDA cores and have no tile plan");
+    return VLFB_E_UNSUPPORTED;
+  }
   gemm_tc_plan(*p, num_sms > 0 ? num_sms : 132, plan);
   return VLFB_OK;
 }
@@ -112,6 +192,11 @@ int vlfb_debug_set_trace(void* buf) { vlfb::gemm_tc_set_trace(buf); return VLFB_
 
 int vlfb_gemm(const vlfb_gemm_params_t* p, void* stream) {
   VLFB_CHECK_ARG(p != nullptr);
+  VLFB_CHECK_ARG(p->groups >= 0);
+  if (p->groups > 1) {                 // Caffe2 grouped Conv: CUDA-core kernels, `engine` does not apply
+    const int rc = validate_gconv(*p);
+    return rc != VLFB_OK ? rc : gconv(*p, static_cast<cudaStream_t>(stream));
+  }
   bool tc_ok = true;
   int rc = validate_gemm(*p, tc_ok);
   if (rc != VLFB_OK) return rc;

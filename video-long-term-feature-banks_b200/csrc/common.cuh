@@ -151,6 +151,7 @@ __device__ __forceinline__ void epilogue_store(const vlfb_gemm_params_t& p, int 
 int gemm_simt(const vlfb_gemm_params_t& p, cudaStream_t stream);
 int relu_bits(const float* x, uint32_t* bits, int64_t n, cudaStream_t stream);     // ops.cu
 int gemm_tc(const vlfb_gemm_params_t& p, cudaStream_t stream);
+int gconv(const vlfb_gemm_params_t& p, cudaStream_t stream);                       // groups > 1 (gconv.cu)
 void gemm_tc_plan(const vlfb_gemm_params_t& p, int num_sms, vlfb_gemm_plan_t* out);
 size_t gemm_tc_workspace_bytes();
 #ifdef VLFB_TRACE

@@ -54,17 +54,29 @@ class CNNModelHelper(object):
     def ConvNd(self, blob_in, blob_out, dim_in, dim_out, kernel, weight_init=None, bias_init=None,
                strides=None, pads=None, no_bias=0, group=1, dilations=None, **kwargs):
         kernels = list(kernel) if isinstance(kernel, (list, tuple)) else [kernel] * 3
-        assert group == 1, 'grouped convolutions are not used by any shipped config'
-        w = self._make_param(blob_out + '_w', [dim_out, dim_in] + kernels,
+        group = int(group)
+        if group > 1:
+            # Caffe2 grouped Conv (ResNeXt branch2b, resnet_helper.py bottleneck_transformation_3d): the CUDA-core
+            # kernels of csrc/gconv.cu take per-group widths that are multiples of 4 in [4, 64], spatial kernels only
+            cig, cog = dim_in // group, dim_out // group
+            if dim_in % group or dim_out % group or not all(c % 4 == 0 and 4 <= c <= 64 for c in (cig, cog)):
+                raise ValueError('%s: grouped conv %d -> %d channels in %d groups needs per-group widths that are '
+                                 'multiples of 4 in [4, 64]' % (blob_out, dim_in, dim_out, group))
+            if len(kernels) != 3 or kernels == [1, 1, 1]:
+                raise ValueError('%s: grouped convs need a 3-D spatial kernel (no grouped 1x1x1 conv)' % blob_out)
+        elif group != 1:
+            raise ValueError('%s: group must be >= 1, got %d' % (blob_out, group))
+        w = self._make_param(blob_out + '_w', [dim_out, dim_in // group] + kernels,
                              weight_init or ('XavierFill', {}), True)
         inputs = [blob_in, w]
         if not no_bias:
             inputs.append(self._make_param(blob_out + '_b', [dim_out],
                                            bias_init or ('ConstantFill', {'value': 0.}), False))
+        extra = {'group': group} if group > 1 else {}
         return self.net.Conv(inputs, blob_out, kernels=kernels,
                              strides=list(strides or [1] * len(kernels)),
                              pads=list(pads or [0] * (2 * len(kernels))),
-                             dilations=list(dilations or [1] * len(kernels)), order=self.order)
+                             dilations=list(dilations or [1] * len(kernels)), order=self.order, **extra)
 
     def FC(self, blob_in, blob_out, dim_in, dim_out, weight_init=None, bias_init=None, **kwargs):
         w = self._make_param(blob_out + '_w', [dim_out, dim_in], weight_init or ('XavierFill', {}), True)

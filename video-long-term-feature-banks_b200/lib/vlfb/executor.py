@@ -281,6 +281,8 @@ class ConvStep(Step):
         self.out = out_name or op.outputs[0]
         self.params = [self.w] + ([self.b] if self.b else [])
         self.round_out = True             # False: the consumer is not a GEMM (SpatialBN) and wants the fp32 sums
+        self.groups = int(op.args.get('group', 1))      # Caffe2 grouped Conv (ResNeXt branch2b): csrc/gconv.cu
+        self.gkw = {'groups': self.groups} if self.groups > 1 else {}     # kernel-wrapper keyword of grouped convs
 
     def _geom(self, ctx, xp):
         a = self.op.args
@@ -314,7 +316,7 @@ class ConvStep(Step):
             bits = empty((y.numel() // 32,), torch.int32)
             ctx.relu_bits[self.out_keys[0]] = bits
         K.conv_fwd(xp, w, phys(y), g, scale=scale, bias=bias, residual=res, relu=self.relu, tf32_out=self.round_out,
-                   relu_bits=bits)
+                   relu_bits=bits, **self.gkw)
         ctx.saved[id(self)] = (xp, g)
         ctx.put(self.out, y, rounded=self.round_out)
 
@@ -339,7 +341,7 @@ class ConvStep(Step):
         store = ctx.ws.params
         if store.trainable(self.w):
             mask = store.stem_mask() if g.C == 4 else None
-            K.conv_wgrad(gp, xp, store.grad(self.w), g, row_scale=scale, col_mask=mask)
+            K.conv_wgrad(gp, xp, store.grad(self.w), g, row_scale=scale, col_mask=mask, **self.gkw)
         if self.b and store.trainable(self.b):
             db = store.grad(self.b)
             rows = gp.numel() // g.Co
@@ -356,8 +358,8 @@ class ConvStep(Step):
             taps = g.kT * g.kH * g.kW
             wt = ctx.net.wt_buffers.get(id(self))                 # filled for all convs by one launch (_prepare_wt)
             if wt is None:
-                wt = empty((g.C, taps, g.Co))
-                K.weight_transpose(store.phys(self.w), wt, scale)     # wt = round_tf32(w * s)
+                wt = empty((g.C, taps, g.Co // self.groups))
+                K.weight_transpose(store.phys(self.w), wt, scale, **self.gkw)     # wt = round_tf32(w * s)
             cur = ctx.grads.get(xkey)
             prod = ctx.net.producer.get(xkey)
             if (isinstance(prod, ConvStep) and ctx.is_last_contribution(xkey) and FUSE_GRAD_FINISH
@@ -372,22 +374,23 @@ class ConvStep(Step):
                 ctx._settle(xkey)                 # a deferred sum must be complete before the gradient is finalised
                 if cur is not None and ctx.owned.get(xkey, False):
                     dx = cur
-                    K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, relu_mask=mask, relu_mask_bits=mbits, tf32_out=True)
+                    K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, relu_mask=mask, relu_mask_bits=mbits, tf32_out=True,
+                                 **self.gkw)
                 else:
                     dx = cl_alloc((g.N, g.C, g.T, g.H, g.W))
                     if dx.shape != ctx.get(self.x).shape:
                         dx = dx.view(ctx.get(self.x).shape)
                     K.conv_dgrad(gp, wt, as5d(phys(dx)), g, residual=None if cur is None else as5d(phys(cur)),
-                                 relu_mask=mask, relu_mask_bits=mbits, tf32_out=True)
+                                 relu_mask=mask, relu_mask_bits=mbits, tf32_out=True, **self.gkw)
                 ctx.set_final_grad(xkey, dx)
                 STATS['fused_grad_finish'] += 1
             elif cur is not None and ctx.owned.get(xkey, False):
                 ctx.counts[xkey] = ctx.counts.get(xkey, 0) + 1
-                K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True)
+                K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, **self.gkw)
             else:
                 dx = cl_alloc((g.N, g.C, g.T, g.H, g.W))
                 sole = ctx.sole(xkey)
-                K.conv_dgrad(gp, wt, phys(dx), g, accumulate=False, tf32_out=sole)
+                K.conv_dgrad(gp, wt, phys(dx), g, accumulate=False, tf32_out=sole, **self.gkw)
                 ctx.add_grad(xkey, dx.view(ctx.get(self.x).shape) if dx.shape != ctx.get(self.x).shape else dx,
                              owned=True, rounded=sole)
 
@@ -1376,9 +1379,9 @@ class CompiledNet(object):
                     if ci == 4:
                         continue                                # the stem never propagates a gradient
                     taps = w.numel() // (co * ci)
-                    wt = empty((ci, taps, co))
+                    wt = empty((ci * st.groups, taps, co // st.groups))      # grouped: [C][taps][Cog], one job per group
                     self.wt_buffers[id(st)] = wt
-                    jobs.append((w, wt, store.phys(st.affine[0]) if st.affine else None))
+                    jobs.extend(K_default.grouped_wt_slices(w, wt, store.phys(st.affine[0]) if st.affine else None, st.groups))
             self._wt_jobs = jobs
         if self._wt_jobs:
             K.weight_transpose_multi(self._wt_jobs, self._wt_cache)

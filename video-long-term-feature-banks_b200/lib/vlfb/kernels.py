@@ -198,15 +198,27 @@ def _set_epilogue(p, scale=None, bias=None, row_scale=None, residual=None, relu=
 
 
 # --------------------------------------------------------------------------- convolution
-def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_out=False, relu_bits=None):
+def _check_groups(g, groups):
+    groups = int(groups)
+    if groups > 1 and (_is_pointwise(g) or g.C == 4):
+        raise ValueError('grouped convolutions need a spatial kernel and C != 4 (no pointwise or stem form)')
+    return groups
+
+
+def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_out=False, relu_bits=None, groups=1):
     """y = epi(conv(x, w)).  x [N,T,H,W,C], w [Co,kT,kH,kW,C], y [N,To,Ho,Wo,Co];
     epi: *scale[co] + bias[co] (+ residual) (ReLU).  C == 4 selects the stem (conv1) path with
     w [Co,kT,kH,8,4].  relu_bits (int32 [y.numel() / 32], with relu): also the sign bits of y, the mask of the
-    ReLU's backward (conv_dgrad relu_mask_bits)."""
+    ReLU's backward (conv_dgrad relu_mask_bits).  groups > 1: Caffe2 grouped Conv, w [Co,kT,kH,kW,C/groups]."""
     _f32c(w, 'w'), _f32c(y, 'y')
     assert tuple(x.shape) == (g.N, g.T, g.H, g.W, g.C) and tuple(y.shape) == out_shape(g)
     M = g.N * g.To * g.Ho * g.Wo
-    if g.C == 4:
+    groups = _check_groups(g, groups)
+    if groups > 1:
+        K = g.kT * g.kH * g.kW * (g.C // groups)
+        assert tuple(w.shape) == (g.Co, g.kT, g.kH, g.kW, g.C // groups)
+        a = _operand(_f32c(x, 'x'), L.OP_CONV_K)
+    elif g.C == 4:
         K = g.kT * g.kH * 32
         assert tuple(w.shape) == (g.Co, g.kT, g.kH, 8, 4)
         a = _operand(x, L.OP_STEM_K, ld=_stem_pitch(x, g))
@@ -221,24 +233,32 @@ def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_
     p.a = a
     p.b = _operand(w, L.OP_DENSE_K, ld=K)
     p.g = g
+    p.groups = groups
     _set_epilogue(p, scale, bias, None, residual, relu, tf32_out)
     if relu_bits is not None:
         assert relu and relu_bits.dtype == torch.int32 and relu_bits.numel() * 32 == y.numel() and relu_bits.is_contiguous()
         p.relu_bits_out = relu_bits.data_ptr()
-    _run_gemm(p, 'conv_fwd', 2.0 * M * g.Co * g.kT * g.kH * g.kW * (3 if g.C == 4 else g.C),
+    _run_gemm(p, 'conv_fwd', 2.0 * M * g.Co * g.kT * g.kH * g.kW * (3 if g.C == 4 else g.C // max(groups, 1)),
               _nbytes(x, w, y, residual) + (relu_bits.numel() * 4.0 if relu_bits is not None else 0.0),
               keep=(x, w, y, scale, bias, residual, relu_bits))
 
 
-def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, tf32_out=False, relu_mask_bits=None):
+def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, tf32_out=False, relu_mask_bits=None,
+               groups=1):
     """dx = finish(conv_transpose(dy, w) [+ dx if accumulate] [+ residual]).  wt [C, kT,kH,kW, Co] (see
     weight_transpose), dx [N,T,H,W,C].  finish = the backward of the ReLU that produced this layer's input
     (relu_mask = that activation, dx zeroed where it is <= 0) and the TF32 rounding the next GEMM needs: when
-    this GEMM is the last contribution to the gradient, both are done here instead of in two more passes."""
+    this GEMM is the last contribution to the gradient, both are done here instead of in two more passes.
+    groups > 1: wt [C, kT,kH,kW, Co/groups] (weight_transpose(..., groups=groups))."""
     _f32c(dy, 'dy'), _f32c(wt, 'wt'), _f32c(dx, 'dx')
     assert tuple(dy.shape) == out_shape(g) and tuple(dx.shape) == (g.N, g.T, g.H, g.W, g.C)
     M = g.N * g.T * g.H * g.W
-    if _is_pointwise(g):
+    groups = _check_groups(g, groups)
+    if groups > 1:
+        K = g.kT * g.kH * g.kW * (g.Co // groups)
+        assert wt.numel() == g.C * K
+        a = _operand(dy, L.OP_DGRAD_K)
+    elif _is_pointwise(g):
         K = g.Co
         a = _operand(dy, L.OP_DENSE_K, ld=g.Co)
     else:
@@ -248,6 +268,7 @@ def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, t
     p.a = a
     p.b = _operand(wt, L.OP_DENSE_K, ld=K)
     p.g = g
+    p.groups = groups
     if accumulate:
         p.flags |= L.EPI_ACCUM
     if residual is not None:
@@ -262,19 +283,25 @@ def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, t
     if tf32_out:
         p.flags |= L.EPI_TF32
     # algorithmic dgrad work = forward MACs of the same layer
-    _run_gemm(p, 'conv_dgrad', 2.0 * g.N * g.To * g.Ho * g.Wo * g.Co * g.kT * g.kH * g.kW * g.C,
+    _run_gemm(p, 'conv_dgrad', 2.0 * g.N * g.To * g.Ho * g.Wo * g.Co * g.kT * g.kH * g.kW * g.C // max(groups, 1),
               _nbytes(dy, wt, dx, residual, relu_mask) + (_nbytes(dx) if accumulate else 0.0) +
               (relu_mask_bits.numel() * 4.0 if relu_mask_bits is not None else 0.0),
               keep=(dy, wt, dx, residual, relu_mask, relu_mask_bits))
 
 
-def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None):
+def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None, groups=1):
     """dw[co,tap,ci] += row_scale[co] * sum_m dy[m,co] * x[gather(m,tap),ci]  (atomic accumulate:
     dw must be zero-initialised or hold a partial sum).  Stem path when C == 4 (dw [Co,kT,kH,8,4],
-    col_mask [32] zeroes the padding lanes)."""
+    col_mask [32] zeroes the padding lanes).  groups > 1: dw [Co,kT,kH,kW,C/groups], ci within co's group."""
     _f32c(dy, 'dy'), _f32c(dw, 'dw')
     Kpos = g.N * g.To * g.Ho * g.Wo
-    if g.C == 4:
+    groups = _check_groups(g, groups)
+    cin = g.C // max(groups, 1)
+    if groups > 1:
+        assert tuple(dw.shape) == (g.Co, g.kT, g.kH, g.kW, cin)
+        taps, n = g.kT, g.kH * g.kW * cin
+        b = _operand(_f32c(x, 'x'), L.OP_CONV_MN)
+    elif g.C == 4:
         taps, n = g.kT, g.kH * 32
         b = _operand(x, L.OP_STEM_MN, ld=_stem_pitch(x, g))
         if col_mask is not None and col_mask.numel() == 32:
@@ -292,19 +319,35 @@ def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None):
     p.taps = taps
     p.d_tap_stride = n
     p.split_k = 0            # split-K and the tile width are chosen together by the library (gemm_tc.cu launch())
+    p.groups = groups
     p.flags |= L.EPI_ATOMIC
     _set_epilogue(p, col_mask, None, row_scale, None, False)
-    _run_gemm(p, 'conv_wgrad', 2.0 * Kpos * g.Co * g.kT * g.kH * g.kW * (3 if g.C == 4 else g.C),
+    _run_gemm(p, 'conv_wgrad', 2.0 * Kpos * g.Co * g.kT * g.kH * g.kW * (3 if g.C == 4 else cin),
               _nbytes(dy, x, dw), keep=(dy, x, dw, row_scale, col_mask))
 
 
-def weight_transpose(w, wt, scale=None):
-    """wt[ci][tap][co] = w[co][tap][ci] * scale[co]."""
+def weight_transpose(w, wt, scale=None, groups=1):
+    """wt[ci][tap][co] = w[co][tap][ci] * scale[co].  groups > 1: w [Co][taps][Cig] -> wt [C][taps][Cog], each group's
+    slab transposed on its own (the dgrad B operand of a grouped conv)."""
     _f32c(w), _f32c(wt)
-    co, ci = w.shape[0], w.shape[-1]
-    taps = w.numel() // (co * ci)
-    _check(L.load().vlfb_weight_transpose(_ptr(w), _ptr(wt), _ptr(scale), co, taps, ci, _stream()),
-            'weight_transpose')
+    for w_, wt_, s_ in grouped_wt_slices(w, wt, scale, groups):
+        co, ci = w_.shape[0], w_.shape[-1]
+        taps = w_.numel() // (co * ci)
+        _check(L.load().vlfb_weight_transpose(_ptr(w_), _ptr(wt_), _ptr(s_), co, taps, ci, _stream()),
+               'weight_transpose')
+
+
+def grouped_wt_slices(w, wt, scale, groups):
+    """[(w slab, wt slab, scale slice)] of each group: w [Co][...][Cig] rows g*Cog.., wt rows g*Cig.. of [C][taps][Cog]."""
+    groups = max(int(groups), 1)
+    if groups == 1:
+        return [(w, wt, scale)]
+    co, cig = w.shape[0], w.shape[-1]
+    cog = co // groups
+    ws, wts = w.view(groups, -1), wt.view(groups, -1)
+    shape = (cog,) + tuple(w.shape[1:])
+    return [(ws[i].view(shape), wts[i].view(cig, -1, cog), None if scale is None else scale[i * cog:(i + 1) * cog])
+            for i in range(groups)]
 
 
 # --------------------------------------------------------------------------- generic matmul

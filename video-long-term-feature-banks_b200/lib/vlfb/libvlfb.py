@@ -33,7 +33,7 @@ class GemmParams(C.Structure):
                 ('residual', C.c_void_p), ('relu_mask', C.c_void_p), ('flags', C.c_int),
                 ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t),
                 ('engine', C.c_int), ('tile_n', C.c_int), ('pair', C.c_int), ('stream_k', C.c_int),
-                ('relu_mask_bits', C.c_void_p), ('relu_bits_out', C.c_void_p)]
+                ('relu_mask_bits', C.c_void_p), ('relu_bits_out', C.c_void_p), ('groups', C.c_int)]
 
 
 class GemmPlan(C.Structure):
