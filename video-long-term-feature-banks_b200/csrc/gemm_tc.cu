@@ -128,6 +128,11 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm,
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(bar)
       : "memory");
 }
+// Arrive on the mbarrier once every cp.async this thread has issued so far has landed (noinc: the arrival is one of the
+// barrier's expected arrivals), without waiting for them.
+__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
@@ -757,6 +762,13 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
       KLoader<is_mn(BK) ? VLFB_OP_DENSE_K : BK, BN_MAX / RSTEP> kb;
       MNLoader<is_mn(BK) ? BK : VLFB_OP_DENSE_MN> mb;
       const int LAG = L.lag;
+      // Publishing a cp.async chunk.  Both operands MN-major (wgrad): the consumers read the stage tiles only through
+      // their generic-proxy rewrite (mn_to_kmajor), so no proxy fence is needed and each thread's arrival on the stage
+      // barrier is triggered by the completion of its copies (cp.async.mbarrier.arrive): the producers run up to
+      // `stages` chunks ahead of the MMAs.  Otherwise a thread publishes chunk c itself after issuing chunk c + lag
+      // (wait_group, then the proxy fence wgmma's async-proxy reads need).  That ties each publication to a stage the
+      // consumers release, and with lag = stages - 2 producers and consumers take turns chunk by chunk.
+      constexpr bool ASYNC_PUB = CP && is_mn(AK) && is_mn(BK);
       // compile-time gates keep the im2col state out of the instantiations that cannot use it (registers)
       const bool im2col_a = (AK == VLFB_OP_CONV_K || AK == VLFB_OP_DGRAD_K) && L.tma_a == 2;
       const bool im2col_b = BK == VLFB_OP_CONV_MN && L.tma_b == 2;
@@ -993,6 +1005,10 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
             if (is_mn(BK)) mb.issue(p, L.out, ti.k_begin + i * KC, ti.k_end, b_tile);
             else kb.issue(p, kc0 + i, b_tile);
           }
+          if (ASYNC_PUB) {                 // published when its copies land; the producer moves on to the next chunk
+            cp_async_mbar_arrive(fbar);
+            continue;
+          }
           cp_async_commit();
           if (it >= LAG) {
             cp_async_wait_dyn(LAG);
@@ -1004,7 +1020,9 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         if (tid == 0 && witem < 4) TR(9 + 2 * witem);
         ++witem;
       }
-      if (cp_any) {
+      if (ASYNC_PUB) {
+        cp_async_wait<0>();              // (no copy may outlive the CTA's producers)
+      } else if (cp_any) {
         cp_async_wait<0>();
         fence_proxy_async();
         for (int c = (it > LAG ? it - LAG : 0); c < it; ++c) {
