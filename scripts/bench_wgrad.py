@@ -108,7 +108,8 @@ def main():
             rec = runs[name][0][i]['rec'] or {}
             rows.append(dict(label=label, count=count, ms=ms, spread=max(run[i]['ms'] for run in runs[name]) -
                              min(run[i]['ms'] for run in runs[name]), tflops=fl / ms * 1e-9, bound_ms=lb,
-                             co_le_64=co <= 64, rec=dict((k, rec.get(k)) for k in ('bn', 'sk', 'split', 'stages', 'tiles'))))
+                             co_le_64=co <= 64,
+                             rec=dict((k, rec.get(k)) for k in ('bn', 'wide', 'sk', 'split', 'stages', 'tiles'))))
         res[name] = rows
     names = [n for n, _ in libs]
     print('%-34s %3s ' % ('launch', 'n') + ' '.join('%24s' % ('%s ms  TF/s  %%bound' % n) for n in names) +
@@ -117,8 +118,8 @@ def main():
         r0 = res[names[-1]][i]
         cols = ' '.join('%10.3f %6.1f %5.1f%%' % (res[n][i]['ms'], res[n][i]['tflops'], 100 * res[n][i]['bound_ms'] / res[n][i]['ms'])
                         for n in names)
-        print('%-34s %3d %s  bn=%s sk=%s split=%s stages=%s tiles=%s' % (
-            r0['label'], r0['count'], cols, *[r0['rec'][k] for k in ('bn', 'sk', 'split', 'stages', 'tiles')]))
+        print('%-34s %3d %s  bn=%s wide=%s sk=%s split=%s stages=%s tiles=%s' % (
+            r0['label'], r0['count'], cols, *[r0['rec'][k] for k in ('bn', 'wide', 'sk', 'split', 'stages', 'tiles')]))
     for grp, sel in (('Co <= 64', True), ('Co > 64', False)):
         tot = ' '.join('%s %.3f ms' % (n, sum(r['ms'] * r['count'] for r in res[n] if r['co_le_64'] == sel)) for n in names)
         print('per step, %s: %s' % (grp, tot))

@@ -3,14 +3,15 @@
 //   D[m,n] = epi( sum_k A[m,k] * B[n,k] ),  fp32 storage, wgmma tf32 MMA, fp32 accumulate in registers.
 //
 // Persistent kernel: grid = min(#tiles, #SMs), one CTA per SM walks a static sequence of 128 x BN output
-// tiles (BN <= 128):
+// tiles (BN <= 128; 64 x 2 BN "wide" tiles when both operands are MN-major and M <= 64, Launch::wide):
 //   PRODUCERS  -- the A/B K-chunks (32 fp32 = one 128-byte swizzle row) go straight from NDHWC tensors into
 //              swizzled shared-memory tiles, never through an im2col buffer: dense operands by TMA tiled
 //              boxes (SWIZZLE_128B K-major, SWIZZLE_128B_ATOM_32B MN-major), convolution gathers by TMA
 //              im2col copies (conv fwd, unit-stride dgrad, wgrad; one thread issues), and what TMA cannot
 //              express (conv1 stem with 16-byte pixels, strided dgrad, unaligned operands) by 16-byte
 //              cp.async with zero-fill = padding (8 warps; a TMA-only build has one issuing warp of four);
-//   CONSUMERS  -- two warpgroups; warpgroup w issues wgmma.m64nBNk8 for tile rows [64 w, 64 w + 64) and then
+//   CONSUMERS  -- two warpgroups; warpgroup w issues wgmma.m64nBNk8 for tile rows [64 w, 64 w + 64) (wide tiles:
+//              columns [w BN, w BN + BN) of the 64 rows) and then
 //              runs the epilogue of those rows from its registers: smem transpose -> fused affine /
 //              residual / ReLU / TF32 rounding -> coalesced 128-bit global stores (or atomics for split-K).
 // wgmma reads tf32 operands K-major only, so an MN-major stage tile (wgrad, transposed matmul operands) is
@@ -58,6 +59,9 @@ constexpr int EPI_WARP_FLOATS = 16 * EPITCH + EPI_COLV;
 constexpr int EPI_STAGE_BYTES = (NEPI / 32) * EPI_WARP_FLOATS * 4;
 constexpr int A_TILE_BYTES = BM * KC * 4;  // 16 KB
 constexpr int MAX_STAGES = 8;
+constexpr int WM = 64;                     // rows of a wide tile (Launch::wide): one wgmma M
+// a wide launch's K-major images (one WM-row A, two 2 BN-row B) live in the epilogue staging tiles
+static_assert(WM * KC * 4 + 2 * (2 * BN_MAX) * KC * 4 <= EPI_STAGE_BYTES, "wide images must fit the epilogue staging");
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -439,7 +443,8 @@ struct KLoader {
 // consumers rewrite it K-major before the MMAs, mn_to_kmajor).
 template <int KIND>
 struct MNLoader {
-  static constexpr int MAXS = (32 * (BN_MAX / 4)) / NPROD;   // copies per thread per chunk at the widest tile
+  static constexpr int SGRP = (32 * (BN_MAX / 4)) / NPROD;   // copies per thread per chunk at a 128-row tile (the
+                                                             // 256-row B tile of a wide launch takes two groups)
   const float* base;
   int64_t ld;
   int tapz, nslot;
@@ -460,7 +465,7 @@ struct MNLoader {
     if (KIND == VLFB_OP_DENSE_MN) base += (int64_t)batch * op.batch_stride;
     ld = op.ld;
     tapz = tap;
-    const int cpr = rows >> 2;            // 16-byte chunks per k-row (8, 16, 32 or 64)
+    const int cpr = rows >> 2;            // 16-byte chunks per k-row (8, 16, 32 or 64; power of two)
     const int lcpr = 31 - __clz(cpr);
     nslot = (KC * cpr) / NPROD;
     kstep = NPROD >> lcpr;
@@ -514,26 +519,30 @@ struct MNLoader {
     }
     int lane_src = kk0;
     uint32_t d = tile + dst0;
+    // groups of SGRP copies: one pass up to the 128-row tiles, two for a wide launch's 256-row B tile (a body unrolled
+    // over all MAXS copies slows the producers of every MN-major launch)
+    for (int j0 = 0; j0 < nslot; j0 += SGRP) {
 #pragma unroll
-    for (int j = 0; j < MAXS; ++j) {
-      if (j >= nslot) break;
-      bool ok = colok;
-      const float* src = base;
-      if (KIND == VLFB_OP_DENSE_MN) {
-        const int k = k0 + lane_src;
-        ok = ok && k < kend;
-        if (ok) src = base + (int64_t)k * ld + mn;
-      } else {
-        const int ra = __shfl_sync(0xffffffffu, info_a, lane_src);
-        const int rb = __shfl_sync(0xffffffffu, info_b, lane_src);
-        ok = ok && (((rb >> sh) & (rb >> sw) & 1) != 0);
-        if (ok) src = base + (ra + slotoff);
+      for (int j = 0; j < SGRP; ++j) {
+        if (j0 + j >= nslot) break;
+        bool ok = colok;
+        const float* src = base;
+        if (KIND == VLFB_OP_DENSE_MN) {
+          const int k = k0 + lane_src;
+          ok = ok && k < kend;
+          if (ok) src = base + (int64_t)k * ld + mn;
+        } else {
+          const int ra = __shfl_sync(0xffffffffu, info_a, lane_src);
+          const int rb = __shfl_sync(0xffffffffu, info_b, lane_src);
+          ok = ok && (((rb >> sh) & (rb >> sw) & 1) != 0);
+          if (ok) src = base + (ra + slotoff);
+        }
+        // columns beyond the matrix are never copied: whatever shared memory holds there only reaches accumulator
+        // columns >= N, which the epilogue does not store (k tails of real columns ARE zero-filled)
+        if (colok) cp_async16(d, src, ok);
+        lane_src += kstep;
+        d += dstep;
       }
-      // columns beyond the matrix are never copied: whatever shared memory holds there only reaches accumulator
-      // columns >= N, which the epilogue does not store (k tails of real columns ARE zero-filled)
-      if (colok) cp_async16(d, src, ok);
-      lane_src += kstep;
-      d += dstep;
     }
   }
 };
@@ -562,6 +571,11 @@ struct ParCls { short nh, nw, rh, rw, ph, pw; int nk; };   // taps per dim, firs
 
 struct Launch {
   int bn;        // tile N (32/64/96/128) = wgmma N
+  // Wide tiles (both operands MN-major and M <= 64: every wgrad with Co <= 64): a tile is 64 rows x 2 bn columns
+  // instead of 128 x bn, and warpgroup w computes columns [w bn, (w + 1) bn) of the 64 rows, so no warpgroup multiplies
+  // padding rows.  Both warpgroups read one 64-row A image; each reads its half of a 2 bn-row B image.  Staged by the
+  // cp.async loaders only; the K-major images alias the epilogue staging tiles, so bn = 128 keeps 3 stages, bn = 64 six.
+  int wide;
   int stages;
   PosDiv out;    // fast divisors of the conv OUTPUT extents (Wo, Ho, To)
   PosDiv in;     // ... and of the INPUT extents (W, H, T) for the dgrad row decode
@@ -626,7 +640,7 @@ __device__ __forceinline__ void decode_tile(const vlfb_gemm_params_t& p, const L
   ti.batch = (p.taps > 1) ? 0 : zz;
   ti.tap = (p.taps > 1) ? zz : 0;
   ti.m0 = mt * BM;
-  ti.n0 = nt * L.bn;
+  ti.n0 = nt * (L.bn << L.wide);       // (a wide launch has one M tile: m0 = 0)
   int kper = (p.K + split_k - 1) / split_k;
   kper = (kper + KC - 1) / KC * KC;
   ti.k_begin = split * kper;
@@ -710,14 +724,20 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int bn = L.bn, S = L.stages;
   const int bnh = bn;
-  const uint32_t b_tile_bytes = (uint32_t)bn * KC * 4;
-  const uint32_t stage_bytes = A_TILE_BYTES + b_tile_bytes;
   // K-major images of the MN-major operands (wgmma reads tf32 operands K-major only): one for A, two for B (chunk i
   // uses B image i % 2)
   constexpr bool TA = is_mn(AK), TB = is_mn(BK);
-  const uint32_t ka_img = smem_base + S * stage_bytes;
-  const uint32_t kb_img = ka_img + (TA ? (uint32_t)A_TILE_BYTES : 0u);
-  const uint32_t epi_base = kb_img + (TB ? 2 * b_tile_bytes : 0u);      // per-consumer-warp transpose tiles
+  // wide tile (Launch::wide): WM A rows, 2 bn B rows per stage; the images alias the epilogue staging tiles, which are
+  // idle during the K loop (one barrier after the loop's final drain orders the MMAs' reads before the staging stores)
+  const bool wide = CP && TA && TB && L.wide != 0;
+  const int a_rows = wide ? WM : BM, b_rows = bn << (wide ? 1 : 0);
+  const uint32_t a_tile_bytes = (uint32_t)a_rows * KC * 4;
+  const uint32_t b_tile_bytes = (uint32_t)b_rows * KC * 4;
+  const uint32_t stage_bytes = a_tile_bytes + b_tile_bytes;
+  const uint32_t img_base = smem_base + S * stage_bytes;
+  const uint32_t epi_base = img_base + (wide ? 0u : (TA ? a_tile_bytes : 0u) + (TB ? 2 * b_tile_bytes : 0u));   // per-consumer-warp transpose tiles
+  const uint32_t ka_img = wide ? epi_base : img_base;
+  const uint32_t kb_img = ka_img + (TA ? a_tile_bytes : 0u);
   const uint32_t bar_base = epi_base + EPI_STAGE_BYTES;
   const uint32_t full0 = bar_base, empty0 = bar_base + 8 * MAX_STAGES;
 
@@ -796,8 +816,11 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         if (tid == 0 && witem < 4) TR(8 + 2 * witem);
         const int nb0 = ti.n0;                           // first D column whose B rows this CTA stages
         if (cp_any) {
+          // (A is loaded as a 128-row tile also when wide: a compile-time row count keeps the producers' per-chunk issue
+          // loop as short as it was; rows >= M are never copied, and a wide launch has M <= 64, so only its WM-row
+          // A stage tile is written)
           if (!tma_a) { if (is_mn(AK)) ma.init(p, p.a, ti.m0, BM, p.M, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { ka.init(p, p.a, ti.m0, BM, p.M, ti.batch, L.out, L.in, ti.k_begin / KC); ka.kend = ti.k_end; } }
-          if (!tma_b) { if (is_mn(BK)) mb.init(p, p.b, ti.n0, bn, p.N, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { kb.init(p, p.b, ti.n0, bn, p.N, ti.batch, L.out, L.in, ti.k_begin / KC); kb.kend = ti.k_end; } }
+          if (!tma_b) { if (is_mn(BK)) mb.init(p, p.b, ti.n0, b_rows, p.N, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { kb.init(p, p.b, ti.n0, bn, p.N, ti.batch, L.out, L.in, ti.k_begin / KC); kb.kend = ti.k_end; } }
         }
         const int kc0 = ti.k_begin / KC;
         // bytes the stage barrier expects
@@ -885,7 +908,7 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           if (need_wait && (NISS == 1 || hid == 0 || cp_any)) mbar_wait(empty0 + 8 * s_cur, wpar);
           if (++s == S) { s = 0; ph ^= 1u; }
           const uint32_t a_tile = smem_base + s_cur * stage_bytes;
-          const uint32_t b_tile = a_tile + A_TILE_BYTES;
+          const uint32_t b_tile = a_tile + a_tile_bytes;
           const uint32_t fbar = fullx + 8 * s_cur;
           if (issuer && tma_bytes) {
             if (hid == 0) mbar_expect_tx(full0 + 8 * s_cur, tma_bytes);
@@ -1033,29 +1056,26 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
     }
   } else {
     // ============================ CONSUMERS (2 warpgroups: wgmma K loop, then the epilogue) ============================
-    // Warp w of warpgroup g holds accumulator rows [64 g + 16 w, +16) of the tile (wgmma fragment layout).  After the K
+    // Warp w of warpgroup g holds accumulator rows [64 g + 16 w, +16) of the tile (wgmma fragment layout; wide tiles: rows
+    // [16 w, +16) of columns [g bn, (g + 1) bn), so every output element still belongs to one warp).  After the K
     // loop the warp writes them to its padded shared-memory tile (16 x EPITCH), so that the epilogue holds no accumulator
     // registers and a warp store / residual load / atomic covers 8 rows x 64 contiguous bytes (whole 32-byte sectors).
     const int ctid = tid - NPRODT;
-    const int wg = ctid >> 7;
-    const int ew = ctid >> 5;            // consumer warp 0-7 = 4 wg + (warp % 4)
-    const int wrow = 16 * ew;            // its first tile row
+    // (from the broadcast warp index: warp-uniform for the compiler, so the wgmma descriptors, which add the warpgroup's
+    // offset, stay in uniform registers)
+    const int ew = warp - NPWT;          // consumer warp 0-7 = 4 wg + (warp % 4)
+    const int wg = ew >> 2;
+    const int wrow = 16 * (wide ? (ew & 3) : ew);   // its first tile row
+    const int wcol = wide ? wg * bn : 0;            // ... and first tile column (a wide tile's halves: one per warpgroup)
     const int lane = tid & 31;
-    const bool stem_pb = BK == VLFB_OP_STEM_MN && L.tma_b == 3 && L.stem_patch != 0;
+    // (patch chunks stage both operands by TMA: never in a cp.async build)
+    const bool stem_pb = !CP && BK == VLFB_OP_STEM_MN && L.tma_b == 3 && L.stem_patch != 0;
     float* stg = reinterpret_cast<float*>(smem_raw + (epi_base - smem_u32(smem_raw))) + ew * EPI_WARP_FLOATS;
     float* wsc = stg + 16 * EPITCH;      // column scale of the tile's columns, then the bias
     float* wbi = wsc + BN_MAX;
-    int s = 0, sprev = 0;
+    int s = 0;
     uint32_t ph = 0;
     int colv_n0 = -1;
-    const bool vec_ok = ((p.ldd & 3) == 0) && ((p.d_batch_stride & 3) == 0) && ((p.d_tap_stride & 3) == 0) &&
-                        ((reinterpret_cast<uintptr_t>(p.d) & 15) == 0) &&
-                        (!p.residual || (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) &&
-                        (!p.relu_mask || (reinterpret_cast<uintptr_t>(p.relu_mask) & 15) == 0) &&
-                        !(p.residual && (p.flags & VLFB_EPI_ACCUM));
-    const int col = (lane & 3) * 4;
-    const bool want_res = (p.residual != nullptr) || (p.flags & VLFB_EPI_ACCUM);
-    const float* res_src = p.residual ? p.residual : p.d;
     const size_t ws_tile_floats = (size_t)BM * bn;
     int tile_iter = 0;
     Sched sc;
@@ -1073,20 +1093,22 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         // chunk i: at its start this warpgroup's MMAs of chunk i - 2 have completed (the wait<1> that ends chunk i - 1),
         // so B image i % 2, which chunk i - 2 read, may be rewritten once both warpgroups are there; the MMAs of chunk
         // i - 1, which read the other image, stay in flight meanwhile.  The single A image waits for all MMAs.
+        // Wide tile: both warpgroups read the one WM-row A image, warpgroup w rows [w BN, (w + 1) BN) of the B image.
+        const uint32_t a_wg = wide ? 0u : (uint32_t)wg * (64 * 128), b_wg = (uint32_t)wcol * 128;
         for (int i = 0; i < ti.nk; ++i) {
           mbar_wait(full0 + 8 * s, ph);
-          const uint32_t a_tile = smem_base + s * stage_bytes, b_tile = a_tile + A_TILE_BYTES;
-          const uint32_t b_img = kb_img + (uint32_t)((i & 1) * BN * 128);
+          const uint32_t a_tile = smem_base + s * stage_bytes, b_tile = a_tile + a_tile_bytes;
+          const uint32_t b_img = kb_img + (i & 1) * b_tile_bytes;
           if (TA || TB) {
             if (TA) wgmma_wait<0>();             // no MMA still reads the A image
             consumers_sync();                    // both warpgroups are done with chunk i - 2 (TA: i - 1)
-            if (TA) mn_to_kmajor(a_tile, ka_img, BM, 4096, 0, ctid);
-            if (TB) mn_to_kmajor(b_tile, b_img, BN, stem_pb ? 2048 : 4096, stem_pb ? p.g.sH : 0, ctid);
+            if (TA) mn_to_kmajor(a_tile, ka_img, a_rows, 4096, 0, ctid);
+            if (TB) mn_to_kmajor(b_tile, b_img, b_rows, stem_pb ? 2048 : 4096, stem_pb ? p.g.sH : 0, ctid);
             fence_proxy_async();                 // generic-proxy writes -> visible to the wgmma (async proxy) reads
             consumers_sync();                    // images complete
           }
-          const uint32_t a_src = (TA ? ka_img : a_tile) + (uint32_t)wg * (64 * 128);
-          const uint32_t b_src = TB ? b_img : b_tile;
+          const uint32_t a_src = (TA ? ka_img : a_tile) + a_wg;
+          const uint32_t b_src = (TB ? b_img : b_tile) + b_wg;
           wgmma_fence();
 #pragma unroll
           for (int j = 0; j < KC / 8; ++j)      // wgmma K = 8 for tf32: 32 bytes along the swizzled 128-byte rows
@@ -1094,15 +1116,17 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           wgmma_commit();
           if (i > 0) {
             wgmma_wait<1>();
-            if ((ctid & 127) == 0) mbar_arrive(empty0 + 8 * sprev);
+            if ((ctid & 127) == 0) mbar_arrive(empty0 + 8 * ((s == 0 ? S : s) - 1));   // chunk i - 1's stage
           }
-          sprev = s;
           if (++s == S) { s = 0; ph ^= 1u; }
         }
         // unconditional: a path that skips this wait (nk == 0) would let ptxas see accumulators in flight after the
         // loop, and it then serialises every wgmma of the kernel
         wgmma_wait<0>();
-        if (ti.nk > 0 && (ctid & 127) == 0) mbar_arrive(empty0 + 8 * sprev);
+        if (ti.nk > 0 && (ctid & 127) == 0) mbar_arrive(empty0 + 8 * ((s == 0 ? S : s) - 1));   // the last chunk's stage
+        // wide: the staging tiles below are the images the other warpgroup's MMAs may still read.  (The next tile's
+        // first chunk barrier orders this epilogue before the next rewrite.)
+        if (wide) consumers_sync();
         // fragment (n8 group j: rows lane / 4 and lane / 4 + 8, columns 8 j + 2 (lane % 4) + {0, 1}) -> stg
         float* r = stg + (lane >> 2) * EPITCH + 2 * (lane & 3);
 #pragma unroll
@@ -1118,6 +1142,15 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         case 96: mma_tile(std::integral_constant<int, 96>{}); break;
         default: mma_tile(std::integral_constant<int, 128>{}); break;
       }
+      // epilogue switches, read per tile (kernel parameters) rather than held in registers through the K loop
+      const bool vec_ok = ((p.ldd & 3) == 0) && ((p.d_batch_stride & 3) == 0) && ((p.d_tap_stride & 3) == 0) &&
+                          ((reinterpret_cast<uintptr_t>(p.d) & 15) == 0) &&
+                          (!p.residual || (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) &&
+                          (!p.relu_mask || (reinterpret_cast<uintptr_t>(p.relu_mask) & 15) == 0) &&
+                          !(p.residual && (p.flags & VLFB_EPI_ACCUM));
+      const int col = (lane & 3) * 4;
+      const bool want_res = (p.residual != nullptr) || (p.flags & VLFB_EPI_ACCUM);
+      const float* res_src = p.residual ? p.residual : p.d;
       if (ew == 0 && lane == 0 && tile_iter < 4) TR(24 + 4 * tile_iter);
       const bool par = AK == VLFB_OP_DGRAD_K && L.par != 0;
       const int64_t tile_off = par ? 0 : (int64_t)ti.batch * p.d_batch_stride + (int64_t)ti.tap * p.d_tap_stride;
@@ -1127,8 +1160,8 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         TileInfo tn;
         if (sched_next(p, L, sn, unit, nunits, tn) && tn.npieces() == 1) {
           const int64_t noff = (int64_t)tn.batch * p.d_batch_stride + (int64_t)tn.tap * p.d_tap_stride;
-          const int segs = bn >> 5;
-          for (int idx = ctid; idx < BM * segs; idx += NEPI) {
+          const int segs = b_rows >> 5;
+          for (int idx = ctid; idx < a_rows * segs; idx += NEPI) {
             const int row = idx / segs, seg = idx - row * segs;
             const int m = tn.m0 + row, n = tn.n0 + seg * 32;
             if (m < p.M && n < p.N) {
@@ -1138,12 +1171,14 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           }
         }
       }
-      if (ti.n0 != colv_n0) {
+      const int n0w = ti.n0 + wcol;      // first D column of this warp's accumulator
+      if (wide || ti.n0 != colv_n0) {
         // per-column affine of this warp's blocks -> shared memory, once per N tile (not per block: the
-        // global-load latency used to sit in front of every block's first FFMA)
+        // global-load latency used to sit in front of every block's first FFMA); every tile when wide (the K loop's
+        // images overwrite it)
         colv_n0 = ti.n0;
         for (int i = lane; i < bn; i += 32) {
-          const int n = ti.n0 + i;
+          const int n = n0w + i;
           wsc[i] = (p.col_scale && n < p.N) ? p.col_scale[n] : 1.f;
           wbi[i] = (p.col_bias && n < p.N) ? p.col_bias[n] : 0.f;
         }
@@ -1165,7 +1200,7 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         // 8 epilogue warps per SM the loads must be in flight while the previous block is stored, otherwise the
         // epilogue is DRAM-latency bound (Little's law) instead of bandwidth bound
         auto load_res = [&](int c0, float4* r) {
-          const int n = ti.n0 + c0 + col;
+          const int n = n0w + c0 + col;
           const bool ok = wres && vec_ok && c0 < bn && n + 3 < p.N;
 #pragma unroll
           for (int i = 0; i < EROWS; ++i) {
@@ -1178,7 +1213,7 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         // the residual, but AFTER the accumulator block has left the registers and packed to 16 bits as soon as
         // it arrives, so that it never coexists with both residual buffers (register budget).
         auto load_mask = [&](int c0, float4* mk) {
-          const int n = ti.n0 + c0 + col;
+          const int n = n0w + c0 + col;
           const bool ok = mode != 1 && vec_ok && c0 < bn && n + 3 < p.N;
 #pragma unroll
           for (int i = 0; i < EROWS; ++i) {
@@ -1214,12 +1249,12 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         float4 rr[EROWS], rn[EROWS];
         if (DB) load_res(0, rr);          // independent of the accumulator: issued before the wait
         for (int c0 = 0; c0 < bn; c0 += EPC) {
-          if (ti.n0 + c0 >= p.N) break;            // warp-uniform
+          if (n0w + c0 >= p.N) break;              // warp-uniform (a wide tile's half past N: no block)
           if (DB) load_res(c0 + EPC, rn);
           else load_res(c0, rr);                   // L2-resident (tile-ahead prefetch)
           float4 mk[EROWS];
           if (MASK) load_mask(c0 + EPC, mk);
-          const int n = ti.n0 + c0 + col;
+          const int n = n0w + c0 + col;
           const bool nfull = n + 3 < p.N;
           const int cvi = c0 + col;
           const float4 cs = *reinterpret_cast<const float4*>(wsc + cvi);
@@ -1667,12 +1702,22 @@ static const Env& env() {
 // A K chunk (32 fp32 of K) of a 128 x bn tile costs max(tensor pipe, operand delivery):
 //   tensor   = 128 x bn x 32 MACs / 1024 tf32 MAC/clk (dense H100 SM) = 4 bn clocks;
 //   delivery = (128 + bn) x 128 B through the SM's L2 port at a model rate of 64 B/clk.
+// A wide chunk (64 x 2 bn, Launch::wide) issues the MMAs of a 128 x bn one and delivers (64 + 2 bn) x 128 B, plus a
+// fixed latency the two terms leave out: the consumers' rewrite of the stage tiles between two 256-thread barriers.
+// (Fitted to the Co = 64 wgrads of the benchmarked network, that term is worth 20-200 model clocks; with it a wide
+// launch takes the wider tile when both widths pad N alike.)
 // A tile adds a fixed fill + epilogue cost (~8 chunks' worth); a stream-K launch adds the fix-up of the shared tiles.
 // The constants rank tile widths against each other; they are model values, not measurements.
-static double chunk_cost(int bn) {
+static double chunk_cost(int bn, bool wide) {
   const double tensor = 4.0 * bn;
-  const double port = (16384.0 + 128.0 * bn) / 64.0;
-  return tensor > port ? tensor : port;
+  const double port = (wide ? 128.0 * (WM + 2 * bn) : 16384.0 + 128.0 * bn) / 64.0;
+  return (tensor > port ? tensor : port) + (wide ? 128.0 : 0.0);
+}
+
+// Wide tiles: both operands MN-major (their K-major images are built by the consumers, so the tile shape is free) and
+// at most one wgmma M of rows.
+static bool wide_tiles(const vlfb_gemm_params_t& p) {
+  return is_mn(p.a.kind) && is_mn(p.b.kind) && p.M <= WM;
 }
 
 struct Plan { int bn, split_k, pair, sk; int tiles, units; double cost; };
@@ -1694,14 +1739,16 @@ static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool
   // Stream-K is opt-in (p.stream_k = 1, VLFB_SK): its fix-up pass costs more than it saves unless the tile count
   // leaves many SMs idle.
   const int U = num_sms;
+  const bool wide = wide_tiles(p);
   for (int wi = 0; wi < 4; ++wi) {
     const int bn = kWidths[wi];
+    const int tn = wide ? 2 * bn : bn;                                          // tile columns
     if (want_bn > 0 ? bn != want_bn : ((bn & (bn - 1)) != 0)) continue;       // 96 only on request
-    if (want_bn <= 0 && bn > 32 && p.N <= bn / 2) continue;                   // do not pad N by 2x
-    const int tiles_m = ceil_div(p.M, BM);
-    const int64_t T = (int64_t)tiles_m * ceil_div(p.N, bn) * zbase;
+    if (want_bn <= 0 && bn > 32 && p.N <= tn / 2) continue;                   // do not pad N by 2x
+    const int tiles_m = wide ? 1 : ceil_div(p.M, BM);
+    const int64_t T = (int64_t)tiles_m * ceil_div(p.N, tn) * zbase;
     const int nkt = ceil_div(p.K, KC);
-    const double cc = chunk_cost(bn);
+    const double cc = chunk_cost(bn, wide);
     const double fixed = 8.0 * cc;
     // (a) static tile loop, optional plain split-K (atomic epilogues only)
     const int smax = p.split_k > 0 ? p.split_k : (atomic && p.K >= 512 ? (p.K / 256 < 128 ? p.K / 256 : 128) : 1);
@@ -1846,6 +1893,7 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       sk_ws = false;
     }
   }
+  L.wide = wide_tiles(p) ? 1 : 0;
   Plan plan;
   bool pow2_only = false;
   for (int attempt = 0; attempt < 4; ++attempt) {
@@ -1936,17 +1984,26 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
           make_tmap_conv_flat(&tmB, p.b.ptr, g, bnh / 32))
         L.tma_b = 5;
     }
+    if (L.wide) {
+      // wide tiles are staged by the cp.async loaders: the MN-major tensor maps' boxes are sized for 128 x bn tiles
+      // (and sm_90a does not encode their SWIZZLE_128B_ATOM_32B pattern)
+      L.tma_a = L.tma_b = 0;
+      L.stem_patch = 0;
+    }
     if (is_mn(BK) && !L.tma_b && (L.bn & (L.bn - 1)) && !pow2_only) { pow2_only = true; continue; }
     const bool fixup = plan.sk && !(p.flags & VLFB_EPI_ATOMIC);
     if (!fixup || (L.tma_a && L.tma_b)) break;
     sk_ws = false;                     // an operand fell back to cp.async: plan again without fix-ups
   }
   const int zbase = L.par ? L.par : (p.taps > 1 ? p.taps : p.batch);
-  L.tiles_m = ceil_div(L.par ? L.par_m : p.M, BM);
-  L.tiles_n = ceil_div(p.N, L.bn);
+  L.tiles_m = L.wide ? 1 : ceil_div(L.par ? L.par_m : p.M, BM);
+  L.tiles_n = ceil_div(p.N, L.bn << L.wide);
   L.total_tiles = (int)((int64_t)L.tiles_m * L.tiles_n * zbase * p.split_k);
-  const int stage_bytes = A_TILE_BYTES + L.bn * KC * 4;
-  const int img_bytes = (is_mn(AK) ? A_TILE_BYTES : 0) + (is_mn(BK) ? 2 * L.bn * KC * 4 : 0);   // K-major images: A, 2 x B
+  // (the kernel computes the same stage layout)
+  const int a_tile_bytes = (L.wide ? WM : BM) * KC * 4, b_tile_bytes = (L.bn << L.wide) * KC * 4;
+  const int stage_bytes = a_tile_bytes + b_tile_bytes;
+  // K-major images: A, 2 x B; a wide launch keeps them in the epilogue staging tiles
+  const int img_bytes = L.wide ? 0 : (is_mn(AK) ? a_tile_bytes : 0) + (is_mn(BK) ? 2 * b_tile_bytes : 0);
   L.stages = (227 * 1024 - EPI_STAGE_BYTES - img_bytes - 2048) / stage_bytes;
   if (L.stages > 6) L.stages = 6;
   if (ev.stages >= 3 && ev.stages <= L.stages) L.stages = ev.stages;
@@ -1986,9 +2043,10 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   // VLFB_DEBUG: one record per launch, space-separated key=value (tests/gemm_paths.py parses it; keep the keys stable)
   if (ev.debug)
     fprintf(stderr, "vlfb gemm_tc: kinds=%d,%d mask=%d M=%d N=%d K=%d z=%d bn=%d sk=%d split=%d tiles=%d units=%d stages=%d "
-            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d\n",
+            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d wide=%d\n",
             AK, BK, MASK ? 1 : 0, p.M, p.N, p.K, zbase, L.bn, L.sk, p.split_k, L.total_tiles, units, L.stages, L.lag, L.tma_a,
-            L.tma_b, cap, L.stem_patch, L.par, cp ? 1 : 0, L.ws_tiles != nullptr ? 1 : 0, lean ? 1 : 0, bits_after ? 1 : 0);
+            L.tma_b, cap, L.stem_patch, L.par, cp ? 1 : 0, L.ws_tiles != nullptr ? 1 : 0, lean ? 1 : 0, bits_after ? 1 : 0,
+            L.wide);
   int rc = VLFB_OK;
   if (cp) rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);     // (fix-ups are planned for TMA-fed launches only)
   else if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
