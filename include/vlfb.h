@@ -127,11 +127,22 @@ typedef struct {
    * fwd / dgrad take every epilogue field except VLFB_EPI_ATOMIC, with ldd % 4 == 0 and 16-byte aligned d / residual /
    * relu_mask.  batch and split_k must be 1 (split_k 0 is accepted as 1).  vlfb_gemm_plan returns VLFB_E_UNSUPPORTED. */
   int groups;
+  /* ---- deterministic accumulation ----
+   * 0: as above.  1, with VLFB_EPI_ATOMIC: no element of d receives more than one contribution during the launch, so
+   * the result is bitwise reproducible (same inputs, same d, same GPU model and library build).  The library picks
+   * split 1, or stream-K whose pieces meet in the workspace and are summed in piece order by the last unit to arrive,
+   * which then applies d += epi(sum) once (alpha, col_scale, col_bias, row_scale and the TF32 rounding as in the
+   * atomic form).  split_k must be 0 or 1, and workspace / workspace_bytes must hold >= vlfb_gemm_workspace_bytes()
+   * (VLFB_E_WORKSPACE otherwise).  groups > 1 (wgrad): each position split writes its partial dw to the workspace's
+   * partial-tile area and a second pass adds them to d in split order.  SIMT engine: split 1 (each element is then
+   * written by one thread).  Without VLFB_EPI_ATOMIC every element is stored once anyway and the field changes nothing. */
+  int deterministic;
 } vlfb_gemm_params_t;
 
 enum { VLFB_ENGINE_TCGEN05 = 0, VLFB_ENGINE_SIMT = 1 };
 
-/* What vlfb_gemm would do for `p` (host-only, no launch; not defined for groups > 1). */
+/* What vlfb_gemm would do for `p` (host-only, no launch; not defined for groups > 1).  With p->deterministic and
+ * VLFB_EPI_ATOMIC, split_k is 1 and stream_k = 1 only when the workspace fields allow the fix-up. */
 typedef struct {
   int tile_n;                 /* output-tile width */
   int split_k;                /* plain split-K factor (atomic epilogues) */
@@ -373,4 +384,5 @@ int vlfb_lfb_gather(const float* bank, int64_t bank_rows, const int32_t* idx, fl
 #ifdef __cplusplus
 }
 #endif
+#include "vlfb_det.h"
 #endif /* VLFB_H_ */

@@ -28,7 +28,10 @@ static int validate_gemm(const vlfb_gemm_params_t& p, bool& tc_ok) {
   VLFB_CHECK_ARG(p.engine == VLFB_ENGINE_TCGEN05 || p.engine == VLFB_ENGINE_SIMT);
   VLFB_CHECK_ARG(p.tile_n == 0 || (p.tile_n >= 32 && p.tile_n <= 256 && p.tile_n % 32 == 0));
   VLFB_CHECK_ARG(p.split_k == 1 || (p.flags & VLFB_EPI_ATOMIC));
-  VLFB_CHECK_ARG(!(p.split_k != 1 && (p.residual || p.relu_mask || p.relu_mask_bits || (p.flags & (VLFB_EPI_RELU | VLFB_EPI_TF32)))));
+  VLFB_CHECK_ARG(p.deterministic == 0 || p.deterministic == 1);
+  VLFB_CHECK_ARG(!(p.deterministic && p.split_k > 1));   // a deterministic launch is never split (split_k 0 = 1)
+  const bool split = p.deterministic ? p.split_k > 1 : p.split_k != 1;
+  VLFB_CHECK_ARG(!(split && (p.residual || p.relu_mask || p.relu_mask_bits || (p.flags & (VLFB_EPI_RELU | VLFB_EPI_TF32)))));
   VLFB_CHECK_ARG(!(p.relu_mask && p.relu_mask_bits));
   if (p.relu_bits_out) {
     if (!((p.flags & VLFB_EPI_RELU) && !(p.flags & VLFB_EPI_ATOMIC) && p.split_k == 1 && p.batch == 1 && p.taps == 1 &&
@@ -103,6 +106,7 @@ static int validate_gconv(const vlfb_gemm_params_t& p) {
   const int G = p.groups;
   VLFB_CHECK_ARG(p.a.ptr && p.b.ptr && p.d);
   VLFB_CHECK_ARG(p.M > 0 && p.N > 0 && p.K > 0);
+  VLFB_CHECK_ARG(p.deterministic == 0 || p.deterministic == 1);
   GCONV_REQUIRE(p.batch == 1, VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 needs batch == 1");
   GCONV_REQUIRE(p.split_k == 0 || p.split_k == 1, VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 needs split_k <= 1");
   GCONV_REQUIRE(p.a.kind != VLFB_OP_STEM_K && p.a.kind != VLFB_OP_STEM_MN && p.b.kind != VLFB_OP_STEM_K &&
@@ -193,6 +197,12 @@ int vlfb_debug_set_trace(void* buf) { vlfb::gemm_tc_set_trace(buf); return VLFB_
 int vlfb_gemm(const vlfb_gemm_params_t* p, void* stream) {
   VLFB_CHECK_ARG(p != nullptr);
   VLFB_CHECK_ARG(p->groups >= 0);
+  if (p->deterministic && (p->flags & VLFB_EPI_ATOMIC) &&
+      !(p->workspace && p->workspace_bytes >= gemm_tc_workspace_bytes() && (reinterpret_cast<uintptr_t>(p->workspace) & 15) == 0)) {
+    set_error("vlfb_gemm: a deterministic VLFB_EPI_ATOMIC launch needs a 16-byte aligned workspace of >= %zu bytes",
+              gemm_tc_workspace_bytes());
+    return VLFB_E_WORKSPACE;
+  }
   if (p->groups > 1) {                 // Caffe2 grouped Conv: CUDA-core kernels, `engine` does not apply
     const int rc = validate_gconv(*p);
     return rc != VLFB_OK ? rc : gconv(*p, static_cast<cudaStream_t>(stream));

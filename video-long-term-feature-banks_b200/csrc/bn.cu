@@ -142,9 +142,11 @@ inline Ws carve(void* workspace, int C) {
   w.f2 = w.f1 + C;
   return w;
 }
-inline void reduce_dims(int64_t rows, int C, dim3* grid, int64_t* rpb) {
+// det: one slab (block) per 32-channel strip, so each accumulator receives a single atomicAdd onto its zero: the sums are
+// reproducible bit for bit (the deterministic entry points of include/vlfb_det.h)
+inline void reduce_dims(int64_t rows, int C, dim3* grid, int64_t* rpb, bool det = false) {
   const int cb = ceil_div(C, 32);
-  int slabs = (4 * 132 + cb - 1) / cb;                      // ~4 blocks of 256 threads per SM
+  int slabs = det ? 1 : (4 * 132 + cb - 1) / cb;            // ~4 blocks of 256 threads per SM
   const int64_t max_slabs = (rows + 127) / 128;
   if (slabs > max_slabs) slabs = (int)max_slabs;
   if (slabs < 1) slabs = 1;
@@ -162,9 +164,9 @@ extern "C" {
 
 size_t vlfb_spatial_bn_workspace_bytes(int C) { return C > 0 ? (size_t)C * 28 + 32 : 0; }
 
-int vlfb_spatial_bn_fwd(const float* x, const float* scale, const float* bias, float* running_mean, float* running_var,
-                        float* saved_mean, float* saved_inv_std, float* y, int64_t rows, int C, float eps, float momentum,
-                        void* workspace, size_t workspace_bytes, void* stream) {
+static int spatial_bn_fwd(const float* x, const float* scale, const float* bias, float* running_mean, float* running_var,
+                          float* saved_mean, float* saved_inv_std, float* y, int64_t rows, int C, float eps, float momentum,
+                          void* workspace, size_t workspace_bytes, void* stream, bool det) {
   VLFB_CHECK_ARG(x && scale && bias && saved_mean && saved_inv_std && y && rows > 0 && C > 0 && (C & 3) == 0);
   VLFB_CHECK_ARG((running_mean == nullptr) == (running_var == nullptr));
   VLFB_CHECK_ARG(workspace && workspace_bytes >= vlfb_spatial_bn_workspace_bytes(C) &&
@@ -176,7 +178,7 @@ int vlfb_spatial_bn_fwd(const float* x, const float* scale, const float* bias, f
   }
   dim3 grid;
   int64_t rpb;
-  reduce_dims(rows, C, &grid, &rpb);
+  reduce_dims(rows, C, &grid, &rpb, det);
   launch_k(bn_reduce_k<0>, grid, dim3(32, 8), 0, ST(stream), x, (const float*)nullptr, x, rows, C, rpb, w.acc);
   VLFB_CHECK_LAUNCH();
   launch_k(bn_finalize_fwd_k, dim3(ceil_div(C, 128)), dim3(128), 0, ST(stream), (const double*)w.acc, x, rows, C, eps, momentum,
@@ -206,9 +208,9 @@ int vlfb_spatial_bn_infer(const float* x, const float* scale, const float* bias,
   return VLFB_OK;
 }
 
-int vlfb_spatial_bn_bwd(const float* dy, const float* x, const float* scale, const float* saved_mean,
-                        const float* saved_inv_std, float* dx, float* dscale, float* dbias, int64_t rows, int C,
-                        void* workspace, size_t workspace_bytes, void* stream) {
+static int spatial_bn_bwd(const float* dy, const float* x, const float* scale, const float* saved_mean,
+                          const float* saved_inv_std, float* dx, float* dscale, float* dbias, int64_t rows, int C,
+                          void* workspace, size_t workspace_bytes, void* stream, bool det) {
   VLFB_CHECK_ARG(dy && x && scale && saved_mean && saved_inv_std && dx && rows > 0 && C > 0 && (C & 3) == 0);
   VLFB_CHECK_ARG(workspace && workspace_bytes >= vlfb_spatial_bn_workspace_bytes(C) &&
                  (reinterpret_cast<uintptr_t>(workspace) & 15) == 0);
@@ -219,7 +221,7 @@ int vlfb_spatial_bn_bwd(const float* dy, const float* x, const float* scale, con
   }
   dim3 grid;
   int64_t rpb;
-  reduce_dims(rows, C, &grid, &rpb);
+  reduce_dims(rows, C, &grid, &rpb, det);
   launch_k(bn_reduce_k<1>, grid, dim3(32, 8), 0, ST(stream), dy, x, saved_mean, rows, C, rpb, w.acc);
   VLFB_CHECK_LAUNCH();
   launch_k(bn_finalize_bwd_k, dim3(ceil_div(C, 128)), dim3(128), 0, ST(stream), (const double*)w.acc, rows, C, scale, saved_mean,
@@ -230,6 +232,38 @@ int vlfb_spatial_bn_bwd(const float* dy, const float* x, const float* scale, con
            (const float4*)w.f0, (const float4*)x, (const float4*)w.f1, (const float4*)w.f2, (float4*)dx, n4, C >> 2);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
+}
+
+}  // extern "C"
+
+extern "C" {
+
+int vlfb_spatial_bn_fwd(const float* x, const float* scale, const float* bias, float* running_mean, float* running_var,
+                        float* saved_mean, float* saved_inv_std, float* y, int64_t rows, int C, float eps, float momentum,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  return spatial_bn_fwd(x, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, y, rows, C, eps, momentum,
+                        workspace, workspace_bytes, stream, false);
+}
+
+int vlfb_spatial_bn_bwd(const float* dy, const float* x, const float* scale, const float* saved_mean,
+                        const float* saved_inv_std, float* dx, float* dscale, float* dbias, int64_t rows, int C,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  return spatial_bn_bwd(dy, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, C, workspace, workspace_bytes,
+                        stream, false);
+}
+
+int vlfb_spatial_bn_fwd_det(const float* x, const float* scale, const float* bias, float* running_mean, float* running_var,
+                            float* saved_mean, float* saved_inv_std, float* y, int64_t rows, int C, float eps,
+                            float momentum, void* workspace, size_t workspace_bytes, void* stream) {
+  return spatial_bn_fwd(x, scale, bias, running_mean, running_var, saved_mean, saved_inv_std, y, rows, C, eps, momentum,
+                        workspace, workspace_bytes, stream, true);
+}
+
+int vlfb_spatial_bn_bwd_det(const float* dy, const float* x, const float* scale, const float* saved_mean,
+                            const float* saved_inv_std, float* dx, float* dscale, float* dbias, int64_t rows, int C,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  return spatial_bn_bwd(dy, x, scale, saved_mean, saved_inv_std, dx, dscale, dbias, rows, C, workspace, workspace_bytes,
+                        stream, true);
 }
 
 }  // extern "C"

@@ -154,6 +154,9 @@ int gemm_tc(const vlfb_gemm_params_t& p, cudaStream_t stream);
 int gconv(const vlfb_gemm_params_t& p, cudaStream_t stream);                       // groups > 1 (gconv.cu)
 void gemm_tc_plan(const vlfb_gemm_params_t& p, int num_sms, vlfb_gemm_plan_t* out);
 size_t gemm_tc_workspace_bytes();
+// the partial-tile area of a vlfb_gemm workspace (never its arrival counters): other deterministic reductions keep their
+// partial sums there; *floats = its capacity
+float* gemm_tc_partials(void* workspace, size_t workspace_bytes, size_t* floats);
 #ifdef VLFB_TRACE
 void gemm_tc_set_trace(void* buf);
 #endif

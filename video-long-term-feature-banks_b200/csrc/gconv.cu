@@ -214,6 +214,7 @@ struct GwGeom {
   int units;               // (Co / 4) * ceil(pairs / GW_PAIRS)
   int per_cta;             // output positions per CTA
   int K;                   // output positions
+  float* part;             // deterministic form: [CTA column][kT][Co][N] partial dw slabs, or nullptr (red.global.add)
 };
 
 __global__ void __launch_bounds__(GC_THREADS, 2) gconv_wgrad_kernel(const vlfb_gemm_params_t p, const GwGeom g) {
@@ -289,10 +290,27 @@ __global__ void __launch_bounds__(GC_THREADS, 2) gconv_wgrad_kernel(const vlfb_g
         float v = acc[s][a][b] * p.alpha;
         if (p.col_scale) v *= __ldg(p.col_scale + n);
         v *= rs;
+        if (g.part) {
+          g.part[(((int64_t)blockIdx.x * g.kT + kt) * g.Co + co + a) * p.N + n] = v;
+          continue;
+        }
         float* dst = p.d + (int64_t)kt * p.d_tap_stride + (int64_t)(co + a) * p.ldd + n;
         asm volatile("red.global.add.f32 [%0], %1;" ::"l"(dst), "f"(v) : "memory");
       }
     }
+  }
+}
+
+// deterministic grouped wgrad, second pass: dw[kt][co][n] += sum of the `splits` partial slabs in split order
+__global__ void gconv_wgrad_sum_k(const vlfb_gemm_params_t p, const float* __restrict__ part, int kT, int splits) {
+  const int64_t slab = (int64_t)kT * p.M * p.N;
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < slab; e += (int64_t)gridDim.x * blockDim.x) {
+    float v = 0.f;
+    for (int s = 0; s < splits; ++s) v += part[s * slab + e];
+    const int n = (int)(e % p.N);
+    const int64_t r = e / p.N;
+    const int co = (int)(r % p.M), kt = (int)(r / p.M);
+    p.d[(int64_t)kt * p.d_tap_stride + (int64_t)co * p.ldd + n] += v;
   }
 }
 
@@ -308,6 +326,7 @@ int gconv(const vlfb_gemm_params_t& p, cudaStream_t stream) {
   const int G = p.groups, Cig = c.C / G, Cog = c.Co / G;
   const bool dgrad = p.a.kind == VLFB_OP_DGRAD_K, wgrad = p.a.kind == VLFB_OP_DENSE_MN;
   dim3 grid;
+  unsigned slabs = 0;                  // deterministic grouped wgrad: partial dw slabs summed by gconv_wgrad_sum_k
   if (wgrad) {
     GwGeom w;
     w.T = c.T; w.H = c.H; w.W = c.W; w.C = c.C; w.To = c.To; w.Ho = c.Ho; w.Wo = c.Wo; w.Co = c.Co;
@@ -322,14 +341,31 @@ int gconv(const vlfb_gemm_params_t& p, cudaStream_t stream) {
     // Positions are split until about 4 CTAs' worth of threads per SM are in flight (fewer splits = fewer atomics),
     // with at least 32 positions per CTA.  gy <= 65535 holds for every valid shape (Co <= 2^31 / positions).
     const int64_t want = (132LL * 4 * GC_THREADS) / ((int64_t)gy * block);
-    const int64_t splits = std::max<int64_t>(1, std::min<int64_t>(want, ceil_div(w.K, 32)));
+    int64_t splits = std::max<int64_t>(1, std::min<int64_t>(want, ceil_div(w.K, 32)));
+    // deterministic: the partial slabs live in the partial-tile area of the GEMM workspace (api.cu checked its size);
+    // as many splits as slabs fit there, and one split writes dw directly
+    const int64_t slab = (int64_t)c.kT * p.M * p.N;
+    float* part = nullptr;
+    size_t part_floats = 0;
+    if (p.deterministic) {
+      part = gemm_tc_partials(p.workspace, p.workspace_bytes, &part_floats);
+      splits = std::min<int64_t>(splits, (int64_t)(part_floats / (size_t)slab));
+      if (splits < 2) { splits = 1; part = nullptr; }
+    }
     w.per_cta = ceil_div(w.K, splits);
+    w.part = part;
     grid = dim3(ceil_div(w.K, w.per_cta), gy, 1);
     if (gy > 65535) {
       set_error("vlfb_gemm: grouped wgrad with %d output-channel units needs more than 65535 CTA rows", w.units);
       return VLFB_E_UNSUPPORTED;
     }
     launch_k(gconv_wgrad_kernel, grid, block, 0, stream, p, w);
+    if (part) {
+      slabs = grid.x;
+      VLFB_CHECK_LAUNCH();
+      launch_k(gconv_wgrad_sum_k, dim3((unsigned)std::min<int64_t>(ceil_div(slab, 256), 132 * 8)), 256, 0, stream, p,
+               (const float*)part, c.kT, (int)grid.x);
+    }
   } else {
     GconvGeom g;
     if (dgrad) {
@@ -352,8 +388,9 @@ int gconv(const vlfb_gemm_params_t& p, cudaStream_t stream) {
   }
   // VLFB_DEBUG: one record per launch, space-separated key=value like gemm_tc's (tests/gconv_cases.py parses it)
   if (debug_on())
-    fprintf(stderr, "vlfb gconv: path=gconv dir=%s groups=%d cig=%d cog=%d M=%d N=%d K=%d grid=%u,%u,%u\n",
-            wgrad ? "wgrad" : (dgrad ? "dgrad" : "fwd"), G, Cig, Cog, p.M, p.N, p.K, grid.x, grid.y, grid.z);
+    fprintf(stderr, "vlfb gconv: path=gconv dir=%s groups=%d cig=%d cog=%d M=%d N=%d K=%d grid=%u,%u,%u det=%d slabs=%u\n",
+            wgrad ? "wgrad" : (dgrad ? "dgrad" : "fwd"), G, Cig, Cog, p.M, p.N, p.K, grid.x, grid.y, grid.z,
+            p.deterministic ? 1 : 0, slabs);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }

@@ -57,6 +57,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const vlfb_gemm_params_t
 int gemm_simt(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   vlfb_gemm_params_t p = p_in;
   if (p.split_k == 0) p.split_k = p.K >= 2048 ? (p.K / 1024 < 32 ? p.K / 1024 : 32) : 1;   // "library's choice"
+  if (p.deterministic) p.split_k = 1;     // one thread per element: a single (atomic) store each
   dim3 grid(ceil_div(p.M, TM), ceil_div(p.N, TN), (p.taps > 1 ? p.taps : p.batch) * p.split_k);
   launch_k(gemm_simt_kernel, grid, 256, 0, stream, p);
   VLFB_CHECK_LAUNCH();

@@ -1480,8 +1480,22 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         else if (!MASK && p.relu_bits_out != nullptr) { if (want_res) run_fast(mode_c, F{}, T{}, T{}); else run_fast(mode_c, F{}, F{}, T{}); }
         else { if (want_res) run_fast(mode_c, F{}, T{}, F{}); else run_fast(mode_c, F{}, F{}, F{}); }
       };
-      // (the 17-warp cp.async builds never take the fix-up path: the host plans stream-K fix-ups for TMA-fed launches only)
-      const bool split_tile = FIX && !CP && ti.npieces() > 1;
+      // (cp.async builds take the fix-up path only in the MN x MN instantiations of deterministic atomic launches)
+      const bool split_tile = FIX && ti.npieces() > 1;
+      // cp.async fix-up, first half: a piece is this warp's raw staging rows, copied to its slot (tile row r at r * tile
+      // columns + column, so a wide tile's two warpgroups fill their own column halves).  gemm_fixup_kernel, launched
+      // after this kernel, sums the slots of every shared tile in piece order and applies the epilogue once.  (The
+      // in-kernel reduction of the TMA builds does not fit these 128-register builds without spills.)
+      auto cp_piece = [&]() {
+        const int bq = bn >> 2, tcols = bn << (wide ? 1 : 0);
+        float* slot = L.ws_tiles + (size_t)(unit * 2 + ti.slot()) * (BM * bn);
+        for (int idx = lane; idx < 16 * bq; idx += 32) {
+          const int r = idx / bq, c = (idx - r * bq) * 4;
+          *reinterpret_cast<float4*>(slot + (size_t)(wrow + r) * tcols + wcol + c) =
+              *reinterpret_cast<const float4*>(stg + r * EPITCH + c);
+        }
+        __syncwarp();
+      };
       // (MASK builds: the lean path reads the mask as sign bits; a float mask takes the general path)
       const bool bits_ok = (p.ldd & 15) == 0 && (p.d_batch_stride & 15) == 0 && (p.d_tap_stride & 15) == 0;
       const bool fast_tile = !CP && vec_ok && (p.N & 15) == 0 && span32_ok(p) && !(MASK && (p.relu_mask != nullptr || !bits_ok));
@@ -1494,7 +1508,8 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           else run_blocks(std::integral_constant<int, 0>{});
         }
       } else {
-        run_blocks(std::integral_constant<int, 0>{});
+        if (split_tile) cp_piece();
+        else run_blocks(std::integral_constant<int, 0>{});
       }
       if (ew == 0 && lane == 0 && tile_iter < 4) TR(25 + 4 * tile_iter);
       ++tile_iter;
@@ -1518,6 +1533,32 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
     }
   }
   if (tid == 0) TR(3);
+}
+
+// Second half of a cp.async stream-K launch with fix-ups (deterministic atomic MN x MN launches): CTA t sums the
+// workspace slots of tile t's pieces in piece order and applies d = epi(sum) (with VLFB_EPI_ATOMIC: d += epi(sum)) once
+// per element.  Tiles that one unit ran whole were stored by the GEMM kernel itself.
+__global__ void __launch_bounds__(256) gemm_fixup_kernel(const vlfb_gemm_params_t p, const Launch L) {
+  const int t = blockIdx.x;
+  const int s0 = t * L.nkt, e0 = s0 + L.nkt;
+  int uf = 0, ul;
+  while (L.bounds[uf + 1] <= s0) ++uf;                  // the unit whose range holds the tile's first chunk
+  for (ul = uf; L.bounds[ul + 1] < e0; ++ul) {}         // ... and its last
+  if (ul == uf) return;
+  const int first_slot = L.bounds[uf] < s0 ? 1 : 0;     // as sched_next assigns the slots
+  TileInfo ti;
+  decode_tile(p, L, t, 1, ti);
+  const int rows = L.wide ? WM : BM, tcols = L.bn << L.wide;
+  const size_t tile_floats = (size_t)BM * L.bn;
+  for (int idx = threadIdx.x; idx < rows * tcols; idx += blockDim.x) {
+    const int r = idx / tcols, c = idx - r * tcols;
+    const int m = ti.m0 + r, n = ti.n0 + c;
+    if (m >= p.M || n >= p.N) continue;
+    float v = 0.f;
+    for (int u = uf; u <= ul; ++u)
+      v += L.ws_tiles[(size_t)(u * 2 + (u == uf ? first_slot : 0)) * tile_floats + idx];
+    epilogue_store(p, ti.batch, ti.tap, m, n, v, true);
+  }
 }
 
 // ---------------------------------------------------------------- host dispatch
@@ -1724,9 +1765,13 @@ struct Plan { int bn, split_k, pair, sk; int tiles, units; double cost; };
 
 // sk_ok = what the workspace allows; pow2_only: a 96-wide request becomes 64 (the cp.async MN-major loader needs a
 // power-of-two tile width).  p.pair is accepted and ignored: Hopper has no CTA-pair MMA (pair is always 0).
+// Deterministic atomic launches (p.deterministic): no plain split-K and no atomic stream-K.  Their schedule is split 1 or
+// stream-K with the workspace fix-up (pieces summed in piece order), the latter weighed by the cost model unless
+// p.stream_k = -1, since it replaces the split-K that such a launch would otherwise take.
 static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool pow2_only = false) {
   const int zbase = p.taps > 1 ? p.taps : p.batch;
   const bool atomic = (p.flags & VLFB_EPI_ATOMIC) != 0;
+  const bool det = atomic && p.deterministic != 0;
   int want_bn = p.tile_n > 0 ? p.tile_n : env().bn;
   if (want_bn > BN_MAX) want_bn = BN_MAX;                                      // wider requests get the widest tile
   if (pow2_only && (want_bn & (want_bn - 1))) want_bn = 64;
@@ -1751,7 +1796,7 @@ static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool
     const double cc = chunk_cost(bn, wide);
     const double fixed = 8.0 * cc;
     // (a) static tile loop, optional plain split-K (atomic epilogues only)
-    const int smax = p.split_k > 0 ? p.split_k : (atomic && p.K >= 512 ? (p.K / 256 < 128 ? p.K / 256 : 128) : 1);
+    const int smax = det ? 1 : p.split_k > 0 ? p.split_k : (atomic && p.K >= 512 ? (p.K / 256 < 128 ? p.K / 256 : 128) : 1);
     for (int sp = (p.split_k > 0 ? p.split_k : 1); sp <= smax; ++sp) {
       const int64_t tiles = T * sp;
       const double rounds = (double)((tiles + U - 1) / U);
@@ -1763,11 +1808,11 @@ static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool
     }
     // (b) stream-K: equal chunk ranges; shared tiles reduced through the workspace (or by atomics)
     const int64_t total = T * nkt;
-    const bool sk_legal = (atomic ? p.split_k != 1 : (sk_ok && p.split_k <= 1)) && want_sk > 0 && nkt >= 2 &&
-                          total >= 2 * (int64_t)U && T * (NEPI / 32) <= SK_CNT_INTS && U <= MAX_UNITS;
+    const bool sk_legal = (det ? sk_ok && want_sk >= 0 : (atomic ? p.split_k != 1 : (sk_ok && p.split_k <= 1)) && want_sk > 0) &&
+                          nkt >= 2 && total >= 2 * (int64_t)U && T * (NEPI / 32) <= SK_CNT_INTS && U <= MAX_UNITS;
     if (sk_legal && (T % U) != 0) {
       const double per_unit = (double)((total + U - 1) / U);
-      const double cost = per_unit * cc + fixed * (double)((T + U - 1) / U) + (atomic ? 1.0 : 2.0) * fixed;
+      const double cost = per_unit * cc + fixed * (double)((T + U - 1) / U) + (atomic && !det ? 1.0 : 2.0) * fixed;
       if (cost < best_sk.cost * 0.999) {
         best_sk.cost = cost; best_sk.bn = bn; best_sk.split_k = 1; best_sk.pair = 0; best_sk.sk = 1;
         best_sk.tiles = (int)T; best_sk.units = U;
@@ -1894,6 +1939,9 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
     }
   }
   L.wide = wide_tiles(p) ? 1 : 0;
+  const bool det = (p.flags & VLFB_EPI_ATOMIC) && p.deterministic;
+  // a deterministic atomic launch whose operands are both MN-major may run its fix-ups in the cp.async build
+  constexpr bool cp_fix = is_mn(AK) && is_mn(BK) && !MASK;
   Plan plan;
   bool pow2_only = false;
   for (int attempt = 0; attempt < 4; ++attempt) {
@@ -1991,8 +2039,8 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       L.stem_patch = 0;
     }
     if (is_mn(BK) && !L.tma_b && (L.bn & (L.bn - 1)) && !pow2_only) { pow2_only = true; continue; }
-    const bool fixup = plan.sk && !(p.flags & VLFB_EPI_ATOMIC);
-    if (!fixup || (L.tma_a && L.tma_b)) break;
+    const bool fixup = plan.sk && (!(p.flags & VLFB_EPI_ATOMIC) || det);
+    if (!fixup || (L.tma_a && L.tma_b) || (cp_fix && det)) break;
     sk_ws = false;                     // an operand fell back to cp.async: plan again without fix-ups
   }
   const int zbase = L.par ? L.par : (p.taps > 1 ? p.taps : p.batch);
@@ -2023,7 +2071,7 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
     L.nkt = ceil_div(p.K, KC);
     units = cap;
     make_bounds(L.bounds, units, (int64_t)L.total_tiles, L.nkt);
-    if (!(p.flags & VLFB_EPI_ATOMIC)) {
+    if (!(p.flags & VLFB_EPI_ATOMIC) || det) {
       L.ws_cnt = reinterpret_cast<int*>(p.workspace);
       L.ws_tiles = reinterpret_cast<float*>(reinterpret_cast<char*>(p.workspace) + (size_t)SK_CNT_INTS * 4);
     }
@@ -2043,12 +2091,25 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   // VLFB_DEBUG: one record per launch, space-separated key=value (tests/gemm_paths.py parses it; keep the keys stable)
   if (ev.debug)
     fprintf(stderr, "vlfb gemm_tc: kinds=%d,%d mask=%d M=%d N=%d K=%d z=%d bn=%d sk=%d split=%d tiles=%d units=%d stages=%d "
-            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d wide=%d\n",
+            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d wide=%d det=%d\n",
             AK, BK, MASK ? 1 : 0, p.M, p.N, p.K, zbase, L.bn, L.sk, p.split_k, L.total_tiles, units, L.stages, L.lag, L.tma_a,
             L.tma_b, cap, L.stem_patch, L.par, cp ? 1 : 0, L.ws_tiles != nullptr ? 1 : 0, lean ? 1 : 0, bits_after ? 1 : 0,
-            L.wide);
+            L.wide, det ? 1 : 0);
   int rc = VLFB_OK;
-  if (cp) rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);     // (fix-ups are planned for TMA-fed launches only)
+  // (cp.async fix-ups exist only in the MN x MN builds, for deterministic atomic launches: the planning loop above
+  // gives any other cp.async launch no workspace)
+  if (cp && L.ws_tiles) {
+    if constexpr (cp_fix) {
+      rc = launch_variant<AK, BK, MASK, true, true>(cfg, p, L, tmA, tmB);
+      if (rc == VLFB_OK) {
+        launch_k(gemm_fixup_kernel, dim3((unsigned)L.total_tiles), 256, 0, stream, p, L);
+        VLFB_CHECK_LAUNCH();
+      }
+    } else {
+      set_error("gemm_tc: stream-K fix-up planned for a cp.async build without one (kinds %d, %d)", AK, BK);
+      return VLFB_E_UNSUPPORTED;
+    }
+  } else if (cp) rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);
   else if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
   else rc = launch_variant<AK, BK, MASK, false, false>(cfg, p, L, tmA, tmB);
   if (rc == VLFB_OK && bits_after) rc = relu_bits(p.d, bits_after, (int64_t)p.M * p.N, stream);
@@ -2066,6 +2127,11 @@ void gemm_tc_plan(const vlfb_gemm_params_t& p, int num_sms, vlfb_gemm_plan_t* ou
 }
 
 size_t gemm_tc_workspace_bytes() { return tc::gemm_tc_workspace_bytes(); }
+float* gemm_tc_partials(void* workspace, size_t workspace_bytes, size_t* floats) {
+  const size_t head = (size_t)tc::SK_CNT_INTS * 4;
+  *floats = workspace && workspace_bytes > head ? (workspace_bytes - head) / 4 : 0;
+  return *floats ? reinterpret_cast<float*>(static_cast<char*>(workspace) + head) : nullptr;
+}
 #ifdef VLFB_TRACE
 void gemm_tc_set_trace(void* buf) { tc::g_trace_buf = reinterpret_cast<unsigned long long*>(buf); }
 #endif

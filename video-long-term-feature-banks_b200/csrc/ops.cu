@@ -289,6 +289,66 @@ __global__ void roi_align_bwd_k(const float* __restrict__ dout, const float* __r
   }
 }
 
+// Deterministic RoIAlign backward, pass 1: thread (r, channel quad) owns column c of RoI r's scratch slab [H][W][C] --
+// zeroes it, then walks its bins and samples in the order roi_align_bwd_k visits them, adding each contribution
+// without atomics.  Pass 2 (roi_scatter_det_k) adds the slabs of each feature map's RoIs in RoI order.
+__global__ void roi_align_bwd_det_k(const float* __restrict__ dout, const float* __restrict__ rois, float* __restrict__ scratch,
+                                    int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total) {
+  const int c4 = C >> 2;
+  const int64_t hwc = (int64_t)H * W * C;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % c4) * 4;
+    const int r = (int)(i / c4);
+    float* f = scratch + r * hwc + c;
+    for (int64_t p = 0; p < (int64_t)H * W; ++p) *reinterpret_cast<float4*>(f + p * C) = make_float4(0.f, 0.f, 0.f, 0.f);
+    const RoiBox b = roi_box(rois + r * 5, scale, PH, PW, sr);
+    const float cnt = (float)(b.gh * b.gw);
+    for (int ph = 0; ph < PH; ++ph)
+      for (int pw = 0; pw < PW; ++pw) {
+        float4 g = *reinterpret_cast<const float4*>(dout + (((int64_t)r * PH + ph) * PW + pw) * C + c);
+        g.x /= cnt; g.y /= cnt; g.z /= cnt; g.w /= cnt;
+        for (int iy = 0; iy < b.gh; ++iy)
+          for (int ix = 0; ix < b.gw; ++ix) {
+            int pos[4];
+            float w[4];
+            if (!roi_sample(b, ph, pw, iy, ix, H, W, pos, w)) continue;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              float4* d = reinterpret_cast<float4*>(f + (int64_t)pos[k] * C);
+              float4 v = *d;
+              v.x += w[k] * g.x; v.y += w[k] * g.y; v.z += w[k] * g.z; v.w += w[k] * g.w;
+              *d = v;
+            }
+          }
+      }
+  }
+}
+
+// pass 2: dfeat[n][p][c] += sum over the RoIs r of feature map n, in RoI order, of scratch[r][p][c]
+__global__ void roi_scatter_det_k(const float* __restrict__ scratch, const float* __restrict__ rois, float* __restrict__ dfeat,
+                                  int HW, int C, int R, int64_t total) {
+  const int c4 = C >> 2;
+  const int64_t hwc = (int64_t)HW * C;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t pc = i % ((int64_t)HW * c4);
+    const int n = (int)(i / ((int64_t)HW * c4));
+    const int64_t e = (pc / c4) * C + (pc % c4) * 4;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    bool any = false;
+    for (int r = 0; r < R; ++r) {
+      if ((int)rois[r * 5] != n) continue;               // the batch index as roi_box reads it
+      const float4 v = *reinterpret_cast<const float4*>(scratch + r * hwc + e);
+      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+      any = true;
+    }
+    if (!any) continue;
+    float4* d = reinterpret_cast<float4*>(dfeat + n * hwc + e);
+    float4 o = *d;
+    o.x += acc.x; o.y += acc.y; o.z += acc.z; o.w += acc.w;
+    *d = o;
+  }
+}
+
 __global__ void roi_table_k(const float* __restrict__ rois, int32_t* __restrict__ pos, float* __restrict__ wts,
                             int32_t* __restrict__ grid, int H, int W, int R, int PH, int PW, int mg, float scale,
                             int sr) {
@@ -1081,6 +1141,52 @@ int vlfb_sgd_nesterov(float* p, float* g, float* m, float* p_tf32, int64_t n, co
   VLFB_CHECK_ARG(p && g && m && lr && n >= 0);
   if (n == 0) return VLFB_OK;
   launch_k(sgd_k, stream_grid(n, TPB, 4), TPB, 0, ST(stream), p, g, m, p_tf32, n, lr, momentum, wd, nesterov);
+  VLFB_CHECK_LAUNCH();
+  return VLFB_OK;
+}
+
+}  // extern "C"
+
+// ---- deterministic forms (include/vlfb_det.h) ---------------------------------------------------------------------
+extern "C" {
+
+size_t vlfb_roi_align_bwd_det_scratch_bytes(int R, int H, int W, int C) {
+  return (R > 0 && H > 0 && W > 0 && C > 0) ? (size_t)R * H * W * C * sizeof(float) : 0;
+}
+
+int vlfb_roi_align_bwd_det(const float* dout, const float* rois, float* dfeat, int N, int H, int W, int C, int R, int PH,
+                           int PW, float spatial_scale, int sampling_ratio, void* scratch, size_t scratch_bytes,
+                           void* stream) {
+  VLFB_CHECK_ARG(dout && rois && dfeat && N > 0 && H > 0 && W > 0 && (C & 3) == 0 && C > 0 && R >= 0 && PH > 0 && PW > 0);
+  VLFB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(dfeat)) & 15) == 0);   // float4 access
+  if (R == 0) return VLFB_OK;
+  if (!scratch || scratch_bytes < vlfb_roi_align_bwd_det_scratch_bytes(R, H, W, C) ||
+      (reinterpret_cast<uintptr_t>(scratch) & 15) != 0) {
+    set_error("vlfb_roi_align_bwd_det: scratch must be 16-byte aligned and hold vlfb_roi_align_bwd_det_scratch_bytes()");
+    return VLFB_E_WORKSPACE;
+  }
+  float* sc = static_cast<float*>(scratch);
+  const int64_t per_roi = (int64_t)R * (C >> 2);
+  launch_k(roi_align_bwd_det_k, stream_grid(per_roi, TPB), TPB, 0, ST(stream), dout, rois, sc, H, W, C, PH, PW,
+           spatial_scale, sampling_ratio, per_roi);
+  VLFB_CHECK_LAUNCH();
+  const int64_t per_pix = (int64_t)N * H * W * (C >> 2);
+  launch_k(roi_scatter_det_k, stream_grid(per_pix, TPB), TPB, 0, ST(stream), (const float*)sc, rois, dfeat, H * W, C, R,
+           per_pix);
+  VLFB_CHECK_LAUNCH();
+  return VLFB_OK;
+}
+
+// One block per 32-column strip over all rows: the 8 row lanes and their fixed-order sum are the whole reduction, and
+// the single atomicAdd per column is the only write to it.
+int vlfb_colsum_det(const float* x, int64_t ld, float* out, int64_t rows, int cols, int accumulate, void* stream) {
+  VLFB_CHECK_ARG(x && out && rows >= 0 && cols > 0);
+  if (!accumulate) {
+    int rc = ew_launch<EW_FILL>(nullptr, nullptr, out, cols, 0.f, 0.f, ST(stream));
+    if (rc != VLFB_OK) return rc;
+  }
+  if (rows == 0) return VLFB_OK;
+  launch_k(colsum_k, dim3(ceil_div(cols, 32), 1), dim3(32, 8), 0, ST(stream), x, ld, out, rows, cols, rows);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }

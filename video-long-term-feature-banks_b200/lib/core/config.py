@@ -103,8 +103,11 @@ __C = _tree({
     # B200.FBO_FOLD: inference nets run each FBO-NL layer as one pass over the raw bank (vlfb.executor.FboFoldStep).
     # B200.LFB_DTYPE: 'f32' | 'bf16' = storage type of the feature-bank windows the folded inference FBO scans (a bf16
     #   copy is made when the bank is fed; scores / softmax / sums stay fp32; parity tolerance 1e-2 instead of 1e-3).
+    # B200.DETERMINISTIC: nets created while it is True run every cross-thread float reduction in a fixed order (no float
+    #   atomics with more than one contribution per element), so that two runs of the same calls from the same state are
+    #   bitwise identical on one GPU model and library build (DESIGN.md 4.5).  A guarantee, not a speed: off by default.
     'B200': {'COMPUTE': 'tf32', 'GEMM_BACKEND': 'tcgen05', 'CUDA_GRAPH': True, 'FBO_FOLD': True, 'FBO_STACK': True,
-             'LFB_DTYPE': 'f32'},
+             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False},
 })
 config = __C
 _DEFAULTS = None

@@ -37,6 +37,11 @@ RELU_BITS = os.environ.get('VLFB_RELU_BITS', '1') == '1'
 POOL_GATHER = int(os.environ.get('VLFB_POOL_GATHER', '1'))     # 2 = gather form only for non-overlapping windows
 
 
+def _mm(ctx):
+    """The matmul of this net: the deterministic form in a B200.DETERMINISTIC net."""
+    return K.matmul_det if ctx.net.det else K.matmul
+
+
 def set_backend(kernels_module, device, dtype=torch.float32):
     global K, DEVICE, DTYPE
     K = kernels_module
@@ -176,7 +181,7 @@ class Ctx(object):
         that consumes this gradient -- the blob's producer, through views -- feeds it to GEMMs, i.e. would round it to
         TF32 anyway: the kernel that computes the gradient then stores it rounded, and the consumer's copy + rounding
         passes disappear.  (A pooling / ReLU / LayerNorm backward keeps receiving the unrounded fp32 values.)"""
-        if self.net.contrib is None:
+        if self.net.contrib is None or self.net.det:
             return False
         while True:
             if self.net.contrib.get(key) != 1:
@@ -341,15 +346,17 @@ class ConvStep(Step):
         store = ctx.ws.params
         if store.trainable(self.w):
             mask = store.stem_mask() if g.C == 4 else None
-            K.conv_wgrad(gp, xp, store.grad(self.w), g, row_scale=scale, col_mask=mask, **self.gkw)
+            wgrad = K.conv_wgrad_det if ctx.net.det else K.conv_wgrad
+            wgrad(gp, xp, store.grad(self.w), g, row_scale=scale, col_mask=mask, **self.gkw)
         if self.b and store.trainable(self.b):
             db = store.grad(self.b)
             rows = gp.numel() // g.Co
+            colsum = K.colsum_det if ctx.net.det else K.colsum
             if scale is None:
-                K.colsum(gp, g.Co, db, rows, g.Co, accumulate=True)
+                colsum(gp, g.Co, db, rows, g.Co, accumulate=True)
             else:
                 t = empty((1, g.Co))
-                K.colsum(gp, g.Co, t, rows, g.Co, accumulate=False)
+                colsum(gp, g.Co, t, rows, g.Co, accumulate=False)
                 K.affine_bwd(t, scale, t)
                 K.axpby(db, 1.0, t.view(-1), 1.0, db)
         xkey = self.in_keys[0]
@@ -362,7 +369,7 @@ class ConvStep(Step):
                 K.weight_transpose(store.phys(self.w), wt, scale, **self.gkw)     # wt = round_tf32(w * s)
             cur = ctx.grads.get(xkey)
             prod = ctx.net.producer.get(xkey)
-            if (isinstance(prod, ConvStep) and ctx.is_last_contribution(xkey) and FUSE_GRAD_FINISH
+            if (isinstance(prod, ConvStep) and ctx.is_last_contribution(xkey) and FUSE_GRAD_FINISH and not ctx.net.det
                     and (cur is None or (is_cl(cur) and as5d(phys(cur)).shape == xp.shape))):
                 # Last contribution to the gradient of a conv output: sum the earlier contributions, apply that
                 # conv's ReLU backward (mask = its output = our input xp) and the TF32 rounding its own
@@ -437,8 +444,9 @@ class SpatialBNStep(Step):
         else:
             c = xp.shape[-1]
             sm, siv = empty((c,)), empty((c,))
-            K.spatial_bn_fwd(xp, st.phys(self.s), st.phys(self.b), st.phys(self.rm), st.phys(self.riv), sm, siv, phys(y),
-                             self.eps, self.momentum)
+            bn_fwd = K.spatial_bn_fwd_det if ctx.net.det else K.spatial_bn_fwd
+            bn_fwd(xp, st.phys(self.s), st.phys(self.b), st.phys(self.rm), st.phys(self.riv), sm, siv, phys(y),
+                   self.eps, self.momentum)
             ctx.put(self.op.outputs[3], sm)
             ctx.put(self.op.outputs[4], siv)
             ctx.saved[id(self)] = (xp, sm, siv)
@@ -455,9 +463,10 @@ class SpatialBNStep(Step):
         st = ctx.ws.params
         need_dx = ctx.net.requires.get(self.in_keys[0], False)
         dx = empty_like_strided(gy)
-        K.spatial_bn_bwd(gp, xp, st.phys(self.s), sm, siv, phys(dx),
-                         st.grad(self.s) if st.trainable(self.s) else None,
-                         st.grad(self.b) if st.trainable(self.b) else None)
+        bn_bwd = K.spatial_bn_bwd_det if ctx.net.det else K.spatial_bn_bwd
+        bn_bwd(gp, xp, st.phys(self.s), sm, siv, phys(dx),
+               st.grad(self.s) if st.trainable(self.s) else None,
+               st.grad(self.b) if st.trainable(self.b) else None)
         if need_dx:
             ctx.add_grad(self.in_keys[0], dx, owned=True)
 
@@ -576,7 +585,8 @@ class PoolStep(Step):
         gp = as5d(phys(gy))
         xkey = self.in_keys[0]
         overlap = g.kT > g.sT or g.kH > g.sH or g.kW > g.sW
-        if self.op.type == 'MaxPool' and (POOL_GATHER == 0 or (POOL_GATHER == 2 and overlap)):
+        # (a deterministic net always takes the gather form: the scatter form adds with atomics)
+        if self.op.type == 'MaxPool' and not ctx.net.det and (POOL_GATHER == 0 or (POOL_GATHER == 2 and overlap)):
             K.fill(flat(dx), 0.0)
             K.maxpool_bwd(gp, arg, as5d(phys(dx)), g)
         elif self.op.type == 'MaxPool':
@@ -585,7 +595,7 @@ class PoolStep(Step):
             # winner of a window is positive iff the window's maximum is) and the TF32 rounding of the conv's wgrad
             # operand are folded in and the conv receives a finished gradient.
             prod = ctx.net.producer.get(xkey)
-            fuse = (FUSE_GRAD_FINISH and isinstance(prod, ConvStep) and prod.relu and ctx.net.contrib is not None
+            fuse = (FUSE_GRAD_FINISH and not ctx.net.det and isinstance(prod, ConvStep) and prod.relu and ctx.net.contrib is not None
                     and ctx.net.contrib.get(xkey) == 1)
             K.maxpool_bwd_gather(gp, arg, yp if fuse else None, as5d(phys(dx)), g, tf32_out=fuse)
             if fuse:
@@ -682,7 +692,7 @@ class BatchMatMulStep(Step):
             d = empty((Bt, N, M)).transpose(1, 2)
         else:
             d = empty((Bt, M, N))
-        K.matmul(A, B, d, tf32_out=True)
+        _mm(ctx)(A, B, d, tf32_out=True)
         ctx.saved[id(self)] = (a, b)
         ctx.put(self.op.outputs[0], d, rounded=True)
 
@@ -700,12 +710,12 @@ class BatchMatMulStep(Step):
         if ctx.net.requires.get(self.in_keys[0], False):
             da = empty_like_strided(a)
             dA = da.transpose(1, 2) if ta else da
-            sole = K.matmul(g, B.transpose(1, 2), dA, tf32_out=ctx.sole(self.in_keys[0]), tf32_optional=True)
+            sole = _mm(ctx)(g, B.transpose(1, 2), dA, tf32_out=ctx.sole(self.in_keys[0]), tf32_optional=True)
             ctx.add_grad(self.in_keys[0], da, owned=True, rounded=sole)
         if ctx.net.requires.get(self.in_keys[1], False):
             db = empty_like_strided(b)
             dB = db.transpose(1, 2) if tb else db
-            sole = K.matmul(A.transpose(1, 2), g, dB, tf32_out=ctx.sole(self.in_keys[1]), tf32_optional=True)
+            sole = _mm(ctx)(A.transpose(1, 2), g, dB, tf32_out=ctx.sole(self.in_keys[1]), tf32_optional=True)
             ctx.add_grad(self.in_keys[1], db, owned=True, rounded=sole)
 
 
@@ -743,17 +753,17 @@ class FboFoldStep(Step):
         wg = P.tf32(self.wg).view(1, -1, d1)                    # [dg][d1]
         dg = int(wg.shape[1])
         u = empty((1, R, d1))
-        K.matmul(flat(theta).view(1, R, d), wphi, u, tf32_out=True)
+        _mm(ctx)(flat(theta).view(1, R, d), wphi, u, tf32_out=True)
         q = empty((1, R, D))
-        K.matmul(u, w1, q)
+        _mm(ctx)(u, w1, q)
         s = empty((R, D))
         prob = empty((R, L_)) if self.prob_name else None
         K.fbo_bank_scan(bank, q.view(R, D), s, self.scale, prob=prob, tf32_out=True)
         t = empty((1, R, d1))
-        K.matmul(s.view(1, R, D), w1.transpose(1, 2), t, bias=None if self.b1 is None else P.phys(self.b1),
+        _mm(ctx)(s.view(1, R, D), w1.transpose(1, 2), t, bias=None if self.b1 is None else P.phys(self.b1),
                  tf32_out=True)
         y = empty((1, R, dg))
-        K.matmul(t, wg.transpose(1, 2), y, bias=None if self.bg is None else P.phys(self.bg), tf32_out=True)
+        _mm(ctx)(t, wg.transpose(1, 2), y, bias=None if self.bg is None else P.phys(self.bg), tf32_out=True)
         if prob is not None:
             ctx.put(self.prob_name, prob.view(R, 1, L_))
         ctx.put(self.op.outputs[0], y.view(R, dg, 1), rounded=True)
@@ -931,7 +941,7 @@ class FCStep(Step):
         w = ctx.ws.params.tf32(self.op.inputs[1])
         b = ctx.ws.params.phys(self.op.inputs[2])
         y = empty((x2.shape[0], w.shape[0]))
-        K.matmul(x2.unsqueeze(0), w.t().unsqueeze(0), y.unsqueeze(0), bias=b)
+        _mm(ctx)(x2.unsqueeze(0), w.t().unsqueeze(0), y.unsqueeze(0), bias=b)
         ctx.saved[id(self)] = (x2, x.shape, x.stride())
         ctx.put(self.op.outputs[0], y)
 
@@ -944,12 +954,13 @@ class FCStep(Step):
         store = ctx.ws.params
         wname, bname = self.op.inputs[1], self.op.inputs[2]
         if store.trainable(wname):
-            K.matmul(gy.t().unsqueeze(0), x2.unsqueeze(0), store.grad(wname).unsqueeze(0), accumulate=True)
+            _mm(ctx)(gy.t().unsqueeze(0), x2.unsqueeze(0), store.grad(wname).unsqueeze(0), accumulate=True)
         if store.trainable(bname):
-            K.colsum(gy, gy.shape[1], store.grad(bname), gy.shape[0], gy.shape[1], accumulate=True)
+            colsum = K.colsum_det if ctx.net.det else K.colsum
+            colsum(gy, gy.shape[1], store.grad(bname), gy.shape[0], gy.shape[1], accumulate=True)
         if ctx.net.requires.get(self.in_keys[0], False):
             dx = torch.empty_strided(xshape, xstride, dtype=DTYPE, device=DEVICE)
-            K.matmul(gy.unsqueeze(0), store.tf32(wname).unsqueeze(0), flat(dx).view(1, x2.shape[0], -1))
+            _mm(ctx)(gy.unsqueeze(0), store.tf32(wname).unsqueeze(0), flat(dx).view(1, x2.shape[0], -1))
             ctx.add_grad(self.in_keys[0], dx, owned=True)
 
 
@@ -1007,7 +1018,8 @@ class RoIAlignStep(Step):
         a = self.op.args
         d = torch.empty_strided(shape, stride, dtype=DTYPE, device=DEVICE)
         K.fill(flat(d), 0.0)
-        K.roi_align_bwd(phys(gy), rois, phys(d), a['spatial_scale'], a['sampling_ratio'])
+        roi_bwd = K.roi_align_bwd_det if ctx.net.det else K.roi_align_bwd
+        roi_bwd(phys(gy), rois, phys(d), a['spatial_scale'], a['sampling_ratio'])
         ctx.add_grad(self.in_keys[0], d, owned=True)
 
 
@@ -1069,9 +1081,16 @@ OPTIMIZER_OPS = ('WeightedSum', 'MomentumSGDUpdate')
 # ====================================================================================== lowering
 class CompiledNet(object):
     def __init__(self, model, ws):
+        from core.config import config as cfg
         self.model = model
         self.ws = ws
         self.name = model.net.Proto().name
+        # read once, when the net is created.  A deterministic net also skips everything the first run's record of
+        # gradient contributions (self.contrib) switches on later -- the grad-finish fusion, producer-side rounding of
+        # sole gradients -- so that its first eager run computes exactly what every later run and graph replay does, and a
+        # run resumed from a checkpoint in a fresh net continues the interrupted one bit for bit.
+        self.det = bool(cfg.B200.get('DETERMINISTIC', False))
+        self._rng_base = None        # deterministic nets: the workspace's dropout offset at the first run
         ops = [op for op in model.net.ops if op.type not in OPTIMIZER_OPS]
         self.update_ops = [op for op in model.net.ops if op.type in OPTIMIZER_OPS]
         self.losses = list(getattr(model, '_losses', []) or [])
@@ -1090,7 +1109,7 @@ class CompiledNet(object):
         # conv + ReLU outputs whose backward mask a consumer conv's dgrad epilogue may apply (grad-finish fusion): they
         # also emit their sign bits
         self.want_relu_bits = set()
-        if self.train and FUSE_GRAD_FINISH and RELU_BITS:
+        if self.train and FUSE_GRAD_FINISH and RELU_BITS and not self.det:
             for st in self.steps:
                 if isinstance(st, ConvStep) and self.requires.get(st.in_keys[0], False):
                     pr = self.producer.get(st.in_keys[0])
@@ -1396,6 +1415,12 @@ class CompiledNet(object):
         from core.config import config as cfg
         ws = self.ws
         ws.begin_run()
+        if self.det:
+            # every run draws the dropout offsets its first run drew, as a graph replay does (the step counter varies
+            # the masks), so the masks of a step depend on the step counter only, not on how many eager runs preceded
+            if self._rng_base is None:
+                self._rng_base = ws.rng_offset
+            ws.rng_offset = self._rng_base
         use_graph = (DEVICE != 'cpu' and cfg.B200.CUDA_GRAPH and not ws.force_eager and K is K_default)
         key = self._input_key() if use_graph else None
         if use_graph:

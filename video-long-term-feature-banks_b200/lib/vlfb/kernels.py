@@ -293,6 +293,16 @@ def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None, groups=1):
     """dw[co,tap,ci] += row_scale[co] * sum_m dy[m,co] * x[gather(m,tap),ci]  (atomic accumulate:
     dw must be zero-initialised or hold a partial sum).  Stem path when C == 4 (dw [Co,kT,kH,8,4],
     col_mask [32] zeroes the padding lanes).  groups > 1: dw [Co,kT,kH,kW,C/groups], ci within co's group."""
+    _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, False)
+
+
+def conv_wgrad_det(dy, x, dw, g, row_scale=None, col_mask=None, groups=1):
+    """conv_wgrad with a reproducible sum: every dw element receives one contribution per launch (split 1 or stream-K
+    with the workspace fix-up; grouped: partial slabs summed in split order)."""
+    _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, True)
+
+
+def _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, det):
     _f32c(dy, 'dy'), _f32c(dw, 'dw')
     Kpos = g.N * g.To * g.Ho * g.Wo
     groups = _check_groups(g, groups)
@@ -321,6 +331,7 @@ def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None, groups=1):
     p.split_k = 0            # split-K and the tile width are chosen together by the library (gemm_tc.cu launch())
     p.groups = groups
     p.flags |= L.EPI_ATOMIC
+    p.deterministic = int(det)
     _set_epilogue(p, col_mask, None, row_scale, None, False)
     _run_gemm(p, 'conv_wgrad', 2.0 * Kpos * g.Co * g.kT * g.kH * g.kW * (3 if g.C == 4 else cin),
               _nbytes(dy, x, dw), keep=(dy, x, dw, row_scale, col_mask))
@@ -378,6 +389,17 @@ def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32
     TF32-rounded: with `tf32_optional` a product that qualifies for split-K (atomic accumulation cannot round) keeps
     the split and leaves the rounding to the consumer -- the split is worth 2x on the K = 3136 non-local gradient
     products."""
+    return _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, False)
+
+
+def matmul_det(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32_optional=False):
+    """matmul with a reproducible sum: the long-K products that matmul splits over atomics run as one deterministic
+    launch (split 1 or stream-K with the workspace fix-up).  Every element gets one contribution onto a zeroed d, so the
+    TF32 rounding is kept (tf32_optional changes nothing) unless d is accumulated."""
+    return _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, True)
+
+
+def _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, det):
     assert a.dim() == 3 and b.dim() == 3 and d.dim() == 3
     Bt, M, K = a.shape
     N = b.shape[2]
@@ -386,8 +408,8 @@ def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32
         # output is column-major: compute d^T = b^T a^T
         assert _dim_ok(d.stride(1), M), 'matmul output needs a unit stride'
         assert bias is None
-        return matmul(b.transpose(1, 2), a.transpose(1, 2), d.transpose(1, 2), alpha, accumulate, None, tf32_out,
-                      tf32_optional)
+        return _matmul(b.transpose(1, 2), a.transpose(1, 2), d.transpose(1, 2), alpha, accumulate, None, tf32_out,
+                       tf32_optional, det)
     ka, lda, sba = _mat_operand(a, 1, 2)
     kb, ldb, sbb = _mat_operand(b, 2, 1)
     p = _base_params(M, N, K, d, d.stride(1) if M > 1 else N, alpha)
@@ -396,18 +418,30 @@ def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32
     p.batch = Bt
     p.d_batch_stride = d.stride(0) if Bt > 1 else 0
     tiles = Bt * ((M + 127) // 128) * ((N + 255) // 256)
-    if tiles <= NUM_SMS // 2 and K >= 1024 and tf32_out and tf32_optional:
-        tf32_out = False
-    if tiles <= NUM_SMS // 2 and K >= 1024 and not tf32_out:
-        # few output tiles with a long reduction (the 4 x 80 x 2560 classifier ran 0.19 ms on ONE CTA; the non-local
-        # affinity products fill 28-56 of 132 SMs): split K over the SMs -- atomic accumulation into a zeroed / kept
-        # D, bias from the first slice; the library picks the split together with the tile width
-        if not accumulate:
-            fill(d, 0.0) if d.is_contiguous() else d.zero_()
-        p.split_k = 0
-        p.flags |= L.EPI_ATOMIC
-    elif accumulate:
-        p.flags |= L.EPI_ACCUM
+    if det:
+        # the same long-K products as below, as one deterministic launch; it stores each element once onto the zeroed d,
+        # so the rounding stays (an accumulated, rounded d keeps the ordinary ACCUM epilogue)
+        if tiles <= NUM_SMS // 2 and K >= 1024 and not (tf32_out and accumulate):
+            if not accumulate:
+                fill(d, 0.0) if d.is_contiguous() else d.zero_()
+            p.split_k = 0
+            p.flags |= L.EPI_ATOMIC
+            p.deterministic = 1
+        elif accumulate:
+            p.flags |= L.EPI_ACCUM
+    else:
+        if tiles <= NUM_SMS // 2 and K >= 1024 and tf32_out and tf32_optional:
+            tf32_out = False
+        if tiles <= NUM_SMS // 2 and K >= 1024 and not tf32_out:
+            # few output tiles with a long reduction (the 4 x 80 x 2560 classifier ran 0.19 ms on ONE CTA; the non-local
+            # affinity products fill 28-56 of 132 SMs): split K over the SMs -- atomic accumulation into a zeroed / kept
+            # D, bias from the first slice; the library picks the split together with the tile width
+            if not accumulate:
+                fill(d, 0.0) if d.is_contiguous() else d.zero_()
+            p.split_k = 0
+            p.flags |= L.EPI_ATOMIC
+        elif accumulate:
+            p.flags |= L.EPI_ACCUM
     _set_epilogue(p, None, bias, None, None, False, tf32_out)
     _run_gemm(p, 'matmul', 2.0 * Bt * M * N * K, 4.0 * Bt * (M * K + K * N + M * N * (2 if accumulate else 1)),
               keep=(a, b, d, bias))
@@ -478,6 +512,22 @@ def spatial_bn_bwd(dy, x, s, sm, siv, dx, ds, db):
            'spatial_bn_bwd')
 
 
+def spatial_bn_fwd_det(x, s, b, rm, rv, sm, siv, y, eps, momentum):
+    """spatial_bn_fwd with reproducible batch statistics (vlfb_spatial_bn_fwd_det)."""
+    ws, nb = _bn_workspace(x.shape[-1])
+    _check(L.load().vlfb_spatial_bn_fwd_det(_ptr(_f32c(x)), _ptr(s), _ptr(b), _ptr(rm), _ptr(rv), _ptr(sm), _ptr(siv),
+                                            _ptr(_f32c(y)), x.numel() // x.shape[-1], x.shape[-1], float(eps),
+                                            float(momentum), _ptr(ws), nb, _stream()), 'spatial_bn_fwd_det')
+
+
+def spatial_bn_bwd_det(dy, x, s, sm, siv, dx, ds, db):
+    """spatial_bn_bwd with reproducible sums (vlfb_spatial_bn_bwd_det)."""
+    ws, nb = _bn_workspace(x.shape[-1])
+    _check(L.load().vlfb_spatial_bn_bwd_det(_ptr(_f32c(dy)), _ptr(_f32c(x)), _ptr(s), _ptr(sm), _ptr(siv),
+                                            _ptr(_f32c(dx)), _ptr(ds), _ptr(db), x.numel() // x.shape[-1], x.shape[-1],
+                                            _ptr(ws), nb, _stream()), 'spatial_bn_bwd_det')
+
+
 def maxpool_fwd(x, y, argmax, g):
     _check(L.load().vlfb_maxpool3d_fwd(_ptr(_f32c(x)), _ptr(_f32c(y)), _ptr(argmax), C.byref(g), _stream()),
             'maxpool_fwd')
@@ -517,6 +567,18 @@ def roi_align_bwd(dout, rois, dfeat, spatial_scale, sampling_ratio=0):
     r, ph, pw, _ = dout.shape
     _check(L.load().vlfb_roi_align_bwd(_ptr(_f32c(dout)), _ptr(_f32c(rois)), _ptr(_f32c(dfeat)), n, h, w, c, r, ph,
                                         pw, float(spatial_scale), int(sampling_ratio), _stream()), 'roi_align_bwd')
+
+
+def roi_align_bwd_det(dout, rois, dfeat, spatial_scale, sampling_ratio=0):
+    """roi_align_bwd in a fixed summation order (vlfb_roi_align_bwd_det); the per-RoI scratch is allocated here."""
+    n, h, w, c = dfeat.shape
+    r, ph, pw, _ = dout.shape
+    lib = L.load()
+    nbytes = int(lib.vlfb_roi_align_bwd_det_scratch_bytes(r, h, w, c))
+    scratch = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=dfeat.device)
+    _check(lib.vlfb_roi_align_bwd_det(_ptr(_f32c(dout)), _ptr(_f32c(rois)), _ptr(_f32c(dfeat)), n, h, w, c, r, ph, pw,
+                                      float(spatial_scale), int(sampling_ratio), _ptr(scratch), nbytes, _stream()),
+           'roi_align_bwd_det')
 
 
 def roi_align_table(rois, h, w, ph, pw, max_grid, spatial_scale, sampling_ratio=0):
@@ -603,6 +665,12 @@ def relu_bwd_tf32(dy, y, dx):
 def colsum(x, ld, out, rows, cols, accumulate=False):
     _check(L.load().vlfb_colsum(_ptr(x), int(ld), _ptr(out), int(rows), int(cols), int(accumulate), _stream()),
             'colsum')
+
+
+def colsum_det(x, ld, out, rows, cols, accumulate=False):
+    """colsum in a fixed summation order (vlfb_colsum_det)."""
+    _check(L.load().vlfb_colsum_det(_ptr(x), int(ld), _ptr(out), int(rows), int(cols), int(accumulate), _stream()),
+           'colsum_det')
 
 
 def sigmoid_fwd(x, y):

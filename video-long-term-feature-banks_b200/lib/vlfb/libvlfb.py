@@ -33,7 +33,8 @@ class GemmParams(C.Structure):
                 ('residual', C.c_void_p), ('relu_mask', C.c_void_p), ('flags', C.c_int),
                 ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t),
                 ('engine', C.c_int), ('tile_n', C.c_int), ('pair', C.c_int), ('stream_k', C.c_int),
-                ('relu_mask_bits', C.c_void_p), ('relu_bits_out', C.c_void_p), ('groups', C.c_int)]
+                ('relu_mask_bits', C.c_void_p), ('relu_bits_out', C.c_void_p), ('groups', C.c_int),
+                ('deterministic', C.c_int)]
 
 
 class GemmPlan(C.Structure):
@@ -122,7 +123,15 @@ SIGNATURES = {
     'vlfb_cast_f32_to_bf16': [_P, _P, _L, _P],
     'vlfb_lfb_gather': [_P, _L, _P, _P, _L, _I, _I, _P],
 }
-RESTYPES = {'vlfb_last_error': C.c_char_p, 'vlfb_fbo_bank_scan_workspace': C.c_size_t,
+# include/vlfb_det.h (included by vlfb.h): the deterministic forms of the streaming reductions
+DET_SIGNATURES = {
+    'vlfb_roi_align_bwd_det_scratch_bytes': [_I, _I, _I, _I],
+    'vlfb_roi_align_bwd_det': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _I, _P, C.c_size_t, _P],
+    'vlfb_colsum_det': [_P, _L, _P, _L, _I, _I, _P],
+    'vlfb_spatial_bn_fwd_det': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _F, _F, _P, C.c_size_t, _P],
+    'vlfb_spatial_bn_bwd_det': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _P, C.c_size_t, _P],
+}
+RESTYPES = {'vlfb_last_error': C.c_char_p, 'vlfb_roi_align_bwd_det_scratch_bytes': C.c_size_t, 'vlfb_fbo_bank_scan_workspace': C.c_size_t,
             'vlfb_fbo_bank_scan_workspace_dt': C.c_size_t,
             'vlfb_fbo_nl_scratch_floats': C.c_size_t,
             'vlfb_gemm_workspace_bytes': C.c_size_t, 'vlfb_spatial_bn_workspace_bytes': C.c_size_t}
@@ -140,7 +149,7 @@ def load():
             'libvlfb.so not found at %s -- build it first (python -c "import __graft_entry__ as g; '
             'g.build()" or make -C csrc).  There is no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, argtypes in SIGNATURES.items():
+    for name, argtypes in list(SIGNATURES.items()) + list(DET_SIGNATURES.items()):
         fn = getattr(lib, name)        # AttributeError if the symbol is missing
         fn.argtypes = argtypes
         fn.restype = RESTYPES.get(name, C.c_int)
