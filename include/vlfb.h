@@ -363,6 +363,10 @@ typedef struct {
   float drop_ratio;                 /* 0 = no dropout on the layer outputs         */
   uint64_t seed;
   const int64_t* step;              /* optional device scalar added to the counter (<< 32), as in vlfb_dropout_fwd */
+  /* optional device int32 scalar (NULL = all R rows; executor.FboStackStep under B200.ROI_CAPACITY): rows >= *live_rows
+   * are padding.  fwd writes zeros to every per-row output of such a row; bwd writes zeros to its da0 / dbp rows and adds
+   * nothing from it to the weight gradients.  The live rows equal an R = *live_rows launch bit for bit. */
+  const int32_t* live_rows;
 } vlfb_fbo_cfg_t;
 
 size_t vlfb_fbo_nl_scratch_floats(const vlfb_fbo_cfg_t* cfg);
@@ -385,4 +389,5 @@ int vlfb_lfb_gather(const float* bank, int64_t bank_rows, const int32_t* idx, fl
 }
 #endif
 #include "vlfb_det.h"
+#include "vlfb_live.h"
 #endif /* VLFB_H_ */

@@ -13,6 +13,7 @@
 // 2. lfb_gather: builds the per-sample (L x D) bank windows on the device from a resident bank tensor and a host
 //    computed row-index table (tools/lfb_loader.py:51-152 + lib/datasets/ava.py:300-323: -1 = zero padding).
 #include <float.h>
+#include <limits.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -78,11 +79,13 @@ __device__ __forceinline__ void unpack16(const uint4& u, float (&f)[EPL]) {
 template <int EPL, int V, int ROWS>
 __global__ void __launch_bounds__(SCAN_TPB, (EPL == 8 && V == 1) ? VLFB_SCAN16_MINB : 2)
 fbo_bank_scan_k(const void* __restrict__ bank, const float* __restrict__ q, float scale, float* __restrict__ part_acc,
-                float* __restrict__ part_ml, float* __restrict__ scores, int L, int S, int rows_per_split) {
+                float* __restrict__ part_ml, float* __restrict__ scores, int L, int S, int rows_per_split,
+                const int32_t* __restrict__ live) {
   constexpr int D = SCAN_TPB * V * EPL;
   constexpr int NW = SCAN_TPB / 32;
   __shared__ float xch[2][NW][ROWS];
   const int r = blockIdx.x / S, sp = blockIdx.x % S;
+  if (live != nullptr && r >= *live) return;          // padding row: fbo_bank_combine_k writes its zeros
   const int row_begin = sp * rows_per_split;
   const int row_end = min(L, row_begin + rows_per_split);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -198,8 +201,15 @@ __global__ void f32_to_bf16_k(const float4* __restrict__ x, uint4* __restrict__ 
 // the A operand of the W_1 matmul).  prob[r][j] = exp(score - M) / lsum when the scores were kept.
 __global__ void fbo_bank_combine_k(const float* __restrict__ part_acc, const float* __restrict__ part_ml,
                                    float* __restrict__ out, float* __restrict__ scores_prob, int S, int D, int L,
-                                   int tf32_out) {
+                                   int tf32_out, const int32_t* __restrict__ live) {
   const int r = blockIdx.y;
+  if (live != nullptr && r >= *live) {                 // padding row: out = 0, prob = 0
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c < D) out[(int64_t)r * D + c] = 0.f;
+    if (scores_prob != nullptr)
+      for (int j = c; j < L; j += gridDim.x * blockDim.x) scores_prob[(int64_t)r * L + j] = 0.f;
+    return;
+  }
   float M = -FLT_MAX;
   for (int s = 0; s < S; ++s)
     if (part_ml[((int64_t)r * S + s) * 2 + 1] > 0.f) M = fmaxf(M, part_ml[((int64_t)r * S + s) * 2]);
@@ -408,6 +418,19 @@ __global__ void __launch_bounds__(NL_TPB, 1) fbo_nl_fwd_k(const NlParams P) {
   float* sE = sO + c.dA;
   float* red = sE + ((c.L + 3) & ~3);
   const float* B = P.bp + (int64_t)r * c.L * c.dB;
+  if (c.live_rows != nullptr && r >= *c.live_rows) {            // padding row: zeros in every per-row output
+    for (int li = 0; li < c.layers; ++li) {
+      const vlfb_fbo_layer_t& l = P.l[li];
+      for (int i = tid; i < c.d; i += NL_TPB) {
+        l.theta[(int64_t)r * c.d + i] = 0.f; l.t[(int64_t)r * c.d + i] = 0.f; l.xhat[(int64_t)r * c.d + i] = 0.f;
+      }
+      for (int i = tid; i < c.dB; i += NL_TPB) l.s[(int64_t)r * c.dB + i] = 0.f;
+      for (int j = tid; j < c.L; j += NL_TPB) l.prob[(int64_t)r * c.L + j] = 0.f;
+      for (int i = tid; i < c.dA; i += NL_TPB) { l.out[(int64_t)r * c.dA + i] = 0.f; l.a_out[(int64_t)r * c.dA + i] = 0.f; }
+      if (tid == 0) { l.ln_mean[r] = 0.f; l.ln_std[r] = 0.f; }
+    }
+    return;
+  }
   for (int i = tid; i < c.dA; i += NL_TPB) sA[i] = P.a0[(int64_t)r * c.dA + i];
   __syncthreads();
   uint64_t step_off = c.step ? ((uint64_t)c.step[0] << 32) : 0ull;
@@ -498,6 +521,12 @@ __global__ void __launch_bounds__(NL_TPB, 1) fbo_nl_bwd_k(const NlParams P) {
   const float* B = P.bp + (int64_t)r * c.L * c.dB;
   float* dB = P.dbp + (int64_t)r * c.L * c.dB;
   const int per_roi = c.dA + c.d + c.dB + c.d + 4;
+  if (c.live_rows != nullptr && r >= *c.live_rows) {            // padding row: zero gradients, no scratch (outer_k skips it)
+    for (int i = tid; i < c.dA; i += NL_TPB) P.da0[(int64_t)r * c.dA + i] = 0.f;
+    float4* dB4 = reinterpret_cast<float4*>(dB);
+    for (int64_t e = tid; e < (int64_t)c.L * (c.dB >> 2); e += NL_TPB) dB4[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
   for (int i = tid; i < c.dA; i += NL_TPB) sDA[i] = P.da_last[(int64_t)r * c.dA + i];
   __syncthreads();
   const uint64_t step_off = c.step ? ((uint64_t)c.step[0] << 32) : 0ull;
@@ -599,6 +628,7 @@ __global__ void __launch_bounds__(256) fbo_nl_outer_k(const NlParams P) {
   const int li = blockIdx.y >> 2, which = blockIdx.y & 3;
   const vlfb_fbo_layer_t& l = P.l[li];
   const int per_roi = c.dA + c.d + c.dB + c.d + 4;
+  const int R = c.live_rows != nullptr ? min(c.R, *c.live_rows) : c.R;     // padding rows add nothing
   const float* scr = P.scratch + (int64_t)li * c.R * per_roi;
   const float* left;
   const float* right;
@@ -614,7 +644,7 @@ __global__ void __launch_bounds__(256) fbo_nl_outer_k(const NlParams P) {
     if (gw) {
       for (int i = threadIdx.x; i < cols; i += blockDim.x) {
         float acc = 0.f;
-        for (int r = 0; r < c.R; ++r) {
+        for (int r = 0; r < R; ++r) {
           float rv = right[(int64_t)r * rstride + i];
           if (which == 0) rv = fmaxf(rv, 0.f);                   // act = relu(xhat)
           acc += left[(int64_t)r * lstride + row] * rv;
@@ -624,7 +654,7 @@ __global__ void __launch_bounds__(256) fbo_nl_outer_k(const NlParams P) {
     }
     if (gb && threadIdx.x == 0) {
       float acc = 0.f;
-      for (int r = 0; r < c.R; ++r) {
+      for (int r = 0; r < R; ++r) {
         float lv = left[(int64_t)r * lstride + row];
         if (which == 2) lv *= scr[(int64_t)r * per_roi + c.dA + c.d + c.dB + c.d];   // theta_o * sum_j dscore_j
         acc += lv;
@@ -679,6 +709,13 @@ size_t vlfb_fbo_bank_scan_workspace(int R, int L, int D) { return vlfb_fbo_bank_
 
 int vlfb_fbo_bank_scan_dt(const void* bank, int bank_dtype, const float* q, float scale, float* out, float* prob, int R,
                           int L, int D, int tf32_out, void* workspace, size_t workspace_bytes, void* stream) {
+  return vlfb_fbo_bank_scan_live(bank, bank_dtype, q, scale, out, prob, R, L, D, tf32_out, workspace, workspace_bytes,
+                                 nullptr, stream);
+}
+
+int vlfb_fbo_bank_scan_live(const void* bank, int bank_dtype, const float* q, float scale, float* out, float* prob, int R,
+                            int L, int D, int tf32_out, void* workspace, size_t workspace_bytes, const int32_t* live_rows,
+                            void* stream) {
   VLFB_CHECK_ARG(bank && q && out && R >= 0 && L > 0);
   VLFB_CHECK_ARG(bank_dtype == VLFB_DT_F32 || bank_dtype == VLFB_DT_BF16);
   VLFB_CHECK_ARG(scan_rows(D, bank_dtype) > 0);
@@ -696,7 +733,8 @@ int vlfb_fbo_bank_scan_dt(const void* bank, int bank_dtype, const float* q, floa
   const int per = (L + S - 1) / S;
   const dim3 grid((unsigned)(R * S));
 #define VLFB_SCAN(EPL, V, ROWS) \
-  launch_k(fbo_bank_scan_k<EPL, V, ROWS>, grid, SCAN_TPB, 0, ST(stream), bank, q, scale, part_acc, part_ml, prob, L, S, per)
+  launch_k(fbo_bank_scan_k<EPL, V, ROWS>, grid, SCAN_TPB, 0, ST(stream), bank, q, scale, part_acc, part_ml, prob, L, S, per, \
+           live_rows)
   if (bank_dtype == VLFB_DT_F32) {
     if (D == 1024) VLFB_SCAN(4, 1, 8);
     else if (D == 2048) VLFB_SCAN(4, 2, 8);
@@ -708,7 +746,7 @@ int vlfb_fbo_bank_scan_dt(const void* bank, int bank_dtype, const float* q, floa
 #undef VLFB_SCAN
   VLFB_CHECK_LAUNCH();
   launch_k(fbo_bank_combine_k, dim3((unsigned)(D / 256), (unsigned)R), 256, 0, ST(stream), (const float*)part_acc,
-           (const float*)part_ml, out, prob, S, D, L, tf32_out);
+           (const float*)part_ml, out, prob, S, D, L, tf32_out, live_rows);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }

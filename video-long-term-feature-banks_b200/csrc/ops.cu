@@ -3,6 +3,7 @@
 // All activations fp32 channels-last; 128-bit loads/stores wherever the channel extent allows;
 // grids are sized in multiples of the 132 SMs (common.cuh: stream_grid).
 #include <float.h>
+#include <limits.h>
 
 #include "common.cuh"
 
@@ -232,15 +233,22 @@ __device__ __forceinline__ bool roi_sample(const RoiBox& b, int ph, int pw, int 
   return true;
 }
 
+// live (device scalar or NULL = all rows): rows r >= *live are padding -- written as zeros, their boxes never read.
 __global__ void roi_align_fwd_k(const float* __restrict__ feat, const float* __restrict__ rois, float* __restrict__ out,
-                                int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total) {
+                                int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total,
+                                const int32_t* __restrict__ live) {
   const int c4 = C >> 2;
+  const int nlive = live != nullptr ? *live : INT_MAX;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % c4) * 4;
     int64_t q = i / c4;
     const int pw = (int)(q % PW); q /= PW;
     const int ph = (int)(q % PH); q /= PH;
     const int r = (int)q;
+    if (r >= nlive) {
+      *reinterpret_cast<float4*>(out + i * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      continue;
+    }
     const RoiBox b = roi_box(rois + r * 5, scale, PH, PW, sr);
     const float* f = feat + (int64_t)b.batch * H * W * C + c;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -261,14 +269,17 @@ __global__ void roi_align_fwd_k(const float* __restrict__ feat, const float* __r
 }
 
 __global__ void roi_align_bwd_k(const float* __restrict__ dout, const float* __restrict__ rois, float* __restrict__ dfeat,
-                                int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total) {
+                                int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total,
+                                const int32_t* __restrict__ live) {
   const int c4 = C >> 2;
+  const int nlive = live != nullptr ? *live : INT_MAX;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % c4) * 4;
     int64_t q = i / c4;
     const int pw = (int)(q % PW); q /= PW;
     const int ph = (int)(q % PH); q /= PH;
     const int r = (int)q;
+    if (r >= nlive) continue;                            // padding row: neither read nor scattered
     const RoiBox b = roi_box(rois + r * 5, scale, PH, PW, sr);
     float* f = dfeat + (int64_t)b.batch * H * W * C + c;
     const float cnt = (float)(b.gh * b.gw);
@@ -293,12 +304,15 @@ __global__ void roi_align_bwd_k(const float* __restrict__ dout, const float* __r
 // zeroes it, then walks its bins and samples in the order roi_align_bwd_k visits them, adding each contribution
 // without atomics.  Pass 2 (roi_scatter_det_k) adds the slabs of each feature map's RoIs in RoI order.
 __global__ void roi_align_bwd_det_k(const float* __restrict__ dout, const float* __restrict__ rois, float* __restrict__ scratch,
-                                    int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total) {
+                                    int H, int W, int C, int PH, int PW, float scale, int sr, int64_t total,
+                                    const int32_t* __restrict__ live) {
   const int c4 = C >> 2;
   const int64_t hwc = (int64_t)H * W * C;
+  const int nlive = live != nullptr ? *live : INT_MAX;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(i % c4) * 4;
     const int r = (int)(i / c4);
+    if (r >= nlive) continue;                            // padding row: its slab is never read by pass 2
     float* f = scratch + r * hwc + c;
     for (int64_t p = 0; p < (int64_t)H * W; ++p) *reinterpret_cast<float4*>(f + p * C) = make_float4(0.f, 0.f, 0.f, 0.f);
     const RoiBox b = roi_box(rois + r * 5, scale, PH, PW, sr);
@@ -326,9 +340,10 @@ __global__ void roi_align_bwd_det_k(const float* __restrict__ dout, const float*
 
 // pass 2: dfeat[n][p][c] += sum over the RoIs r of feature map n, in RoI order, of scratch[r][p][c]
 __global__ void roi_scatter_det_k(const float* __restrict__ scratch, const float* __restrict__ rois, float* __restrict__ dfeat,
-                                  int HW, int C, int R, int64_t total) {
+                                  int HW, int C, int R, int64_t total, const int32_t* __restrict__ live) {
   const int c4 = C >> 2;
   const int64_t hwc = (int64_t)HW * C;
+  if (live != nullptr) R = min(R, *live);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t pc = i % ((int64_t)HW * c4);
     const int n = (int)(i / ((int64_t)HW * c4));
@@ -899,22 +914,32 @@ int vlfb_avgpool3d_bwd(const float* dy, float* dx, const vlfb_conv_geom_t* g, in
 
 int vlfb_roi_align_fwd(const float* feat, const float* rois, float* out, int N, int H, int W, int C, int R, int PH,
                        int PW, float spatial_scale, int sampling_ratio, void* stream) {
+  return vlfb_roi_align_fwd_live(feat, rois, out, N, H, W, C, R, PH, PW, spatial_scale, sampling_ratio, nullptr, stream);
+}
+
+int vlfb_roi_align_fwd_live(const float* feat, const float* rois, float* out, int N, int H, int W, int C, int R, int PH,
+                            int PW, float spatial_scale, int sampling_ratio, const int32_t* live_rows, void* stream) {
   VLFB_CHECK_ARG(feat && rois && out && N > 0 && H > 0 && W > 0 && (C & 3) == 0 && R >= 0 && PH > 0 && PW > 0);
   const int64_t total = (int64_t)R * PH * PW * (C >> 2);
   if (total == 0) return VLFB_OK;
   launch_k(roi_align_fwd_k, stream_grid(total, TPB), TPB, 0, ST(stream), feat, rois, out, H, W, C, PH, PW, spatial_scale,
-                                                                  sampling_ratio, total);
+                                                                  sampling_ratio, total, live_rows);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }
 
 int vlfb_roi_align_bwd(const float* dout, const float* rois, float* dfeat, int N, int H, int W, int C, int R, int PH,
                        int PW, float spatial_scale, int sampling_ratio, void* stream) {
+  return vlfb_roi_align_bwd_live(dout, rois, dfeat, N, H, W, C, R, PH, PW, spatial_scale, sampling_ratio, nullptr, stream);
+}
+
+int vlfb_roi_align_bwd_live(const float* dout, const float* rois, float* dfeat, int N, int H, int W, int C, int R, int PH,
+                            int PW, float spatial_scale, int sampling_ratio, const int32_t* live_rows, void* stream) {
   VLFB_CHECK_ARG(dout && rois && dfeat && N > 0 && H > 0 && W > 0 && (C & 3) == 0 && R >= 0 && PH > 0 && PW > 0);
   const int64_t total = (int64_t)R * PH * PW * (C >> 2);
   if (total == 0) return VLFB_OK;
   launch_k(roi_align_bwd_k, stream_grid(total, TPB), TPB, 0, ST(stream), dout, rois, dfeat, H, W, C, PH, PW, spatial_scale,
-                                                                  sampling_ratio, total);
+                                                                  sampling_ratio, total, live_rows);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }
@@ -1157,6 +1182,13 @@ size_t vlfb_roi_align_bwd_det_scratch_bytes(int R, int H, int W, int C) {
 int vlfb_roi_align_bwd_det(const float* dout, const float* rois, float* dfeat, int N, int H, int W, int C, int R, int PH,
                            int PW, float spatial_scale, int sampling_ratio, void* scratch, size_t scratch_bytes,
                            void* stream) {
+  return vlfb_roi_align_bwd_det_live(dout, rois, dfeat, N, H, W, C, R, PH, PW, spatial_scale, sampling_ratio, scratch,
+                                     scratch_bytes, nullptr, stream);
+}
+
+int vlfb_roi_align_bwd_det_live(const float* dout, const float* rois, float* dfeat, int N, int H, int W, int C, int R,
+                                int PH, int PW, float spatial_scale, int sampling_ratio, void* scratch,
+                                size_t scratch_bytes, const int32_t* live_rows, void* stream) {
   VLFB_CHECK_ARG(dout && rois && dfeat && N > 0 && H > 0 && W > 0 && (C & 3) == 0 && C > 0 && R >= 0 && PH > 0 && PW > 0);
   VLFB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(dfeat)) & 15) == 0);   // float4 access
   if (R == 0) return VLFB_OK;
@@ -1168,11 +1200,11 @@ int vlfb_roi_align_bwd_det(const float* dout, const float* rois, float* dfeat, i
   float* sc = static_cast<float*>(scratch);
   const int64_t per_roi = (int64_t)R * (C >> 2);
   launch_k(roi_align_bwd_det_k, stream_grid(per_roi, TPB), TPB, 0, ST(stream), dout, rois, sc, H, W, C, PH, PW,
-           spatial_scale, sampling_ratio, per_roi);
+           spatial_scale, sampling_ratio, per_roi, live_rows);
   VLFB_CHECK_LAUNCH();
   const int64_t per_pix = (int64_t)N * H * W * (C >> 2);
   launch_k(roi_scatter_det_k, stream_grid(per_pix, TPB), TPB, 0, ST(stream), (const float*)sc, rois, dfeat, H * W, C, R,
-           per_pix);
+           per_pix, live_rows);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }

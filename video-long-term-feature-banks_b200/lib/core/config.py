@@ -106,8 +106,14 @@ __C = _tree({
     # B200.DETERMINISTIC: nets created while it is True run every cross-thread float reduction in a fixed order (no float
     #   atomics with more than one contribution per element), so that two runs of the same calls from the same state are
     #   bitwise identical on one GPU model and library build (DESIGN.md 4.5).  A guarantee, not a speed: off by default.
+    # B200.ROI_CAPACITY: C > 0 = nets created while it is set that have a RoIAlign on 'proposals{sfx}' (AVA train, test and
+    #   lfb_infer_only nets) keep their per-RoI inputs (proposals, labels, original_boxes, metadata, lfb) in buffers of C
+    #   rows, so a batch with any number r <= C of boxes replays the same captured step; a device-side count tells the
+    #   kernels which rows are real, and FetchBlob returns the r live rows.  C is a memory and compute budget the data
+    #   pipeline chooses (clips per GPU x boxes per clip after the detection threshold).  0 = the RoI count is part of
+    #   the captured graph's key, as before (DESIGN.md 4.6).
     'B200': {'COMPUTE': 'tf32', 'GEMM_BACKEND': 'tcgen05', 'CUDA_GRAPH': True, 'FBO_FOLD': True, 'FBO_STACK': True,
-             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False},
+             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False, 'ROI_CAPACITY': 0},
 })
 config = __C
 _DEFAULTS = None

@@ -166,13 +166,22 @@ class DeviceLfb(object):
 
     def feed(self, blob_name, index_table):
         """Assemble the windows directly into the net's `lfb{suffix}` input blob (what FeedBlob(name, windows) would
-        have produced, TF32 rounding of the GEMM operand included) -- R*L*4 bytes cross PCIe instead of R*L*dim*4."""
+        have produced, TF32 rounding of the GEMM operand included) -- R*L*4 bytes cross PCIe instead of R*L*dim*4.
+        In a B200.ROI_CAPACITY net the table is extended to C rows with -1 (zero windows), as FeedBlob pads."""
         from vlfb import workspace
         name = workspace._unscoped(blob_name)
+        cap = workspace._roi_rows(name, np.shape(index_table))
+        rows = int(np.shape(index_table)[0]) if cap is not None else None
+        if cap is not None:
+            table = np.full((cap,) + tuple(np.shape(index_table)[1:]), -1, dtype=np.int32)
+            table[:rows] = np.asarray(index_table)
+            index_table = table
         shape = tuple(np.shape(index_table)) + (self.dim,)
         dst = workspace._static(name, shape, self.bank.dtype)
         self.gather(index_table, out=dst, tf32_out=True)
         workspace.bank_companion(name, dst)                  # B200.LFB_DTYPE 'bf16': the scan operand of the folded FBO
+        if cap is not None:
+            workspace.set_live_rows(name, rows)
         ws = workspace.current()
         ws.blobs[name] = dst
         ws.rounded.add(name)

@@ -20,6 +20,7 @@ import os
 import torch
 
 from . import kernels as K_default
+from .libvlfb import VlfbError
 
 K = K_default          # tests may swap in a torch-CPU kernel set (tests/fake_kernels.py)
 DEVICE = 'cuda'
@@ -35,11 +36,19 @@ RELU_BITS = os.environ.get('VLFB_RELU_BITS', '1') == '1'
 # max-pool backward in gather form (no fill, no atomics, pool1 folds conv1's ReLU backward + rounding); '0' = the scatter
 # form (zero fill + one atomic per output element + the separate ReLU-backward pass)
 POOL_GATHER = int(os.environ.get('VLFB_POOL_GATHER', '1'))     # 2 = gather form only for non-overlapping windows
+# the per-RoI inputs of an AVA net (model_builder_video.py), suffixed like 'proposals{sfx}': B200.ROI_CAPACITY buffers
+ROI_INPUTS = ('proposals', 'labels', 'original_boxes', 'metadata', 'lfb')
 
 
 def _mm(ctx):
     """The matmul of this net: the deterministic form in a B200.DETERMINISTIC net."""
     return K.matmul_det if ctx.net.det else K.matmul
+
+
+def _live_kw(ctx, blob):
+    """{'live_rows': device count} when `blob` is RoI-indexed in a B200.ROI_CAPACITY net, else {} (all rows)."""
+    live = ctx.net.live_rows(blob)
+    return {} if live is None else {'live_rows': live}
 
 
 def set_backend(kernels_module, device, dtype=torch.float32):
@@ -758,7 +767,7 @@ class FboFoldStep(Step):
         _mm(ctx)(u, w1, q)
         s = empty((R, D))
         prob = empty((R, L_)) if self.prob_name else None
-        K.fbo_bank_scan(bank, q.view(R, D), s, self.scale, prob=prob, tf32_out=True)
+        K.fbo_bank_scan(bank, q.view(R, D), s, self.scale, prob=prob, tf32_out=True, **_live_kw(ctx, self.theta))
         t = empty((1, R, d1))
         _mm(ctx)(s.view(1, R, D), w1.transpose(1, 2), t, bias=None if self.b1 is None else P.phys(self.b1),
                  tf32_out=True)
@@ -837,6 +846,7 @@ class FboStackStep(Step):
             ld['drop_offset'] = ctx.ws.next_rng(R * dA)[1] if dropout else 0
             layers.append(ld)
         cfgd = self._cfg(ctx, R, L_, dropout)
+        cfgd.update(_live_kw(ctx, self.op.inputs[0]))
         K.fbo_nl_fwd(cfgd, layers, a0, bp)
         outs = self.op.outputs
         for li, ld in enumerate(layers):
@@ -1006,20 +1016,21 @@ class RoIAlignStep(Step):
         fp = phys(feat)                               # [N,H,W,C]
         r = rois.shape[0]
         y = cl_alloc((r, feat.shape[1], a['pooled_h'], a['pooled_w']))
-        K.roi_align_fwd(fp, rois, phys(y), a['spatial_scale'], a['sampling_ratio'])
+        live = _live_kw(ctx, self.op.inputs[1])
+        K.roi_align_fwd(fp, rois, phys(y), a['spatial_scale'], a['sampling_ratio'], **live)
         ctx.put(self.op.outputs[0], y)
-        ctx.saved[id(self)] = (rois, feat.shape, feat.stride())
+        ctx.saved[id(self)] = (rois, feat.shape, feat.stride(), live)
 
     def bwd(self, ctx):
         gy = ctx.pop_grad(self.out_keys[0])
         if gy is None:
             return
-        rois, shape, stride = ctx.saved.pop(id(self))
+        rois, shape, stride, live = ctx.saved.pop(id(self))
         a = self.op.args
         d = torch.empty_strided(shape, stride, dtype=DTYPE, device=DEVICE)
         K.fill(flat(d), 0.0)
         roi_bwd = K.roi_align_bwd_det if ctx.net.det else K.roi_align_bwd
-        roi_bwd(phys(gy), rois, phys(d), a['spatial_scale'], a['sampling_ratio'])
+        roi_bwd(phys(gy), rois, phys(d), a['spatial_scale'], a['sampling_ratio'], **live)
         ctx.add_grad(self.in_keys[0], d, owned=True)
 
 
@@ -1136,6 +1147,66 @@ class CompiledNet(object):
             produced.update(op.outputs)
         self._graphs = collections.OrderedDict()     # input signature -> captured step (LRU)
         self._eager_runs = {}                        # input signature -> eager runs so far (two before capture)
+        self._setup_roi_capacity(int(cfg.B200.get('ROI_CAPACITY', 0)), ops)
+
+    # ---- B200.ROI_CAPACITY (DESIGN.md 4.6)
+    def _setup_roi_capacity(self, cap, ops):
+        """A net with a RoIAlign on 'proposals{sfx}' is lowered at C = cap RoI rows: its per-RoI inputs are registered
+        with the workspace (fed into C-row buffers, with a device live count r), and every blob computed from them along
+        the leading dimension is marked RoI-indexed (the kernels that can skip padding rows get the live count; FetchBlob
+        returns the r live rows)."""
+        self.roi_capacity, self.roi_inputs, self.roi_sfx, self.roi_blobs = 0, [], None, set()
+        rois = [op.inputs[1] for op in ops if op.type == 'RoIAlign' and op.inputs[1].startswith('proposals')]
+        if cap <= 0 or not rois:
+            return
+        sfx = rois[0][len('proposals'):]
+        for op in ops:
+            if op.type == 'SoftmaxWithLoss':
+                raise VlfbError('%s: B200.ROI_CAPACITY = %d on a net with SoftmaxWithLoss (%s), whose mean over rows would '
+                                'count the padding rows' % (self.name, cap, op.outputs[-1]))
+        names = set(p + sfx for p in ROI_INPUTS)
+        self.roi_capacity, self.roi_sfx = cap, sfx
+        self.roi_inputs = [n for n in self.external_inputs if n in names]
+        marked = set(self.roi_inputs)
+        for st in self.steps:
+            if isinstance(st, (SigmoidCELossStep, SoftmaxCELossStep)):
+                continue                                      # a reduction over all rows
+            ins = [k[0] for k in st.in_keys] + ([st.res_key[0]] if isinstance(st, ConvStep) and st.res_key else [])
+            if not any(n in marked for n in ins):
+                continue
+            outs = [k[0] for k in st.out_keys]
+            marked.update(outs[:1] if isinstance(st, SpatialBNStep) else outs)   # not the per-channel statistics
+            if isinstance(st, FboFoldStep) and st.prob_name:
+                marked.add(st.prob_name)
+        self.roi_blobs = marked
+        self._roi_marks = dict((n, (cap, sfx)) for n in marked)
+        if self.ws is None:
+            return                                            # the builder's gradient analysis (data_parallel.py)
+        for n in self.roi_inputs:
+            self.ws.roi_capacity[n] = (cap, sfx)
+        self.ws.roi_blobs.update(self._roi_marks)
+
+    def live_rows(self, blob):
+        """The device live count when `blob` is RoI-indexed in this net, else None."""
+        if blob not in self.roi_blobs:
+            return None
+        return self.ws.roi_live[self.roi_sfx][0]
+
+    def _check_roi_rows(self):
+        """Every per-RoI input holds C rows and was fed the same number of live rows for this step."""
+        ws = self.ws
+        fed = {}
+        for n in self.roi_inputs:
+            t = ws.blobs.get(n)
+            if not isinstance(t, torch.Tensor):
+                continue
+            if int(t.shape[0]) != self.roi_capacity or n not in ws.roi_fed:
+                raise VlfbError('%s: %d rows, not a B200.ROI_CAPACITY = %d buffer (fed before net %s was created?)'
+                                % (n, int(t.shape[0]), self.roi_capacity, self.name))
+            fed[n] = ws.roi_fed[n]
+        if len(set(fed.values())) > 1:
+            raise VlfbError('per-RoI inputs of one step fed with different RoI counts: %s'
+                            % ', '.join('%s %d' % kv for kv in sorted(fed.items())))
 
     # ---- SSA-style versioning of in-place blobs
     def _version(self, ops):
@@ -1414,6 +1485,9 @@ class CompiledNet(object):
         eager between the two captured halves.  Graphs are cached per input signature (e.g. per RoI count)."""
         from core.config import config as cfg
         ws = self.ws
+        if self.roi_capacity:
+            self._check_roi_rows()
+            ws.roi_blobs.update(self._roi_marks)        # names shared with another net (train / test) are this net's now
         ws.begin_run()
         if self.det:
             # every run draws the dropout offsets its first run drew, as a graph replay does (the step counter varies

@@ -554,30 +554,41 @@ def avgpool_bwd(dy, dx, g, accumulate=False):
             'avgpool_bwd')
 
 
-def roi_align_fwd(feat, rois, out, spatial_scale, sampling_ratio=0):
-    """feat [N,H,W,C], rois [R,5], out [R,PH,PW,C]."""
+def _live(live_rows):
+    """Device int32 scalar of a B200.ROI_CAPACITY net (rows >= its value are padding), or None = all rows."""
+    if live_rows is not None:
+        assert live_rows.dtype == torch.int32 and live_rows.numel() == 1 and live_rows.is_cuda
+    return _ptr(live_rows)
+
+
+def roi_align_fwd(feat, rois, out, spatial_scale, sampling_ratio=0, live_rows=None):
+    """feat [N,H,W,C], rois [R,5], out [R,PH,PW,C].  live_rows: rows >= live_rows[0] are written as zeros, their boxes
+    never read."""
     n, h, w, c = feat.shape
     r, ph, pw, _ = out.shape
-    _check(L.load().vlfb_roi_align_fwd(_ptr(_f32c(feat)), _ptr(_f32c(rois)), _ptr(_f32c(out)), n, h, w, c, r, ph, pw,
-                                        float(spatial_scale), int(sampling_ratio), _stream()), 'roi_align_fwd')
+    _check(L.load().vlfb_roi_align_fwd_live(_ptr(_f32c(feat)), _ptr(_f32c(rois)), _ptr(_f32c(out)), n, h, w, c, r, ph, pw,
+                                             float(spatial_scale), int(sampling_ratio), _live(live_rows), _stream()),
+           'roi_align_fwd')
 
 
-def roi_align_bwd(dout, rois, dfeat, spatial_scale, sampling_ratio=0):
+def roi_align_bwd(dout, rois, dfeat, spatial_scale, sampling_ratio=0, live_rows=None):
     n, h, w, c = dfeat.shape
     r, ph, pw, _ = dout.shape
-    _check(L.load().vlfb_roi_align_bwd(_ptr(_f32c(dout)), _ptr(_f32c(rois)), _ptr(_f32c(dfeat)), n, h, w, c, r, ph,
-                                        pw, float(spatial_scale), int(sampling_ratio), _stream()), 'roi_align_bwd')
+    _check(L.load().vlfb_roi_align_bwd_live(_ptr(_f32c(dout)), _ptr(_f32c(rois)), _ptr(_f32c(dfeat)), n, h, w, c, r, ph,
+                                             pw, float(spatial_scale), int(sampling_ratio), _live(live_rows), _stream()),
+           'roi_align_bwd')
 
 
-def roi_align_bwd_det(dout, rois, dfeat, spatial_scale, sampling_ratio=0):
+def roi_align_bwd_det(dout, rois, dfeat, spatial_scale, sampling_ratio=0, live_rows=None):
     """roi_align_bwd in a fixed summation order (vlfb_roi_align_bwd_det); the per-RoI scratch is allocated here."""
     n, h, w, c = dfeat.shape
     r, ph, pw, _ = dout.shape
     lib = L.load()
     nbytes = int(lib.vlfb_roi_align_bwd_det_scratch_bytes(r, h, w, c))
     scratch = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=dfeat.device)
-    _check(lib.vlfb_roi_align_bwd_det(_ptr(_f32c(dout)), _ptr(_f32c(rois)), _ptr(_f32c(dfeat)), n, h, w, c, r, ph, pw,
-                                      float(spatial_scale), int(sampling_ratio), _ptr(scratch), nbytes, _stream()),
+    _check(lib.vlfb_roi_align_bwd_det_live(_ptr(_f32c(dout)), _ptr(_f32c(rois)), _ptr(_f32c(dfeat)), n, h, w, c, r, ph, pw,
+                                           float(spatial_scale), int(sampling_ratio), _ptr(scratch), nbytes,
+                                           _live(live_rows), _stream()),
            'roi_align_bwd_det')
 
 
@@ -749,6 +760,7 @@ def _fbo_structs(cfgd, layers):
     c.ln_eps, c.drop_ratio, c.seed = float(cfgd.get('ln_eps', 1e-5)), float(cfgd.get('drop_ratio', 0.0)), int(cfgd.get('seed', 0))
     step = cfgd.get('step')
     c.step = step.data_ptr() if step is not None else None
+    c.live_rows = _live(cfgd.get('live_rows'))
     arr = (L.FboLayer * len(layers))()
     for i, ld in enumerate(layers):
         for k in FBO_LAYER_KEYS:
@@ -763,7 +775,7 @@ def _fbo_structs(cfgd, layers):
 
 def fbo_nl_fwd(cfgd, layers, a0, bp):
     """All FBO-NL layers forward in one launch.  cfgd: R, L, dA, d, dB, scale, pre_act_ln, [ln_eps, drop_ratio, seed,
-    step]; layers: dicts of tensors keyed by FBO_LAYER_KEYS (weights [out][in], saved activations [R][...])."""
+    step, live_rows]; layers: dicts of tensors keyed by FBO_LAYER_KEYS (weights [out][in], saved activations [R][...])."""
     _f32c(a0, 'a0'), _f32c(bp, 'bp')
     assert tuple(a0.shape) == (cfgd['R'], cfgd['dA']) and tuple(bp.shape) == (cfgd['R'], cfgd['L'], cfgd['dB'])
     c, arr = _fbo_structs(cfgd, layers)
@@ -785,10 +797,10 @@ def fbo_nl_bwd(cfgd, layers, a0, bp, da_last, da0, dbp):
 
 
 # --------------------------------------------------------------------------- raw feature-bank kernels (csrc/fbo.cu)
-def fbo_bank_scan(bank, q, out, scale, prob=None, tf32_out=False):
+def fbo_bank_scan(bank, q, out, scale, prob=None, tf32_out=False, live_rows=None):
     """out[r] = sum_j softmax_j(scale * q[r].bank[r,j]) * bank[r,j]: the folded inference-mode FBO-NL layer, one pass
     over the raw bank.  bank [R,L,D] fp32 or bf16 (storage type only: the arithmetic is fp32), q [R,D], out [R,D],
-    prob [R,L] or None."""
+    prob [R,L] or None.  live_rows: rows >= live_rows[0] are not scanned (out = 0, prob = 0)."""
     assert bank.is_contiguous() and bank.dtype in (torch.float32, torch.bfloat16), 'bank must be contiguous fp32 / bf16'
     _f32c(q, 'q'), _f32c(out, 'out')
     dt = L.DT_BF16 if bank.dtype == torch.bfloat16 else L.DT_F32
@@ -802,11 +814,11 @@ def fbo_bank_scan(bank, q, out, scale, prob=None, tf32_out=False):
         raise L.VlfbError('fbo_bank_scan: unsupported bank row width %d (fp32: 1024, 2048 or 4096; bf16: 2048 or 4096)' % d)
     wsp = torch.empty(max(nbytes, 4) // 4, dtype=torch.float32, device=bank.device)
     args = (_ptr(bank), dt, _ptr(q), float(scale), _ptr(out), _ptr(prob), r, l, d, int(tf32_out), _ptr(wsp),
-            C.c_size_t(nbytes), _stream())
-    _check(lib.vlfb_fbo_bank_scan_dt(*args), 'fbo_bank_scan')
+            C.c_size_t(nbytes), _live(live_rows), _stream())
+    _check(lib.vlfb_fbo_bank_scan_live(*args), 'fbo_bank_scan')
     if _PROFILE is not None:
         _PROFILE.append(('fbo_bank_scan R=%d L=%d D=%d %s' % (r, l, d, 'bf16' if dt else 'f32'),
-                         lambda: lib.vlfb_fbo_bank_scan_dt(*args), 4.0 * r * l * d, _nbytes(bank, q, out), LABEL,
+                         lambda: lib.vlfb_fbo_bank_scan_live(*args), 4.0 * r * l * d, _nbytes(bank, q, out), LABEL,
                          (bank, q, out, prob, wsp)))
 
 

@@ -55,7 +55,7 @@ class FboLayer(C.Structure):
 class FboCfg(C.Structure):
     _fields_ = [('R', C.c_int), ('L', C.c_int), ('dA', C.c_int), ('d', C.c_int), ('dB', C.c_int), ('layers', C.c_int),
                 ('scale', C.c_float), ('pre_act', C.c_int), ('pre_act_ln', C.c_int), ('ln_eps', C.c_float),
-                ('drop_ratio', C.c_float), ('seed', C.c_uint64), ('step', C.c_void_p)]
+                ('drop_ratio', C.c_float), ('seed', C.c_uint64), ('step', C.c_void_p), ('live_rows', C.c_void_p)]
 
 
 _P, _I, _L, _F, _U = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64
@@ -131,6 +131,13 @@ DET_SIGNATURES = {
     'vlfb_spatial_bn_fwd_det': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _F, _F, _P, C.c_size_t, _P],
     'vlfb_spatial_bn_bwd_det': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _P, C.c_size_t, _P],
 }
+# include/vlfb_live.h (included by vlfb.h): the entry points with a live row count (B200.ROI_CAPACITY)
+LIVE_SIGNATURES = {
+    'vlfb_roi_align_fwd_live': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P],
+    'vlfb_roi_align_bwd_live': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P],
+    'vlfb_roi_align_bwd_det_live': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _I, _P, C.c_size_t, _P, _P],
+    'vlfb_fbo_bank_scan_live': [_P, _I, _P, _F, _P, _P, _I, _I, _I, _I, _P, C.c_size_t, _P, _P],
+}
 RESTYPES = {'vlfb_last_error': C.c_char_p, 'vlfb_roi_align_bwd_det_scratch_bytes': C.c_size_t, 'vlfb_fbo_bank_scan_workspace': C.c_size_t,
             'vlfb_fbo_bank_scan_workspace_dt': C.c_size_t,
             'vlfb_fbo_nl_scratch_floats': C.c_size_t,
@@ -149,7 +156,7 @@ def load():
             'libvlfb.so not found at %s -- build it first (python -c "import __graft_entry__ as g; '
             'g.build()" or make -C csrc).  There is no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, argtypes in list(SIGNATURES.items()) + list(DET_SIGNATURES.items()):
+    for name, argtypes in list(SIGNATURES.items()) + list(DET_SIGNATURES.items()) + list(LIVE_SIGNATURES.items()):
         fn = getattr(lib, name)        # AttributeError if the symbol is missing
         fn.argtypes = argtypes
         fn.restype = RESTYPES.get(name, C.c_int)

@@ -12,9 +12,11 @@ import numpy as np
 import torch
 
 from . import executor as X
+from .libvlfb import VlfbError
 
 _SCOPE = re.compile(r'^gpu_\d+/')
 STEM_PAD_L, STEM_PAD_R = 3, 5          # zero pixels around every row of a fed clip (conv1: kW = 7, pad 3, stride 2)
+_INT_DTYPES = (torch.int32, torch.int64, torch.uint8, torch.bool, torch.int16, torch.int8)
 
 
 def _unscoped(name):
@@ -215,6 +217,13 @@ class Workspace(object):
         self.force_eager = False
         self.step = 0
         self._step_t = None
+        # B200.ROI_CAPACITY (DESIGN.md 4.6): per-RoI input name -> (capacity C, suffix), registered by the nets that use
+        # it; RoI-indexed blob name -> (C, suffix) (FetchBlob returns the live rows); suffix -> [device int32 live count,
+        # host copy]; per-RoI input name -> the row count of its last feed
+        self.roi_capacity = {}
+        self.roi_blobs = {}
+        self.roi_live = {}
+        self.roi_fed = {}
 
     def begin_run(self):
         """Advance the device-side step counter (dropout masks of captured graphs depend on it)."""
@@ -357,8 +366,14 @@ def EnqueueBlobs(feed):
     with torch.cuda.stream(ws.copy_stream):
         for name, arr in feed.items():
             src = arr if isinstance(arr, torch.Tensor) else torch.as_tensor(np.ascontiguousarray(arr))
-            is_int = src.dtype in (torch.int32, torch.int64, torch.uint8, torch.bool, torch.int16, torch.int8)
-            st = _static('%s/stage%d' % (_unscoped(name), slot), src.shape, torch.int32 if is_int else X.DTYPE)
+            is_int = src.dtype in _INT_DTYPES
+            shape = tuple(src.shape)
+            cap = _roi_rows(_unscoped(name), shape)
+            if cap is not None:
+                shape = (cap,) + shape[1:]              # a per-RoI input: the slot keeps its C-row shape and address
+            st = _static('%s/stage%d' % (_unscoped(name), slot), shape, torch.int32 if is_int else X.DTYPE)
+            if cap is not None:
+                st = st[:src.shape[0]]
             st.copy_(src, non_blocking=True)
             staged[_unscoped(name)] = st
         ev = torch.cuda.Event()
@@ -392,11 +407,52 @@ def _static(key, shape, dtype):
     return t
 
 
+def _roi_rows(name, shape):
+    """Capacity C when `name` is a per-RoI input of a B200.ROI_CAPACITY net (None otherwise), after checking that the
+    `shape[0]` rows fed fit it."""
+    ent = _ws.roi_capacity.get(name)
+    if ent is None:
+        return None
+    cap = ent[0]
+    r = int(shape[0]) if len(shape) else 0
+    if not 1 <= r <= cap:
+        raise VlfbError('%s: %d RoI rows fed; B200.ROI_CAPACITY = %d holds 1 to %d' % (name, r, cap, cap))
+    return cap
+
+
+def set_live_rows(name, rows):
+    """Record that per-RoI input `name` was fed `rows` live rows: the host copy, and the device count the kernels read,
+    written in stream order behind the feed."""
+    sfx = _ws.roi_capacity[name][1]
+    ent = _ws.roi_live.get(sfx)
+    if ent is None:
+        ent = _ws.roi_live[sfx] = [torch.zeros(1, dtype=torch.int32, device=X.DEVICE), 0]
+    ent[0].fill_(int(rows))
+    ent[1] = int(rows)
+    _ws.roi_fed[name] = int(rows)
+
+
+def _input_buffer(name, src, dtype):
+    """The static device buffer of input `name` holding `src`.  A per-RoI input of a B200.ROI_CAPACITY net gets C rows:
+    the r fed rows, then rows [r, C) rewritten with padding at every feed (labels -1, the sigmoid loss's ignore value;
+    anything else 0), so that its shape and address never change and no padded row holds stale or uninitialised data."""
+    cap = _roi_rows(name, tuple(src.shape))
+    if cap is None:
+        dst = _static(name, src.shape, dtype)
+        dst.copy_(src, non_blocking=True)
+        return dst
+    r = int(src.shape[0])
+    dst = _static(name, (cap,) + tuple(src.shape[1:]), dtype)
+    dst[:r].copy_(src, non_blocking=True)
+    dst[r:].fill_(-1 if name.startswith('labels') else 0)
+    set_live_rows(name, r)
+    return dst
+
+
 def _feed_activation(name, arr):
     src = arr if isinstance(arr, torch.Tensor) else torch.as_tensor(np.ascontiguousarray(arr))
-    if src.dtype in (torch.int32, torch.int64, torch.uint8, torch.bool, torch.int16, torch.int8):
-        dst = _static(name, src.shape, torch.int32)
-        dst.copy_(src, non_blocking=True)
+    if src.dtype in _INT_DTYPES:
+        dst = _input_buffer(name, src, torch.int32)
         _ws.blobs[name] = dst
         _ws.rounded.discard(name)
         return
@@ -429,8 +485,7 @@ def _feed_activation(name, arr):
         _ws.blobs[name] = p.permute(0, 4, 1, 2, 3)
         _ws.rounded.add(name)
         return
-    dst = _static(name, src.shape, X.DTYPE)
-    dst.copy_(src, non_blocking=True)
+    dst = _input_buffer(name, src, X.DTYPE)
     bank_companion(name, dst)
     if dst.dim() >= 2 and dst.shape[-1] >= 64:                    # feature banks are GEMM operands
         X.K.round_tf32(dst.view(-1), dst.view(-1))
@@ -480,8 +535,8 @@ def FeedBlob(name, arr, device_option=None):
 class _PendingFetch(object):
     """Handle returned by FetchBlobAsync: .get() waits for the device->host copy and returns the numpy value."""
 
-    def __init__(self, host, event, scalar):
-        self._host, self._event, self._scalar = host, event, scalar
+    def __init__(self, host, event, scalar, rows=None):
+        self._host, self._event, self._scalar, self._rows = host, event, scalar, rows
 
     def ready(self):
         return self._event is None or self._event.query()
@@ -490,6 +545,8 @@ class _PendingFetch(object):
         if self._event is not None:
             self._event.synchronize()
         a = self._host if isinstance(self._host, np.ndarray) else self._host.numpy().copy()
+        if self._rows is not None:
+            a = a[:self._rows]
         return a.reshape(()) if (self._scalar and a.size == 1) else a
 
 
@@ -517,7 +574,15 @@ def FetchBlobAsync(name):
     host.copy_(t, non_blocking=True)         # strided logical views are copied element-wise: logical layout on the host
     ev = torch.cuda.Event()
     ev.record(torch.cuda.current_stream())
-    return _PendingFetch(host, ev, scalar)
+    return _PendingFetch(host, ev, scalar, live_rows(name, t))
+
+
+def live_rows(name, t):
+    """Number of live rows of blob `name` (tensor t) when it is RoI-indexed in a B200.ROI_CAPACITY net, else None."""
+    ent = _ws.roi_blobs.get(name)
+    if ent is None or t.dim() == 0 or int(t.shape[0]) != ent[0] or ent[1] not in _ws.roi_live:
+        return None
+    return _ws.roi_live[ent[1]][1]
 
 
 def FetchBlob(name):
@@ -534,6 +599,9 @@ def FetchBlob(name):
         return np.array(t, dtype=np.int64)
     if t.dim() == 5 and t.shape[1] == 4 and name.startswith('data'):
         t = t[:, :3]
+    rows = live_rows(name, t)
+    if rows is not None:
+        t = t[:rows]
     a = t.detach().cpu().contiguous().numpy()
     if not t.is_cuda:
         a = a.copy()              # the CPU test engine would otherwise hand out a view of a reusable input buffer
