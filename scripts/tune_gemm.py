@@ -45,15 +45,14 @@ def timeit(fn, reps=5):
 
 
 def main():
-    configs = [dict(), dict(VLFB_FENCE='1'), dict(VLFB_FENCE='1', VLFB_LAG='3'), dict(VLFB_FENCE='1', VLFB_LAG='4'),
-               dict(VLFB_LAG='1'), dict(VLFB_LAG='3'), dict(VLFB_TMA='0'), dict(VLFB_TMA='0', VLFB_FENCE='1', VLFB_LAG='3')]
+    configs = [dict(), dict(VLFB_LAG='1'), dict(VLFB_LAG='3'), dict(VLFB_TMA='0')]
     for name, shp in SHAPES.items():
         g, x, w, y, wt = make(*shp)
         dw = torch.zeros_like(w)
         dx = torch.empty_like(x)
         flops = 2.0 * g.N * g.To * g.Ho * g.Wo * g.Co * g.C * g.kT * g.kH * g.kW
         for cfg in configs:
-            for k in ('VLFB_BN', 'VLFB_STAGES', 'VLFB_LAG', 'VLFB_TMA', 'VLFB_FENCE'):
+            for k in ('VLFB_BN', 'VLFB_STAGES', 'VLFB_LAG', 'VLFB_TMA'):
                 os.environ.pop(k, None)
             os.environ.update(cfg)
             tf = timeit(lambda: K.conv_fwd(x, w, y, g, relu=True, tf32_out=True))

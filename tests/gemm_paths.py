@@ -55,14 +55,12 @@ CONFIGS = {
     'default': {},
     'tma0': {'VLFB_TMA': '0'},
     'im2col0': {'VLFB_IM2COL': '0'},
-    'tmamn0': {'VLFB_TMA_MN': '0'},
-    'fuse0': {'VLFB_FUSE_ATOMS': '0'},
     'nopatch': {'VLFB_NO_PATCH': '1'},
     'nopar': {'VLFB_NO_PAR': '1'},
 }
 # every environment override of the GEMM (a configuration sets some of them; the rest must be unset)
-SWITCHES = ('VLFB_TMA', 'VLFB_IM2COL', 'VLFB_TMA_MN', 'VLFB_FUSE_ATOMS', 'VLFB_NO_PATCH', 'VLFB_NO_PAR', 'VLFB_BN',
-            'VLFB_STAGES', 'VLFB_LAG', 'VLFB_SK', 'VLFB_DEBUG')
+SWITCHES = ('VLFB_TMA', 'VLFB_IM2COL', 'VLFB_NO_PATCH', 'VLFB_NO_PAR', 'VLFB_BN', 'VLFB_STAGES', 'VLFB_LAG', 'VLFB_SK',
+            'VLFB_DEBUG')
 
 OP_DENSE_K, OP_DENSE_MN, OP_CONV_K, OP_DGRAD_K, OP_CONV_MN, OP_STEM_K, OP_STEM_MN = range(7)
 
@@ -111,7 +109,8 @@ def _case(name, op, seed, runs, **kw):
 
 # runs: configuration -> the path fields the case must take there (kinds / mask / tma / cp / bn / sk / fix / lean /
 # bits2 / patch / par / split as printed by VLFB_DEBUG).  Kinds: 0 DENSE_K, 1 DENSE_MN, 2 CONV_K, 3 DGRAD_K, 4 CONV_MN,
-# 5 STEM_K, 6 STEM_MN.  tma_a: 0 cp.async, 1 TMA tiled, 2 im2col, 3 stem, 4 fused MN atoms; tma_b adds 5 = conv_flat.
+# 5 STEM_K, 6 STEM_MN.  tma_a: 0 cp.async, 1 TMA tiled, 2 im2col, 3 stem; tma_b: 0 cp.async, 1 TMA tiled.  MN-major
+# operands always report 0.
 CASES = []
 
 
@@ -170,10 +169,8 @@ _add('dgrad_pointwise_float_mask', 'conv_dgrad', 12, geom=G(2, 3, 6, 6, 64, 160,
      epi=dict(residual=True, mask_float=True, tf32=True),
      runs={'default': dict(kinds=(0, 0), mask=1, tma=(1, 1), cp=0, lean=1),
            'tma0': dict(kinds=(0, 0), mask=1, tma=(0, 0), cp=1)})
-# ---- convolution wgrad (kernels.conv_wgrad): DENSE_MN x CONV_MN / STEM_MN, atomic, split or stream-K.  On sm_90a every
-# MN-major operand is staged by cp.async: the tensor maps of the MN-major TMA paths (make_tmap_mn / _mn4, the wgrad
-# im2col and conv_flat maps, the conv1 wgrad rows and patches) use CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, which the H100
-# driver does not encode, so launch() falls back to the gather loaders (UNREACHABLE_SM90 in test_gpu_gemm_paths.py).
+# ---- convolution wgrad (kernels.conv_wgrad): DENSE_MN x CONV_MN / STEM_MN, atomic, split or stream-K.  Both operands
+# are MN-major, so every wgrad is staged by the cp.async gather loaders (cp=1, tma=0,0) whatever the switches say.
 _add('wgrad_3x3', 'conv_wgrad', 13, geom=G(2, 3, 9, 10, 32, 64, (1, 3, 3), pd=(0, 1, 1)),
      epi=dict(row_scale=True),
      runs={'default': dict(kinds=(1, 4), tma=(0, 0), cp=1),
@@ -187,9 +184,9 @@ _add('wgrad_c36', 'conv_wgrad', 15, geom=G(1, 2, 6, 6, 36, 64, (1, 3, 3), pd=(0,
 _add('wgrad_stream_k_atomic', 'conv_wgrad', 16, geom=G(2, 8, 14, 14, 64, 64, (1, 3, 3), pd=(0, 1, 1)),
      epi=dict(), opts=dict(stream_k=1),
      runs={'default': dict(kinds=(1, 4), cp=1, sk=1, fix=0)})
-# conv1 wgrad 1x3x3 / stride (1, 2, 2) on a W-padded clip with Wo = 16 and Ho even: the only geometry whose N = 32 kH
-# fits one tile (the patch-chunk form needs it); the requested 96-wide tile is re-planned to 64 (pow2_only) because
-# the MN-major B operand falls back to cp.async
+# conv1 wgrad 1x3x3 / stride (1, 2, 2) on a W-padded clip with Wo = 16 and Ho even: N = 32 kH fits one tile; the
+# requested 96-wide tile becomes 64 (pow2_only) because the cp.async loader of the MN-major B operand needs a
+# power-of-two width
 _add('stem_wgrad_1x3x3_t128', 'conv_wgrad', 17, geom=G(1, 2, 32, 32, 4, 64, (1, 3, 3), st=(1, 2, 2), pd=(0, 1, 1)),
      pitched=True, epi=dict(row_scale=True), opts=dict(tile_n=128),
      runs={'default': dict(kinds=(1, 6), tma=(0, 0), patch=0, cp=1, bn=128),
@@ -220,16 +217,13 @@ _add('raw_kk_t32_tails', 'raw', 23, Z=2, M=129, N=100, K=300, a_mn=False, b_mn=F
            'tma0': dict(kinds=(0, 0), tma=(0, 0), cp=1, bn=32)})
 _add('raw_kmn_t96', 'raw', 24, Z=1, M=192, N=160, K=256, a_mn=False, b_mn=True, gn=4, gm=3,
      epi=dict(scale=True, bias=True, relu=True), opts=dict(tile_n=96),
-     runs={'default': dict(kinds=(0, 1), tma=(1, 0), cp=1, bn=64),          # pow2_only re-plan: MN-major cp.async
-           'tmamn0': dict(kinds=(0, 1), tma=(1, 0), cp=1, bn=64)})
+     runs={'default': dict(kinds=(0, 1), tma=(1, 0), cp=1, bn=64)})          # pow2_only: MN-major B by cp.async
 _add('raw_mnk_t64_k32', 'raw', 25, Z=3, M=236, N=72, K=32, a_mn=True, b_mn=False, gn=4, gm=2,
      epi=dict(bias=True, residual=True), opts=dict(tile_n=64),
-     runs={'default': dict(kinds=(1, 0), tma=(0, 1), cp=1, bn=64),
-           'tmamn0': dict(kinds=(1, 0), tma=(0, 1), cp=1, bn=64)})
+     runs={'default': dict(kinds=(1, 0), tma=(0, 1), cp=1, bn=64)})
 _add('raw_mnmn_t128_accum', 'raw', 26, Z=2, M=256, N=200, K=200, a_mn=True, b_mn=True, gn=4, gm=1,
      epi=dict(accum=True), opts=dict(tile_n=128),
-     runs={'default': dict(kinds=(1, 1), tma=(0, 0), cp=1, bn=128),
-           'fuse0': dict(kinds=(1, 1), tma=(0, 0), cp=1, bn=128)})
+     runs={'default': dict(kinds=(1, 1), tma=(0, 0), cp=1, bn=128)})
 _add('raw_k16_big_bias', 'raw', 27, Z=1, M=127, N=48, K=16, a_mn=False, b_mn=False, gn=4, gm=1,
      epi=dict(bias=True, bias_scale=64.0),
      runs={'default': dict(kinds=(0, 0), tma=(0, 0), cp=1)})

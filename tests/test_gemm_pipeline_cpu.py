@@ -10,7 +10,8 @@ These tests pin the pipeline down:
   - every K loop waits with `DEPBAR.LE gsb0, 0x1` (the previous chunk's MMAs stay in flight);
   - MN-major B with a K-major A (transposed matmul B operands): no full drain inside the K loop at all; MN-major A
     (wgrad, transposed matmul A operands): one drain per chunk, for the single A image;
-  - no register spills, except in three stream-K fix-up builds at the 168-register cap, which may not grow.
+  - no register spills, except in two stream-K fix-up builds at the 168-register cap, which may not grow;
+  - exactly the expected instantiations are built: TMA-only builds (CP = false) for K-major operand pairs only.
 """
 import os
 import re
@@ -25,12 +26,27 @@ import __graft_entry__ as G
 SRC = os.path.join(G.CSRC, 'gemm_tc.cu')
 MN_KINDS = {1, 4, 6}                 # VLFB_OP_DENSE_MN, VLFB_OP_CONV_MN, VLFB_OP_STEM_MN (include/vlfb.h)
 # (A kind, B kind, MASK, CP, FIX) -> spill-store bytes allowed
-# The two MASK builds spilled before the pipeline was restored.  The wgrad (DENSE_MN x CONV_MN) fix-up build spills since
-# the B images are double-buffered (the 4 x 4 rewrite holds 16 more registers at the 168 cap).  It is fed by TMA only,
-# and the MN-major TMA maps cannot be encoded on sm_90a (tests/gemm_paths.py UNREACHABLE_SM90), so no launch runs it;
-# the entry must go when those maps are re-encoded and the build becomes reachable.
-SPILL_ALLOWED = {(0, 0, 1, 0, 1): 24, (3, 0, 1, 0, 1): 12, (1, 4, 0, 0, 1): 8}
+# The two MASK builds spilled before the pipeline was restored.
+SPILL_ALLOWED = {(0, 0, 1, 0, 1): 24, (3, 0, 1, 0, 1): 12}
 MMA_PER_CHUNK = 4                    # 32 fp32 of K per chunk / wgmma k8
+# (A kind, B kind, MASK) of every launch gemm_tc() dispatches (kinds: include/vlfb.h)
+DISPATCHED = [(2, 0, 0), (5, 0, 0), (3, 0, 0), (1, 4, 0), (1, 6, 0), (0, 0, 0), (0, 1, 0), (1, 0, 0), (1, 1, 0),
+              (3, 0, 1), (0, 0, 1)]
+
+
+def expected_builds():
+    """(A kind, B kind, MASK, CP, FIX) of every gemm_tc_kernel instantiation.  A pair with an MN-major operand is staged
+    (partly) by cp.async, so it has only CP = true builds: FIX = 0, and FIX = 1 for the MN x MN pairs without a mask
+    (the cp.async fix-up of deterministic launches).  A K-major pair has the cp.async build and both TMA-only builds."""
+    out = set()
+    for ak, bk, mask in DISPATCHED:
+        if ak in MN_KINDS or bk in MN_KINDS:
+            out.add((ak, bk, mask, 1, 0))
+            if ak in MN_KINDS and bk in MN_KINDS and not mask:
+                out.add((ak, bk, mask, 1, 1))
+        else:
+            out.update({(ak, bk, mask, 1, 0), (ak, bk, mask, 0, 0), (ak, bk, mask, 0, 1)})
+    return out
 
 NAME_RE = re.compile(r'_ZN4vlfb2tc14gemm_tc_kernelILi(\d+)ELi(\d+)ELb(\d)ELb(\d)ELb(\d)EEEv\w*')
 INSN_RE = re.compile(r'/\*([0-9a-f]{4,})\*/\s+([^;]*);')
@@ -139,6 +155,13 @@ def test_every_instantiation_is_reported(compiled):
     for key, body in compiled['funcs'].items():
         chunks, n = _chunks(body)
         assert n and n % MMA_PER_CHUNK == 0, '%s: %d HGMMA' % (_fmt(key), n)
+
+
+def test_instantiations_are_exactly_the_dispatched_builds(compiled):
+    want = expected_builds()
+    assert len(want) == 26
+    got = set(compiled['funcs'])
+    assert got == want, 'unexpected: %s; missing: %s' % (sorted(map(_fmt, got - want)), sorted(map(_fmt, want - got)))
 
 
 def test_no_serialized_wgmma(compiled):

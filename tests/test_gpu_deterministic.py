@@ -197,8 +197,8 @@ def kernel_checks():
 
 
 def forced_cp_checks():
-    """With the TMA paths switched off (VLFB_TMA_MN=0 VLFB_IM2COL=0) every wgrad runs in the cp.async build on 128 x BN
-    tiles when Co > 64: the fix-up of gemm_fixup_kernel on narrow tiles."""
+    """Every wgrad runs in the cp.async build (both operands are MN-major), on 128 x BN tiles when Co > 64: the fix-up
+    of gemm_fixup_kernel on narrow tiles."""
     from vlfb import kernels as K
     import wgrad_cases as WC
     seen = 0
@@ -226,7 +226,7 @@ def test_deterministic_kernels():
 
 
 def test_deterministic_wgrad_fixup_on_128_row_cp_async_tiles():
-    _worker(['--forced-cp'], {'VLFB_TMA_MN': '0', 'VLFB_IM2COL': '0'}, 'FORCED CP CHECKS OK')
+    _worker(['--forced-cp'], {}, 'FORCED CP CHECKS OK')
 
 
 # ------------------------------------------------------------------------------------------------ model level

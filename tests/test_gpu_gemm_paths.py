@@ -66,17 +66,7 @@ def test_gemm_paths_match_fp64_and_declared_path(cfg, tmp_dir):
     assert not bad, 'configuration %s:\n  ' % cfg + '\n  '.join(bad)
 
 
-# Every tensor map of an MN-major operand (make_tmap_mn / make_tmap_mn4, the wgrad im2col and conv_flat maps, the conv1
-# wgrad row and patch maps, make_tmap_dy4) is encoded with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  sm_90 does not support
-# the ATOM swizzle modes, so that encode fails and launch() stages every MN-major operand by cp.async: these combinations
-# of the kernel are not reachable on sm_90a.  (Stream-K atomic with TMA-fed operands is reached by a K-major matmul
-# instead of the wgrad.)
-UNREACHABLE_SM90 = {
-    'instantiation kinds=1,4 mask=0 cp=0', 'instantiation kinds=1,6 mask=0 cp=0', 'instantiation kinds=0,1 mask=0 cp=0',
-    'instantiation kinds=1,0 mask=0 cp=0', 'instantiation kinds=1,1 mask=0 cp=0',
-    'loader tma_a=4', 'loader tma_b=2', 'loader tma_b=3', 'loader tma_b=4', 'loader tma_b=5',
-    'conv1 wgrad patch chunks (tma_b=3)', 'conv1 wgrad TMA rows without patches',
-}
+MN_KINDS = (GP.OP_DENSE_MN, GP.OP_CONV_MN, GP.OP_STEM_MN)
 
 
 def _strided(case_name):
@@ -100,18 +90,17 @@ def test_gemm_path_coverage(tmp_dir):
         return any(pred(n, f, p) for n, f, p in seen)
 
     need = {}
-    pairs = [(2, 0), (5, 0), (3, 0), (1, 4), (1, 6), (0, 0), (0, 1), (1, 0), (1, 1)]
-    for ak, bk in pairs:
-        for cp in (0, 1):
-            need['instantiation kinds=%d,%d mask=0 cp=%d' % (ak, bk, cp)] = \
-                (lambda ak=ak, bk=bk, cp=cp: any_(lambda n, f, p: p['kinds'] == (ak, bk) and p['mask'] == 0 and p['cp'] == cp))
-    for ak, bk in [(3, 0), (0, 0)]:
-        for cp in (0, 1):
-            need['instantiation kinds=%d,%d mask=1 cp=%d' % (ak, bk, cp)] = \
-                (lambda ak=ak, bk=bk, cp=cp: any_(lambda n, f, p: p['kinds'] == (ak, bk) and p['mask'] == 1 and p['cp'] == cp))
-    for v in range(5):
+    # (A kind, B kind, mask): TMA-only (cp=0) builds exist for K-major pairs only
+    builds = [(2, 0, 0), (5, 0, 0), (3, 0, 0), (1, 4, 0), (1, 6, 0), (0, 0, 0), (0, 1, 0), (1, 0, 0), (1, 1, 0),
+              (3, 0, 1), (0, 0, 1)]
+    for ak, bk, mask in builds:
+        for cp in ((1,) if ak in MN_KINDS or bk in MN_KINDS else (0, 1)):
+            need['instantiation kinds=%d,%d mask=%d cp=%d' % (ak, bk, mask, cp)] = \
+                (lambda ak=ak, bk=bk, mask=mask, cp=cp:
+                 any_(lambda n, f, p: p['kinds'] == (ak, bk) and p['mask'] == mask and p['cp'] == cp))
+    for v in range(4):
         need['loader tma_a=%d' % v] = lambda v=v: any_(lambda n, f, p: p['tma_a'] == v)
-    for v in range(6):
+    for v in range(2):
         need['loader tma_b=%d' % v] = lambda v=v: any_(lambda n, f, p: p['tma_b'] == v)
     for bn in (32, 64, 96, 128):
         for cp in (0, 1):
@@ -127,8 +116,6 @@ def test_gemm_path_coverage(tmp_dir):
         'schedule stream-K atomic cp=1': lambda: any_(lambda n, f, p: p['sk'] == 1 and p['fix'] == 0 and f['atomic'] and p['cp'] == 1),
         'conv1 fwd patch tiles (tma_a=3)': lambda: any_(lambda n, f, p: p['kinds'] == (5, 0) and p['tma_a'] == 3 and p['patch'] == 1),
         'conv1 fwd TMA rows without patches': lambda: any_(lambda n, f, p: p['kinds'] == (5, 0) and p['tma_a'] == 3 and p['patch'] == 0),
-        'conv1 wgrad patch chunks (tma_b=3)': lambda: any_(lambda n, f, p: p['kinds'] == (1, 6) and p['tma_b'] == 3 and p['patch'] == 1),
-        'conv1 wgrad TMA rows without patches': lambda: any_(lambda n, f, p: p['kinds'] == (1, 6) and p['tma_b'] == 3 and p['patch'] == 0),
         'strided dgrad as parity classes': lambda: any_(lambda n, f, p: p['kinds'] == (3, 0) and p['par'] > 0),
         'strided dgrad by the gather loader': lambda: any_(lambda n, f, p: p['kinds'] == (3, 0) and p['par'] == 0 and p['tma_a'] == 0 and _strided(n)),
         'sign bits in-kernel': lambda: any_(lambda n, f, p: f['relu'] and p['bits2'] == 0 and 'bits' in GP.case_by_name(n).get('epi', {})),
@@ -143,8 +130,19 @@ def test_gemm_path_coverage(tmp_dir):
         'batch > 1': lambda: any_(lambda n, f, p: p['z'] > 1 and p['kinds'][1] in (0, 1) and p['kinds'][0] in (0, 1)),
         'taps > 1': lambda: any_(lambda n, f, p: p['z'] > 1 and p['kinds'][1] in (4, 6)),
     })
-    missing = [name for name, pred in need.items() if name not in UNREACHABLE_SM90 and not pred()]
+    missing = [name for name, pred in need.items() if not pred()]
     assert not missing, 'not covered by any passing case: ' + '; '.join(missing)
-    # ... and the paths the H100 cannot take stay untaken: once one is reached, move its cases' declarations to it
-    reached = [name for name in UNREACHABLE_SM90 if need[name]()]
-    assert not reached, 'declared unreachable on sm_90a but taken: ' + '; '.join(reached)
+
+
+def test_mn_major_operands_are_staged_by_cp_async(tmp_dir):
+    """Every launch record, in every configuration: an MN-major operand has no TMA loader and runs in a cp.async build."""
+    bad = []
+    for cfg in sorted(GP.CONFIGS):
+        _, recs = _run(cfg, tmp_dir)
+        for r in recs:
+            for p in r['paths']:
+                ak, bk = p['kinds']
+                if (ak in MN_KINDS and p['tma'][0] != 0) or (bk in MN_KINDS and p['tma'][1] != 0) or \
+                        ((ak in MN_KINDS or bk in MN_KINDS) and p['cp'] != 1):
+                    bad.append('%s / %s: kinds=%d,%d tma=%d,%d cp=%d' % (cfg, r['case'], ak, bk, p['tma'][0], p['tma'][1], p['cp']))
+    assert not bad, '\n'.join(bad)

@@ -5,11 +5,11 @@
 // Persistent kernel: grid = min(#tiles, #SMs), one CTA per SM walks a static sequence of 128 x BN output
 // tiles (BN <= 128; 64 x 2 BN "wide" tiles when both operands are MN-major and M <= 64, Launch::wide):
 //   PRODUCERS  -- the A/B K-chunks (32 fp32 = one 128-byte swizzle row) go straight from NDHWC tensors into
-//              swizzled shared-memory tiles, never through an im2col buffer: dense operands by TMA tiled
-//              boxes (SWIZZLE_128B K-major, SWIZZLE_128B_ATOM_32B MN-major), convolution gathers by TMA
-//              im2col copies (conv fwd, unit-stride dgrad, wgrad; one thread issues), and what TMA cannot
-//              express (conv1 stem with 16-byte pixels, strided dgrad, unaligned operands) by 16-byte
-//              cp.async with zero-fill = padding (8 warps; a TMA-only build has one issuing warp of four);
+//              swizzled shared-memory tiles, never through an im2col buffer: dense K-major operands by TMA
+//              tiled boxes (SWIZZLE_128B), convolution gathers by TMA im2col copies (conv fwd, unit-stride
+//              dgrad), the conv1 stem by overlapping-window TMA boxes (one thread issues), and MN-major operands
+//              and what TMA cannot express (strided dgrad outside the parity classes, unaligned operands) by
+//              16-byte cp.async with zero-fill = padding (8 warps; a TMA-only build has one producer warpgroup);
 //   CONSUMERS  -- two warpgroups; warpgroup w issues wgmma.m64nBNk8 for tile rows [64 w, 64 w + 64) (wide tiles:
 //              columns [w BN, w BN + BN) of the 64 rows) and then
 //              runs the epilogue of those rows from its registers: smem transpose -> fused affine /
@@ -40,15 +40,7 @@ constexpr int BN_MAX = 128;    // widest tile: a warpgroup holds 64 x BN fp32 ac
 constexpr int KC = 32;         // fp32 per K chunk (128 B)
 constexpr int NPROD = 256;     // 8 cp.async producer warps = 2 per scheduler, so the address-generation latency of
                                // one warp hides behind the other
-// TMA-only builds: warps whose lane 0 issues the TMA boxes of a K chunk (box b by warp b % NTMAW).  A build parameter,
-// default one issuer: concurrent issuers only interleave the boxes of different stages; fewer, larger boxes (one 4-D
-// box per MN-major operand tile, below) are the way to cut the per-box cost of the TMA unit.
-#ifndef VLFB_TMA_WARPS
-#define VLFB_TMA_WARPS 1
-#endif
-constexpr int NTMAW = VLFB_TMA_WARPS;
 constexpr int RSTEP = NPROD / 8;   // rows covered by one pass of the K-major loaders
-static_assert(NTMAW >= 1 && NTMAW <= 4, "TMA issuers live in the producer warpgroup");
 constexpr int NEPI = 256;          // 2 consumer warpgroups (MMA + epilogue); warp w of a warpgroup owns 16 tile rows
 constexpr int NPROD_TMA = 128;     // producer threads of a TMA-only build: one warpgroup, so the consumers are warpgroup-aligned
 constexpr int EPC = 16;            // accumulator columns per epilogue step
@@ -117,12 +109,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, int c4,
@@ -223,10 +209,9 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 }
 
 // Consumer-side rewrite of an MN-major stage tile into the K-major SWIZZLE_128B image [row][128 B] that wgmma reads
-// (tf32 operands in shared memory must be K-major).  Source: `rows` x 32 k as [atom of 32 elements][k-row][128 B],
-// 16-byte chunk c of k-row k at byte (16 c) ^ (32 (k & 3)) (SWIZZLE_128B_ATOM_32B / MNLoader), atoms `atom_stride`
-// bytes apart; k-rows 128 B apart, or, for the conv1 wgrad patch tile (row_gap = sH), k-rows 16-31 (the patch's second
-// output row) row_gap 2 KB slabs further.  Image: element (n, k) at n * 128 + 16 ((k / 4) ^ (n % 8)) + 4 (k % 4).
+// (tf32 operands in shared memory must be K-major).  Source: `rows` x 32 k as [atom of 32 elements][k-row][128 B]
+// (MNLoader), 16-byte chunk c of k-row k at byte (16 c) ^ (32 (k & 3)), k-rows 128 B and atoms 4 KB apart.
+// Image: element (n, k) at n * 128 + 16 ((k / 4) ^ (n % 8)) + 4 (k % 4).
 // Unit u = t + NEPI j moves a 4 n x 4 k block: k-quad kq = u % 8, source chunk c = kq ^ ((u / 8) % 8) of atom u / 64.
 // It reads chunk c of k-rows 4 kq .. 4 kq + 3 (four v4 loads), transposes in registers and writes rows n = 32 atom +
 // 4 c + q, q = 0..3, at k-quad kq (four v4 stores).  A 16-byte access is served in four phases of 8 lanes, and a phase
@@ -235,17 +220,16 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 //   loads:  slot = c ^ 2 (k & 3) = kq ^ b ^ 2 r for load r  -> 8 distinct slots;
 //   stores: slot = kq ^ (n % 8) = kq ^ 4 ((kq ^ b) & 1) ^ q  -> kq ^ const on even kq, kq ^ (const ^ 4) on odd kq, a
 //           bijection of 0..7 (bit 0 is kept) -> 8 distinct slots.
-__device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int rows, int atom_stride, int row_gap, int ctid) {
+__device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int rows, int ctid) {
   for (int u = ctid; u < rows * 2; u += NEPI) {
     const int kq = u & 7, c = kq ^ ((u >> 3) & 7), atom = u >> 6;
     float v[4][4];
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
       const int k = 4 * kq + r;
-      const uint32_t koff = row_gap ? (uint32_t)((k >> 4) * row_gap * 2048 + (k & 15) * 128) : (uint32_t)(k * 128);
       asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
                    : "=f"(v[r][0]), "=f"(v[r][1]), "=f"(v[r][2]), "=f"(v[r][3])
-                   : "r"(src + (uint32_t)(atom * atom_stride) + koff + (uint32_t)((c * 16) ^ (r << 5)))
+                   : "r"(src + (uint32_t)(atom * 4096 + k * 128) + (uint32_t)((c * 16) ^ (r << 5)))
                    : "memory");
     }
 #pragma unroll
@@ -439,8 +423,7 @@ struct KLoader {
 
 // ---------------------------------------------------------------- MN-major loaders
 // Tile = 32 k-rows, each `rows`*4 bytes of the m (or n) extent, stored as
-// [atom of 32 elements][32 k-rows][128 B] (MN-major SWIZZLE_128B_ATOM_32B; the
-// consumers rewrite it K-major before the MMAs, mn_to_kmajor).
+// [atom of 32 elements][32 k-rows][128 B] (the consumers rewrite it K-major before the MMAs, mn_to_kmajor).
 template <int KIND>
 struct MNLoader {
   static constexpr int SGRP = (32 * (BN_MAX / 4)) / NPROD;   // copies per thread per chunk at a 128-row tile (the
@@ -473,8 +456,7 @@ struct MNLoader {
     const int c = threadIdx.x & (cpr - 1);
     mn = row0 + c * 4;
     colok = mn < limit;
-    // atom-major tile [atom of 32 elements][32 k-rows][128 B] in the SWIZZLE_128B_BASE32B pattern (32-byte
-    // units XOR (k & 3)).  Same image as a TMA box with SWIZZLE_128B_ATOM_32B.
+    // atom-major tile [atom of 32 elements][32 k-rows][128 B], 32-byte units of a k-row XOR (k & 3).
     // kstep is a multiple of 4 whenever a thread owns more than one copy, so the XOR term is per-thread.
     const int r = kk0 & 3, cc8 = c & 7;
     dst0 = (uint32_t)((c >> 3) * 4096 + kk0 * 128 + ((((cc8 >> 1) ^ r) << 5) | ((cc8 & 1) << 4)));
@@ -581,19 +563,15 @@ struct Launch {
   PosDiv in;     // ... and of the INPUT extents (W, H, T) for the dgrad row decode
   FastDiv cdiv;  // input channels C (wgrad: n -> (tap, ci))
   FastDiv kwdiv; // kW
-  int tma_a, tma_b;  // operand fetched by TMA instead of cp.async: 1 = dense tiled boxes, 2 = im2col (conv gathers),
-                     // 3 = conv1 stem rows: {8 px x 4 ch = 128 B, 16 output positions} boxes of the overlapping-window
-                     //     view of a W-padded clip (make_tmap_stem)
+  int tma_a, tma_b;  // loader of each operand (K-major only; MN-major operands are always 0): 0 = cp.async, 1 = dense
+                     // tiled boxes, 2 = im2col (conv gathers, A only), 3 = conv1 stem rows (A only): {8 px x 4 ch =
+                     // 128 B, 16 output positions} boxes of the overlapping-window view of a W-padded clip (make_tmap_stem)
   int lag;           // cp.async groups kept in flight before a stage is published (< stages)
   int tiles_m, tiles_n, total_tiles;
   int stem_patch;    // conv1 forward: an M tile = a 16 (wo) x 8 (ho) patch of one output frame instead of 128 consecutive
                      // positions, so that ONE strided TMA box stages the whole A tile of a K chunk (tile row r =
                      // (ho0 + r / 16, wo0 + r % 16)); the fast epilogue maps rows back (patch_row)
-  int patch_wb, patch_hb;   // patches per output row / per frame column: Wo / 16, Ho / 8 (forward), Ho / 2 (wgrad)
-                            // conv1 WGRAD (B = STEM_MN) with stem_patch: K chunk = the 32 output positions of a
-                            // 16 (wo) x 2 (ho) patch; ONE box stages the sH + kH input rows all kH filter-row atoms need
-                            // ([input row][16 windows][128 B] slabs; atom kh of output row j = slab j*sH + kh, so the
-                            // atom stride is one slab) and one 4-D box per 32 channels stages dY^T
+  int patch_wb, patch_hb;   // patches per output row / per frame column: Wo / 16, Ho / 8
   // Strided conv dgrad (A = DGRAD_K, sH / sW = 2) as sH * sW PARITY CLASSES: the input positions (h, w) = (sH h' + ph,
   // sW w' + pw) of one class receive only the filter taps kh = rh + sH j, kw = rw + sW i (rh = (ph + pH) % sH ...), i.e.
   // each class is a unit-stride convolution over dY with nh x nw taps (3x3 stride 2: 1 + 2 + 2 + 4 = 9 taps for the four
@@ -710,9 +688,9 @@ __device__ __forceinline__ bool sched_next(const vlfb_gemm_params_t& p, const La
 // Persistent, warp-specialised: grid = min(#tiles, #SMs) CTAs; every role walks the same work sequence (Sched).  The
 // smem ring (full/empty) runs continuously across tiles, so the producers stage the next tile while the consumers
 // run the epilogue of the current one.
-// CP = false: both operands are staged by TMA, so one producer warpgroup (one issuing warp) suffices and the CTA is
-// 12 warps with up to 168 registers per thread; the 16-warp CP = true build (8 cp.async gather warps: conv1 stem,
-// strided dgrad, operands TMA cannot address) is capped at 128.
+// CP = false: both operands are K-major and staged by TMA, so one producer warpgroup (one issuing thread) suffices and
+// the CTA is 12 warps with up to 168 registers per thread; the 16-warp CP = true build (8 cp.async gather warps:
+// MN-major operands, conv1 stem on a dense clip, strided dgrad, operands TMA cannot address) is capped at 128.
 // FIX: the stream-K fix-up (a piece of a shared tile through the workspace) is compiled in; only the launches that plan
 // fix-ups use these instantiations.  Its last-arriver decision is per warp, so the K loop must leave no MMA in flight
 // when it ends on any path (ptxas would otherwise serialise every wgmma of the kernel, tests/test_gemm_pipeline_cpu.py).
@@ -720,10 +698,10 @@ template <int AK, int BK, bool MASK, bool CP, bool FIX>
 __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_kernel(const vlfb_gemm_params_t p, const Launch L,
                                                               const __grid_constant__ CUtensorMap tmA,
                                                               const __grid_constant__ CUtensorMap tmB) {
+  static_assert(CP || (!is_mn(AK) && !is_mn(BK)), "MN-major operands are staged by cp.async only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int bn = L.bn, S = L.stages;
-  const int bnh = bn;
   // K-major images of the MN-major operands (wgmma reads tf32 operands K-major only): one for A, two for B (chunk i
   // uses B image i % 2)
   constexpr bool TA = is_mn(AK), TB = is_mn(BK);
@@ -747,7 +725,7 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform role: producer / consumer branches are not divergent
   const int unit = (int)blockIdx.x;
   const int nunits = (int)gridDim.x;
-  const bool tma_a = L.tma_a != 0, tma_b = L.tma_b != 0;
+  const bool tma_a = !is_mn(AK) && L.tma_a != 0, tma_b = !is_mn(BK) && L.tma_b != 0;
   const bool cp_any = CP && !(tma_a && tma_b);
 
 #ifdef VLFB_TRACE
@@ -769,13 +747,10 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
   if (tid == 0) TR(2);
 
   if (warp < NPWT) {
-    // ============================ PRODUCERS (8 cp.async warps / NTMAW TMA issuers) ============================
-    // TMA issuers: thread 0 in a CP build; lane 0 of every producer warp in a TMA-only build.  All issuers walk the same
-    // tile / chunk sequence with their own copy of the (deterministic) gather state and wait for the free stage
-    // themselves; issuer `hid` launches the boxes b with b % NISS == hid; issuer 0 posts the expected byte count.
-    constexpr int NISS = CP ? 1 : NTMAW;
-    const int hid = CP ? 0 : (tid >> 5);
-    const bool issuer = CP ? (tid == 0) : ((tid & 31) == 0 && hid < NTMAW);
+    // ============================ PRODUCERS (8 cp.async warps / one TMA issuer) ============================
+    // The TMA issuer is thread 0: it posts the expected byte count and issues the boxes of every chunk, after waiting for
+    // the free stage like every cp.async thread.
+    const bool issuer = tid == 0;
     if (cp_any || issuer) {
       KLoader<is_mn(AK) ? VLFB_OP_DENSE_K : AK, BM / RSTEP> ka;
       MNLoader<is_mn(AK) ? AK : VLFB_OP_DENSE_MN> ma;
@@ -791,23 +766,17 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
       constexpr bool ASYNC_PUB = CP && is_mn(AK) && is_mn(BK);
       // compile-time gates keep the im2col state out of the instantiations that cannot use it (registers)
       const bool im2col_a = (AK == VLFB_OP_CONV_K || AK == VLFB_OP_DGRAD_K) && L.tma_a == 2;
-      const bool im2col_b = BK == VLFB_OP_CONV_MN && L.tma_b == 2;
-      constexpr int NATOM = BK == VLFB_OP_CONV_MN ? 8 : 1;
-      // im2col state of the issuing thread: window origin of the tile's first row + filter-tap cursor (A), and
-      // per 32-column atom the channel slice / tap offsets of the wgrad B tile
+      // im2col state of the issuing thread: window origin of the tile's first row + filter-tap cursor
       int ia_w = 0, ia_h = 0, ia_d = 0, ia_n = 0, ic_t = 0, ic_h = 0, ic_w = 0, ic_c = 0, icpt = 1;
-      int ib_c[NATOM], ib_off[NATOM], ib_atoms = 0;
       // conv1 stem rows (tma 3): the 128 tile rows = 8 groups of 16 consecutive output positions (16 | Wo, so a group
       // never crosses an output row): per group the window origin (wo, hi0 = ho sH - pH, ti0 = to sT - pT, n)
       const bool stem_a = AK == VLFB_OP_STEM_K && L.tma_a == 3;
-      const bool stem_b = BK == VLFB_OP_STEM_MN && L.tma_b == 3;
       constexpr int NSG = AK == VLFB_OP_STEM_K ? 8 : 1;
       int sg_w[NSG], sg_ht[NSG], sg_n[NSG];
       // chunk counter over the CTA's whole work sequence; ring slot / phase / lagged slot advance
       // incrementally (S is a run-time value: `it % S` cost three integer divisions per chunk per thread)
       int it = 0, s = 0, sl = 0;
       uint32_t ph = 0;
-      const uint32_t fullx = full0;
       Sched sc;
       sched_init(sc, L, unit);
       TileInfo ti;
@@ -824,7 +793,7 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
         }
         const int kc0 = ti.k_begin / KC;
         // bytes the stage barrier expects
-        uint32_t tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + (tma_b ? b_tile_bytes : 0u);
+        const uint32_t tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + (tma_b ? b_tile_bytes : 0u);
         if (issuer && stem_a && L.stem_patch) {
           const vlfb_conv_geom_t& g = p.g;
           const int mt = ti.m0 / BM;
@@ -871,153 +840,52 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           ic_c = kc0 - tap * icpt;
           decode_tap(tap, g.kH, g.kW, ic_t, ic_h, ic_w);     // (par: kc0 = 0 -> all zero; ic_h / ic_w count the class's taps)
         }
-        if (issuer && im2col_b) {
-          const vlfb_conv_geom_t& g = p.g;
-          ib_atoms = 0;
-#pragma unroll
-          for (int a = 0; a < NATOM; ++a) {
-            const int ncol = nb0 + a * 32;
-            if (a * 32 < bnh && ncol < p.N) {
-              uint32_t tap_hw, ci, qh, qw;
-              fd_divmod((uint32_t)ncol, L.cdiv, tap_hw, ci);       // n = (kh*kW + kw) * C + ci
-              fd_divmod(tap_hw, L.kwdiv, qh, qw);
-              ib_c[a] = (int)ci;
-              ib_off[a] = ((int)qh * g.dH << 16) | ((int)qw * g.dW);
-              ib_atoms = a + 1;
-            }
-          }
-          tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + 4096u * (uint32_t)ib_atoms;
-        }
-        if (issuer && stem_b) {
-          ib_atoms = 0;                                             // atoms = filter rows kh of this N tile
-          for (int a = 0; a * 32 < bn && ti.n0 + a * 32 < p.N; ++a) ib_atoms = a + 1;
-          tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + 4096u * (uint32_t)ib_atoms;
-          if (L.stem_patch) {
-            int a_atoms = 0;
-            for (int a = 0; a * 32 < p.M && a < BM / 32; ++a) a_atoms = a + 1;
-            tma_bytes = 4096u * (uint32_t)a_atoms + 2048u * (uint32_t)(p.g.sH + p.g.kH);
-          }
-        }
         for (int i = 0; i < ti.nk; ++i, ++it) {
-          // Helper issuers (hid > 0) wait for the free stage LAZILY, right before their first box of the chunk: an issuer
-          // without a box in a chunk (2-box chunks on 3 issuers) must not wait at all -- nothing would depend on it, the
-          // others would lap it by two phases of the stage barrier and its parity wait would then never return.
-          const bool need_wait = it >= S;
-          const uint32_t wpar = ph ^ 1u;
           const int s_cur = s;
-          if (need_wait && (NISS == 1 || hid == 0 || cp_any)) mbar_wait(empty0 + 8 * s_cur, wpar);
+          if (it >= S) mbar_wait(empty0 + 8 * s_cur, ph ^ 1u);
           if (++s == S) { s = 0; ph ^= 1u; }
           const uint32_t a_tile = smem_base + s_cur * stage_bytes;
           const uint32_t b_tile = a_tile + a_tile_bytes;
-          const uint32_t fbar = fullx + 8 * s_cur;
+          const uint32_t fbar = full0 + 8 * s_cur;
           if (issuer && tma_bytes) {
-            if (hid == 0) mbar_expect_tx(full0 + 8 * s_cur, tma_bytes);
-            int box = 0;                                  // boxes of this chunk, in issue order
-            bool waited = NISS == 1 || hid == 0;
-            auto mine = [&]() {
-              const bool m = NISS == 1 || (box % NISS) == hid;
-              ++box;
-              if (m && !waited) {
-                if (need_wait) mbar_wait(empty0 + 8 * s_cur, wpar);
-                waited = true;
-              }
-              return m;
-            };
+            mbar_expect_tx(fbar, tma_bytes);
             if (stem_a) {
               const vlfb_conv_geom_t& g = p.g;
               if (L.stem_patch) {                     // one {128 B x 16 wo x 8 rows (stride sH)} box = the whole A tile
-                if (mine()) tma_load_5d(a_tile, &tmA, 0, sg_w[0], (sg_ht[0] >> 16) + ic_h, (int)(short)(sg_ht[0] & 0xFFFF) + ic_t, sg_n[0], fbar);
+                tma_load_5d(a_tile, &tmA, 0, sg_w[0], (sg_ht[0] >> 16) + ic_h, (int)(short)(sg_ht[0] & 0xFFFF) + ic_t, sg_n[0], fbar);
               } else {
 #pragma unroll
                 for (int q = 0; q < NSG; ++q)
-                  if (mine()) tma_load_5d(a_tile + q * 2048, &tmA, 0, sg_w[q], (sg_ht[q] >> 16) + ic_h, (int)(short)(sg_ht[q] & 0xFFFF) + ic_t,
+                  tma_load_5d(a_tile + q * 2048, &tmA, 0, sg_w[q], (sg_ht[q] >> 16) + ic_h, (int)(short)(sg_ht[q] & 0xFFFF) + ic_t,
                               sg_n[q], fbar);
               }
               if (++ic_h == g.kH) { ic_h = 0; ++ic_t; }
             } else if (im2col_a) {
               const vlfb_conv_geom_t& g = p.g;
               if (AK == VLFB_OP_CONV_K) {
-                if (mine()) tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, ic_w * g.dW, ic_h * g.dH, ic_t * g.dT, fbar);
+                tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, ic_w * g.dW, ic_h * g.dH, ic_t * g.dT, fbar);
               } else if (AK == VLFB_OP_DGRAD_K && L.par) {
                 // tap (kt, rh + sH ic_h, rw + sW ic_w) of the class: dY offset (taps - 1 - index), weights at the original tap
                 const ParCls& c = L.par_cls[ti.batch];
-                if (mine()) tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, c.nw - 1 - ic_w, c.nh - 1 - ic_h, (g.kT - 1 - ic_t) * g.dT, fbar);
+                tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, c.nw - 1 - ic_w, c.nh - 1 - ic_h, (g.kT - 1 - ic_t) * g.dT, fbar);
                 const int tap = (ic_t * g.kH + c.rh + g.sH * ic_h) * g.kW + c.rw + g.sW * ic_w;
-                if (mine()) tma_load_3d(b_tile, &tmB, tap * g.Co + ic_c * KC, nb0, 0, fbar);
+                tma_load_3d(b_tile, &tmB, tap * g.Co + ic_c * KC, nb0, 0, fbar);
                 if (++ic_c == icpt) {
                   ic_c = 0;
                   if (++ic_w == c.nw) { ic_w = 0; if (++ic_h == c.nh) { ic_h = 0; ++ic_t; } }
                 }
               } else {
-                if (mine()) tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, (g.kW - 1 - ic_w) * g.dW,
+                tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, (g.kW - 1 - ic_w) * g.dW,
                     (g.kH - 1 - ic_h) * g.dH, (g.kT - 1 - ic_t) * g.dT, fbar);
               }
               if (!(AK == VLFB_OP_DGRAD_K && L.par) && ++ic_c == icpt) {
                 ic_c = 0;
                 if (++ic_w == g.kW) { ic_w = 0; if (++ic_h == g.kH) { ic_h = 0; ++ic_t; } }
               }
-            } else if (tma_a && !(stem_b && L.stem_patch)) {
-              if (is_mn(AK) && L.tma_a == 4) {            // all atoms of the tile in one box
-                if (mine()) tma_load_4d(a_tile, &tmA, 0, ti.k_begin + i * KC, ti.m0 >> 5, ti.batch, fbar);
-              } else if (is_mn(AK)) {
-                for (int a = 0; a < BM / 32; ++a)
-                  if (mine()) tma_load_3d(a_tile + a * 4096, &tmA, ti.m0 + a * 32, ti.k_begin + i * KC, ti.batch, fbar);
-              } else {
-                if (mine()) tma_load_3d(a_tile, &tmA, (kc0 + i) * KC, ti.m0, ti.batch, fbar);
-              }
+            } else if (tma_a) {
+              tma_load_3d(a_tile, &tmA, (kc0 + i) * KC, ti.m0, ti.batch, fbar);
             }
-            if (stem_b && L.stem_patch) {
-              const vlfb_conv_geom_t& g = p.g;
-              const int q = ti.k_begin / KC + i;                     // chunk -> patch (wb, row pair, frame)
-              const int wb = q % L.patch_wb, q2 = q / L.patch_wb;
-              const int hp = q2 % L.patch_hb, rest = q2 / L.patch_hb;
-              const int to = rest % g.To, n = rest / g.To;
-              if (mine()) tma_load_5d(b_tile, &tmB, 0, wb * 16, hp * 2 * g.sH - g.pH, to * g.sT - g.pT + ti.tap, n, fbar);
-              for (int a = 0; a * 32 < p.M && a < BM / 32; ++a)      // dY^T: {32 channels, 16 wo, 2 ho} per atom
-                if (mine()) tma_load_4d(a_tile + a * 4096, &tmA, ti.m0 + a * 32, wb * 16, hp * 2, rest, fbar);
-            } else if (stem_b) {
-              // conv1 wgrad B tile: 32 output positions (k rows) = 2 groups of 16; per filter row kh one 32-column atom
-              // (8 px x 4 ch) = two {128 B x 16 positions} boxes of the overlapping-window view
-              const vlfb_conv_geom_t& g = p.g;
-              const int kh0 = ti.n0 >> 5;
-#pragma unroll
-              for (int hf = 0; hf < 2; ++hf) {
-                const int kpos = ti.k_begin + i * KC + 16 * hf;
-                const Pos4 o = decode_pos_fast((uint32_t)(kpos < p.K ? kpos : 0), L.out);
-                const int bn_ = kpos < p.K ? o.n : g.N;
-                const int bh = o.h * g.sH - g.pH + kh0, bt = o.t * g.sT - g.pT + ti.tap;
-                for (int a = 0; a < ib_atoms; ++a)
-                  if (mine()) tma_load_5d(b_tile + a * 4096 + hf * 2048, &tmB, 0, o.w, bh + a, bt, bn_, fbar);
-              }
-            } else if (BK == VLFB_OP_CONV_MN && L.tma_b == 5) {
-              // wgrad B tile of a convolution without spatial taps: 32 consecutive positions of one clip, shifted by whole
-              // frames for the temporal tap, all channel atoms of the tile in ONE box (make_tmap_conv_flat)
-              const vlfb_conv_geom_t& g = p.g;
-              const uint32_t hw = (uint32_t)(g.H * g.W), thw = (uint32_t)g.T * hw;
-              const uint32_t kpos = (uint32_t)(ti.k_begin + i * KC);
-              const uint32_t n = kpos / thw;
-              const int pos = (int)(kpos - n * thw) + (ti.tap * g.dT - g.pT) * (int)hw;
-              if (mine()) tma_load_4d(b_tile, &tmB, 0, pos, nb0 >> 5, (int)n, fbar);
-            } else if (im2col_b) {
-              // wgrad B tile: 32 output positions (k rows) x one (kh, kw, 32-channel) atom per copy
-              const vlfb_conv_geom_t& g = p.g;
-              const Pos4 o = decode_pos_fast((uint32_t)(ti.k_begin + i * KC), L.out);
-              const int bw = o.w * g.sW - g.pW, bh = o.h * g.sH - g.pH, bd = o.t * g.sT - g.pT;
-#pragma unroll
-              for (int a = 0; a < NATOM; ++a)
-                if (a < ib_atoms)
-                  if (mine()) tma_load_im2col(b_tile + a * 4096, &tmB, ib_c[a], bw, bh, bd, o.n, ib_off[a] & 0xFFFF, ib_off[a] >> 16,
-                      ti.tap * g.dT, fbar);
-            } else if (tma_b && !(AK == VLFB_OP_DGRAD_K && L.par)) {
-              if (is_mn(BK) && L.tma_b == 4) {
-                if (mine()) tma_load_4d(b_tile, &tmB, 0, ti.k_begin + i * KC, nb0 >> 5, ti.batch, fbar);
-              } else if (is_mn(BK)) {
-                for (int a = 0; a < bnh / 32; ++a)
-                  if (mine()) tma_load_3d(b_tile + a * 4096, &tmB, nb0 + a * 32, ti.k_begin + i * KC, ti.batch, fbar);
-              } else {
-                if (mine()) tma_load_3d(b_tile, &tmB, (kc0 + i) * KC, nb0, ti.batch, fbar);
-              }
-            }
+            if (tma_b && !(AK == VLFB_OP_DGRAD_K && L.par)) tma_load_3d(b_tile, &tmB, (kc0 + i) * KC, nb0, ti.batch, fbar);
           }
           if (!cp_any) continue;
           if (!tma_a) {
@@ -1068,8 +936,6 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
     const int wrow = 16 * (wide ? (ew & 3) : ew);   // its first tile row
     const int wcol = wide ? wg * bn : 0;            // ... and first tile column (a wide tile's halves: one per warpgroup)
     const int lane = tid & 31;
-    // (patch chunks stage both operands by TMA: never in a cp.async build)
-    const bool stem_pb = !CP && BK == VLFB_OP_STEM_MN && L.tma_b == 3 && L.stem_patch != 0;
     float* stg = reinterpret_cast<float*>(smem_raw + (epi_base - smem_u32(smem_raw))) + ew * EPI_WARP_FLOATS;
     float* wsc = stg + 16 * EPITCH;      // column scale of the tile's columns, then the bias
     float* wbi = wsc + BN_MAX;
@@ -1102,8 +968,8 @@ __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_ke
           if (TA || TB) {
             if (TA) wgmma_wait<0>();             // no MMA still reads the A image
             consumers_sync();                    // both warpgroups are done with chunk i - 2 (TA: i - 1)
-            if (TA) mn_to_kmajor(a_tile, ka_img, a_rows, 4096, 0, ctid);
-            if (TB) mn_to_kmajor(b_tile, b_img, b_rows, stem_pb ? 2048 : 4096, stem_pb ? p.g.sH : 0, ctid);
+            if (TA) mn_to_kmajor(a_tile, ka_img, a_rows, ctid);
+            if (TB) mn_to_kmajor(b_tile, b_img, b_rows, ctid);
             fence_proxy_async();                 // generic-proxy writes -> visible to the wgmma (async proxy) reads
             consumers_sync();                    // images complete
           }
@@ -1598,56 +1464,6 @@ static bool make_tmap(CUtensorMap* tm, const vlfb_operand_t& op, int rows, int K
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// Dense MN-major fp32 matrix [K rows][extent] (+batch): box = {32 elements, 32 k-rows, 1} written in the
-// SWIZZLE_128B_ATOM_32B pattern = one MN-major atom column (4 KB) per copy.
-static bool make_tmap_mn(CUtensorMap* tm, const vlfb_operand_t& op, int extent, int K, int batch) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc || op.kind != VLFB_OP_DENSE_MN || K < KC || extent < 32) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)extent, (cuuint64_t)K, (cuuint64_t)(batch > 1 ? batch : 1)};
-  cuuint64_t strides[2] = {(cuuint64_t)op.ld * 4, (cuuint64_t)(batch > 1 ? op.batch_stride : (int64_t)K * op.ld) * 4};
-  if ((strides[0] & 15) || (strides[1] & 15) || strides[1] == 0) return false;
-  cuuint32_t box[3] = {32, (cuuint32_t)KC, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(op.ptr), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// The same operand as ONE box per tile: a 4-D view {32 elements of an atom, K rows, atom index, batch} -- the atom
-// dimension has the SMALLEST stride (128 B), which a tiled map may have -- with box {32, 32 k-rows, natoms, 1}: the copy
-// writes atom after atom, i.e. exactly the [atom][k][32] layout the per-atom copies produce, in one instruction instead
-// of one per atom.  The TMA unit's cost is per BOX, so fewer boxes per K chunk.  Needs whole atoms (extent % 32 == 0).
-static bool make_tmap_mn4(CUtensorMap* tm, const vlfb_operand_t& op, int extent, int K, int batch, int natoms) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc || op.kind != VLFB_OP_DENSE_MN || K < KC || extent < 32 || (extent & 31) || natoms < 1 || natoms > 8) return false;
-  cuuint64_t dims[4] = {32, (cuuint64_t)K, (cuuint64_t)(extent / 32), (cuuint64_t)(batch > 1 ? batch : 1)};
-  cuuint64_t strides[3] = {(cuuint64_t)op.ld * 4, 128, (cuuint64_t)(batch > 1 ? op.batch_stride : (int64_t)K * op.ld) * 4};
-  if ((strides[0] & 15) || (strides[2] & 15) || strides[2] == 0) return false;
-  cuuint32_t box[4] = {32, (cuuint32_t)KC, (cuuint32_t)natoms, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(op.ptr), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-// wgrad activation operand of a convolution WITHOUT spatial taps (1x1x1 and kTx1x1, unit strides, no spatial padding --
-// two thirds of the convolutions of the nets): the k rows of a chunk are 32 consecutive positions of one clip, shifted by
-// whole frames for the temporal tap, so the gather is a dense 4-D view {32 channels of an atom, T*H*W positions of a
-// clip, atom index, clip}; frames outside the clip are out of range in the position dimension and read as zeros.
-// ONE box per K chunk instead of up to 8 im2col copies.  Needs T*H*W % 32 == 0 (a chunk never straddles two clips).
-static bool make_tmap_conv_flat(CUtensorMap* tm, const float* x, const vlfb_conv_geom_t& g, int natoms) {
-  EncodeTiledFn enc = encode_fn();
-  const int64_t thw = (int64_t)g.T * g.H * g.W;
-  if (!enc || g.kH != 1 || g.kW != 1 || g.sT != 1 || g.sH != 1 || g.sW != 1 || g.pH != 0 || g.pW != 0) return false;
-  if ((g.C & 31) || (thw & 31) || g.To != g.T || g.Ho != g.H || g.Wo != g.W || natoms < 1 || natoms > 8) return false;
-  cuuint64_t dims[4] = {32, (cuuint64_t)thw, (cuuint64_t)(g.C / 32), (cuuint64_t)g.N};
-  cuuint64_t strides[3] = {(cuuint64_t)g.C * 4, 128, (cuuint64_t)thw * g.C * 4};
-  cuuint32_t box[4] = {32, (cuuint32_t)KC, (cuuint32_t)natoms, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 // 5-D im2col map of an NDHWC fp32 tensor [N, D, H, W, C]: `pixels` window origins x 32 channels per copy.
 // lower/upper = bounding-box corners {W, H, D}; strides = traversal strides {W, H, D}.
 typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1655,8 +1471,7 @@ typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
                                    CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                    CUtensorMapFloatOOBfill);
 static bool make_tmap_im2col(CUtensorMap* tm, const float* base, int N, int D, int H, int W, int C, const int lower[3],
-                             const int upper[3], const int strides[3], int pixels, CUtensorMapSwizzle swz,
-                             int chan = KC) {
+                             const int upper[3], const int strides[3], int pixels) {
   static EncodeIm2colFn enc = nullptr;
   static bool tried = false;
   if (!tried) {
@@ -1667,15 +1482,15 @@ static bool make_tmap_im2col(CUtensorMap* tm, const float* base, int N, int D, i
         q == cudaDriverEntryPointSuccess)
       enc = reinterpret_cast<EncodeIm2colFn>(ptr);
   }
-  if (!enc || (C % chan) != 0 || (reinterpret_cast<uintptr_t>(base) & 15)) return false;
+  if (!enc || (C % KC) != 0 || (reinterpret_cast<uintptr_t>(base) & 15)) return false;
   for (int i = 0; i < 3; ++i)
     if (lower[i] < -16 || lower[i] > 15 || upper[i] < -16 || upper[i] > 15 || strides[i] < 1 || strides[i] > 8) return false;
   cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)N};
   cuuint64_t gstr[4] = {(cuuint64_t)C * 4, (cuuint64_t)C * 4 * W, (cuuint64_t)C * 4 * W * H, (cuuint64_t)C * 4 * W * H * D};
   cuuint32_t estr[5] = {1, (cuuint32_t)strides[0], (cuuint32_t)strides[1], (cuuint32_t)strides[2], 1};
   return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(base), dims, gstr, lower, upper,
-             (cuuint32_t)chan, (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+             (cuuint32_t)KC, (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // conv1 stem (C padded to 4, 16-byte pixels): overlapping-window view of a clip whose rows are stored with `pitch`
@@ -1683,8 +1498,7 @@ static bool make_tmap_im2col(CUtensorMap* tm, const float* base, int N, int D, i
 // at padded pixel wo * sW (i.e. real pixel wo * sW - pW), dim1 = wo (stride sW pixels: consecutive windows OVERLAP),
 // dim2 / dim3 = input row / frame (their out-of-range coordinates read as zeros = the H / T padding), dim4 = clip.
 // One box = 16 consecutive output positions of one output row.
-static bool make_tmap_stem(CUtensorMap* tm, const float* ptr, const vlfb_conv_geom_t& g, int64_t pitch, CUtensorMapSwizzle swz,
-                           int box_rows = 1) {
+static bool make_tmap_stem(CUtensorMap* tm, const float* ptr, const vlfb_conv_geom_t& g, int64_t pitch, int box_rows = 1) {
   EncodeTiledFn enc = encode_fn();
   if (!enc || g.C != 4 || (g.Wo & 15) || g.dT != 1 || g.dH != 1 || g.dW != 1 || g.kW > 8) return false;
   if (pitch < g.pW + g.W || pitch < (int64_t)(g.Wo - 1) * g.sW + 8 || (reinterpret_cast<uintptr_t>(ptr) & 15)) return false;
@@ -1694,31 +1508,16 @@ static bool make_tmap_stem(CUtensorMap* tm, const float* ptr, const vlfb_conv_ge
                         (cuuint64_t)pitch * 16 * g.H * g.T};
   // box_rows > 1: that many input rows `sH` apart (= consecutive OUTPUT rows) in one box: boxDim = rows * stride with
   // elementStride = stride loads ceil(boxDim / stride) = rows elements (cuTensorMapEncodeTiled)
-  // box_rows < 0: -box_rows CONSECUTIVE input rows (conv1 wgrad: the sH + kH rows two output rows' filter windows span)
-  cuuint32_t box[5] = {32, 16, (cuuint32_t)(box_rows > 1 ? box_rows * g.sH : (box_rows < 0 ? -box_rows : 1)), 1, 1};
+  cuuint32_t box[5] = {32, 16, (cuuint32_t)(box_rows > 1 ? box_rows * g.sH : 1), 1, 1};
   cuuint32_t estr[5] = {1, 1, (cuuint32_t)(box_rows > 1 ? g.sH : 1), 1, 1};
   if (box[2] > 256 || estr[2] > 8) return false;
   return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(base), dims, gstr, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// conv1 wgrad A operand in patch order: dY [N*To][Ho][Wo][Co] as a 4-D map; box {32 channels, 16 wo, 2 ho} = the 32 k-rows
-// of a patch chunk for one 32-channel atom, in the MN-major atom layout (SWIZZLE_128B_ATOM_32B).
-static bool make_tmap_dy4(CUtensorMap* tm, const float* dy, const vlfb_conv_geom_t& g) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc || (g.Co & 3) || (reinterpret_cast<uintptr_t>(dy) & 15)) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)g.Co, (cuuint64_t)g.Wo, (cuuint64_t)g.Ho, (cuuint64_t)g.N * g.To};
-  cuuint64_t gstr[3] = {(cuuint64_t)g.Co * 4, (cuuint64_t)g.Co * 4 * g.Wo, (cuuint64_t)g.Co * 4 * g.Wo * g.Ho};
-  cuuint32_t box[4] = {32, 16, 2, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(dy), dims, gstr, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // tuning overrides, read once (scripts/tune_gemm.py); the per-call fields of vlfb_gemm_params_t take precedence
-struct Env { int bn, stages, lag, sk, debug, no_patch, no_par; bool tma_mn, im2col, fuse_atoms; };
+struct Env { int bn, stages, lag, sk, debug, no_patch, no_par; bool im2col; };
 static Env read_env() {
   Env e;
   auto geti = [](const char* name, int dflt) { const char* v = getenv(name); return v ? atoi(v) : dflt; };
@@ -1729,9 +1528,7 @@ static Env read_env() {
   e.debug = geti("VLFB_DEBUG", 0);
   e.no_patch = geti("VLFB_NO_PATCH", 0);
   e.no_par = geti("VLFB_NO_PAR", 0);
-  e.tma_mn = geti("VLFB_TMA_MN", 1) != 0;
   e.im2col = geti("VLFB_IM2COL", 1) != 0;
-  e.fuse_atoms = geti("VLFB_FUSE_ATOMS", 1) != 0;
   return e;
 }
 static const Env& env() {
@@ -1763,8 +1560,8 @@ static bool wide_tiles(const vlfb_gemm_params_t& p) {
 
 struct Plan { int bn, split_k, pair, sk; int tiles, units; double cost; };
 
-// sk_ok = what the workspace allows; pow2_only: a 96-wide request becomes 64 (the cp.async MN-major loader needs a
-// power-of-two tile width).  p.pair is accepted and ignored: Hopper has no CTA-pair MMA (pair is always 0).
+// sk_ok = what the workspace allows; pow2_only: a 96-wide request becomes 64 (the cp.async MN-major loader, which
+// stages every MN-major B, needs a power-of-two tile width).  p.pair is accepted and ignored: Hopper has no CTA-pair MMA (pair is always 0).
 // Deterministic atomic launches (p.deterministic): no plain split-K and no atomic stream-K.  Their schedule is split 1 or
 // stream-K with the workspace fix-up (pieces summed in piece order), the latter weighed by the cost model unless
 // p.stream_k = -1, since it replaces the split-K that such a launch would otherwise take.
@@ -1774,7 +1571,7 @@ static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool
   const bool det = atomic && p.deterministic != 0;
   int want_bn = p.tile_n > 0 ? p.tile_n : env().bn;
   if (want_bn > BN_MAX) want_bn = BN_MAX;                                      // wider requests get the widest tile
-  if (pow2_only && (want_bn & (want_bn - 1))) want_bn = 64;
+  if (pow2_only && want_bn == 96) want_bn = 64;                                // (the one width not a power of two)
   const int want_sk = p.stream_k != 0 ? p.stream_k : env().sk;
   Plan best, best_sk;
   best.cost = 1e30; best.bn = 32; best.split_k = p.split_k > 0 ? p.split_k : 1; best.pair = 0; best.sk = 0;
@@ -1943,7 +1740,9 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   // a deterministic atomic launch whose operands are both MN-major may run its fix-ups in the cp.async build
   constexpr bool cp_fix = is_mn(AK) && is_mn(BK) && !MASK;
   Plan plan;
-  bool pow2_only = false;
+  // MN-major operands have no tensor map (sm_90 has no swizzle mode for their atom layout): the cp.async loaders stage
+  // them, and the MN-major B loader needs a power-of-two tile width
+  constexpr bool pow2_only = is_mn(BK);
   for (int attempt = 0; attempt < 4; ++attempt) {
     if (L.par) {                       // plan for the class sub-problems: M' rows, one z slice per class
       vlfb_gemm_params_t pp = p;
@@ -1955,19 +1754,10 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
     }
     L.bn = plan.bn;
     p.split_k = plan.split_k;
-    const int bnh = L.bn;
     memset(&tmA, 0, sizeof(tmA));
     memset(&tmB, 0, sizeof(tmB));
-    const bool mn_tma = ev.tma_mn;
-    L.tma_a = (AK == VLFB_OP_DENSE_K && make_tmap(&tmA, p.a, p.M, p.K, p.batch, BM)) ||
-              (AK == VLFB_OP_DENSE_MN && mn_tma && make_tmap_mn(&tmA, p.a, p.M, p.K, p.batch)) ? 1 : 0;
-    L.tma_b = (BK == VLFB_OP_DENSE_K && make_tmap(&tmB, p.b, p.N, p.K, p.batch, bnh)) ||
-              (BK == VLFB_OP_DENSE_MN && mn_tma && make_tmap_mn(&tmB, p.b, p.N, p.K, p.batch)) ? 1 : 0;
-    // MN-major tiles as ONE box (all atoms of the tile) instead of one box per 32-element atom
-    if (ev.fuse_atoms) {
-      if (AK == VLFB_OP_DENSE_MN && L.tma_a == 1 && make_tmap_mn4(&tmA, p.a, p.M, p.K, p.batch, BM / 32)) L.tma_a = 4;
-      if (BK == VLFB_OP_DENSE_MN && L.tma_b == 1 && make_tmap_mn4(&tmB, p.b, p.N, p.K, p.batch, bnh / 32)) L.tma_b = 4;
-    }
+    L.tma_a = AK == VLFB_OP_DENSE_K && make_tmap(&tmA, p.a, p.M, p.K, p.batch, BM) ? 1 : 0;
+    L.tma_b = BK == VLFB_OP_DENSE_K && make_tmap(&tmB, p.b, p.N, p.K, p.batch, L.bn) ? 1 : 0;
     if (ev.im2col) {
       // conv gathers as TMA im2col copies: one instruction per K chunk instead of 1024 16-byte cp.asyncs
       const int pad_lo[3] = {-g.pW, -g.pH, -g.pT};
@@ -1975,16 +1765,16 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       const int cstr[3] = {g.sW, g.sH, g.sT};
       const int ones[3] = {1, 1, 1};
       if (AK == VLFB_OP_CONV_K &&
-          make_tmap_im2col(&tmA, p.a.ptr, g.N, g.T, g.H, g.W, g.C, pad_lo, pad_hi, cstr, BM, CU_TENSOR_MAP_SWIZZLE_128B))
+          make_tmap_im2col(&tmA, p.a.ptr, g.N, g.T, g.H, g.W, g.C, pad_lo, pad_hi, cstr, BM))
         L.tma_a = 2;
       if (AK == VLFB_OP_DGRAD_K && unit_dgrad) {
         const int lo[3] = {g.pW - (g.kW - 1) * g.dW, g.pH - (g.kH - 1) * g.dH, g.pT - (g.kT - 1) * g.dT};
         const int hi[3] = {-g.pW, -g.pH, -g.pT};
-        if (make_tmap_im2col(&tmA, p.a.ptr, g.N, g.To, g.Ho, g.Wo, g.Co, lo, hi, ones, BM, CU_TENSOR_MAP_SWIZZLE_128B))
+        if (make_tmap_im2col(&tmA, p.a.ptr, g.N, g.To, g.Ho, g.Wo, g.Co, lo, hi, ones, BM))
           L.tma_a = 2;
       }
       if (AK == VLFB_OP_DGRAD_K && L.par) {
-        if (L.tma_b && make_tmap_im2col(&tmA, p.a.ptr, g.N, g.To, g.Ho, g.Wo, g.Co, par_lo, par_hi, ones, BM, CU_TENSOR_MAP_SWIZZLE_128B))
+        if (L.tma_b && make_tmap_im2col(&tmA, p.a.ptr, g.N, g.To, g.Ho, g.Wo, g.Co, par_lo, par_hi, ones, BM))
           L.tma_a = 2;
         else { L.par = 0; continue; }   // not addressable: plan again for the cp.async gather path (any geometry)
       }
@@ -1995,50 +1785,16 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
                              (!p.residual || ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && !(p.flags & VLFB_EPI_ACCUM)));
         L.stem_patch = 0;
         if (fast_ok && (g.Ho & 7) == 0 && (g.Wo & 15) == 0 && !ev.no_patch &&
-            make_tmap_stem(&tmA, p.a.ptr, g, p.a.ld, CU_TENSOR_MAP_SWIZZLE_128B, 8)) {
+            make_tmap_stem(&tmA, p.a.ptr, g, p.a.ld, 8)) {
           L.tma_a = 3;
           L.stem_patch = 1;
           L.patch_wb = g.Wo / 16;
           L.patch_hb = g.Ho / 8;
-        } else if (make_tmap_stem(&tmA, p.a.ptr, g, p.a.ld, CU_TENSOR_MAP_SWIZZLE_128B)) {
+        } else if (make_tmap_stem(&tmA, p.a.ptr, g, p.a.ld)) {
           L.tma_a = 3;
         }
       }
-      if (BK == VLFB_OP_STEM_MN && p.b.ld > 0 && L.tma_a) {
-        L.stem_patch = 0;
-        CUtensorMap tmA2;
-        memset(&tmA2, 0, sizeof(tmA2));
-        // patch chunks: needs dY dense [N*To][Ho][Wo][Co] (ld == M), whole patches, all filter rows in one N tile, and the
-        // sH + kH input-row slabs (2 KB each) inside the B stage
-        if (!ev.no_patch && AK == VLFB_OP_DENSE_MN && p.a.ld == p.M && p.batch == 1 && (g.Ho & 1) == 0 && (g.Wo & 15) == 0 &&
-            p.N <= L.bn && (g.sH + g.kH) * 2048 <= L.bn * KC * 4 && (p.K % KC) == 0 && g.sH <= 8 &&
-            make_tmap_stem(&tmB, p.b.ptr, g, p.b.ld, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, -(g.sH + g.kH)) &&
-            make_tmap_dy4(&tmA2, p.a.ptr, g)) {
-          tmA = tmA2;
-          L.tma_b = 3;
-          L.stem_patch = 1;
-          L.patch_wb = g.Wo / 16;
-          L.patch_hb = g.Ho / 2;
-        } else if (make_tmap_stem(&tmB, p.b.ptr, g, p.b.ld, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) {
-          L.tma_b = 3;
-        }
-      }
-      if (BK == VLFB_OP_CONV_MN && (g.C % KC) == 0 && L.tma_a &&
-          make_tmap_im2col(&tmB, p.b.ptr, g.N, g.T, g.H, g.W, g.C, pad_lo, pad_hi, cstr, KC,
-                           CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
-        L.tma_b = 2;
-      // ... and without spatial taps the whole B tile of a chunk is one dense box (make_tmap_conv_flat)
-      if (BK == VLFB_OP_CONV_MN && L.tma_b == 2 && ev.fuse_atoms &&
-          make_tmap_conv_flat(&tmB, p.b.ptr, g, bnh / 32))
-        L.tma_b = 5;
     }
-    if (L.wide) {
-      // wide tiles are staged by the cp.async loaders: the MN-major tensor maps' boxes are sized for 128 x bn tiles
-      // (and sm_90a does not encode their SWIZZLE_128B_ATOM_32B pattern)
-      L.tma_a = L.tma_b = 0;
-      L.stem_patch = 0;
-    }
-    if (is_mn(BK) && !L.tma_b && (L.bn & (L.bn - 1)) && !pow2_only) { pow2_only = true; continue; }
     const bool fixup = plan.sk && (!(p.flags & VLFB_EPI_ATOMIC) || det);
     if (!fixup || (L.tma_a && L.tma_b) || (cp_fix && det)) break;
     sk_ws = false;                     // an operand fell back to cp.async: plan again without fix-ups
@@ -2077,7 +1833,7 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
     }
   }
   const int smem = L.stages * stage_bytes + img_bytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  const bool cp = !(L.tma_a && L.tma_b);
+  const bool cp = is_mn(AK) || is_mn(BK) || !(L.tma_a && L.tma_b);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)units);
   cfg.blockDim = dim3((unsigned)((cp ? NPROD : NPROD_TMA) + NEPI));
@@ -2109,9 +1865,12 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       set_error("gemm_tc: stream-K fix-up planned for a cp.async build without one (kinds %d, %d)", AK, BK);
       return VLFB_E_UNSUPPORTED;
     }
-  } else if (cp) rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);
-  else if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
-  else rc = launch_variant<AK, BK, MASK, false, false>(cfg, p, L, tmA, tmB);
+  } else if (cp) {
+    rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);
+  } else if constexpr (!is_mn(AK) && !is_mn(BK)) {       // TMA-only builds exist for K-major pairs only
+    if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
+    else rc = launch_variant<AK, BK, MASK, false, false>(cfg, p, L, tmA, tmB);
+  }
   if (rc == VLFB_OK && bits_after) rc = relu_bits(p.d, bits_after, (int64_t)p.M * p.N, stream);
   return rc;
 }
