@@ -139,14 +139,21 @@ def _check_addressable(a, b, d):
 
 
 def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32_optional=False):
+    from vlfb import kernels as RK
     _check_addressable(a, b, d)
+    Bt, M, K = a.shape
+    N = b.shape[2]
+    if not RK._dim_ok(d.stride(2), N):          # the wrapper computes d^T = b^T a^T
+        M, N = N, M
+    # as kernels.matmul: a product split over K accumulates atomically, so with tf32_optional it declines the rounding
+    if tf32_out and tf32_optional and Bt * ((M + 127) // 128) * ((N + 255) // 256) <= RK.NUM_SMS // 2 and K >= 1024:
+        tf32_out = False
     r = torch.bmm(a, b) * alpha
     if bias is not None:
         r = r + bias
     if accumulate:
-        d.add_(r)
-    else:
-        d.copy_(_q(r, tf32_out))
+        r = d + r
+    d.copy_(_q(r, tf32_out))                    # the epilogue rounds an accumulated result too
     return bool(tf32_out)
 
 
@@ -237,19 +244,21 @@ def avgpool_bwd(dy, dx, g, accumulate=False):
         dx.copy_(r)
 
 
+# RoIAlign samples like the fp64 oracle (torchvision), in fp64 whatever the tensors' dtype: in fp32 torchvision rounds its
+# sample coordinates differently from the kernel's fp32 sample table, by more than a summation bound allows.
 def roi_align_fwd(feat, rois, out, spatial_scale, sampling_ratio=0):
     import torchvision
-    o = torchvision.ops.roi_align(feat.permute(0, 3, 1, 2), rois, (out.shape[1], out.shape[2]), spatial_scale,
-                                  sampling_ratio, False)
+    o = torchvision.ops.roi_align(feat.permute(0, 3, 1, 2).double(), rois.double(), (out.shape[1], out.shape[2]),
+                                  spatial_scale, sampling_ratio, False)
     out.copy_(o.permute(0, 2, 3, 1))
 
 
 def roi_align_bwd(dout, rois, dfeat, spatial_scale, sampling_ratio=0):
     import torchvision
-    f = torch.zeros(dfeat.permute(0, 3, 1, 2).shape, dtype=dout.dtype, requires_grad=True)
-    o = torchvision.ops.roi_align(f, rois, (dout.shape[1], dout.shape[2]), spatial_scale, sampling_ratio, False)
-    o.backward(dout.permute(0, 3, 1, 2))
-    dfeat.add_(f.grad.permute(0, 2, 3, 1))
+    f = torch.zeros(dfeat.permute(0, 3, 1, 2).shape, dtype=torch.float64, requires_grad=True)
+    o = torchvision.ops.roi_align(f, rois.double(), (dout.shape[1], dout.shape[2]), spatial_scale, sampling_ratio, False)
+    o.backward(dout.permute(0, 3, 1, 2).double())
+    dfeat.copy_(dfeat.double() + f.grad.permute(0, 2, 3, 1))
 
 
 def softmax_fwd(x, p, scale=1.0, tf32_out=False):

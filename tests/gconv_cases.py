@@ -292,6 +292,35 @@ def reference(case, t):
     return v, bound
 
 
+def reference_of_call(dir, g, groups, x=None, w=None, dy=None, wt=None, scale=None, bias=None, residual=None,
+                      relu=False, tf32=False, prev=None, mask=None, row_scale=None, col_scale=None):
+    """`reference` of one grouped vlfb.kernels call from its arguments: dir 'fwd' (conv_fwd: x, w, scale, bias,
+    residual, relu, tf32), 'dgrad' (conv_dgrad: dy, wt [C][taps][Cog] with any scale already folded in, prev = dx when
+    it accumulates, residual, mask = the ReLU mask as floats, tf32) or 'wgrad' (conv_wgrad: dy, x, prev = dw, row_scale,
+    col_scale = the col_mask).  Tensors channels-last as the wrapper takes them.  Returns (fp64 result in the output's
+    shape, bound)."""
+    case = dict(dir=dir, N=g.N, T=g.T, H=g.H, W=g.W, C=g.C, Co=g.Co, groups=int(groups), k=(g.kT, g.kH, g.kW),
+                s=(g.sT, g.sH, g.sW), p=(g.pT, g.pH, g.pW), d=(g.dT, g.dH, g.dW), epi={})
+    G, cig, cog, taps = int(groups), g.C // int(groups), g.Co // int(groups), g.kT * g.kH * g.kW
+    dev = next(v for v in (x, dy, w, wt) if v is not None).device
+    z = lambda *s: torch.zeros(s, dtype=torch.float64, device=dev)
+    if wt is not None:               # w[gi Cog + o][tap][i] = wt[gi Cig + i][tap][o]
+        w = wt.reshape(G, cig, taps, cog).permute(0, 3, 2, 1).reshape(g.Co, g.kT, g.kH, g.kW, cig)
+    t = dict(x=x if x is not None else z(g.N, g.T, g.H, g.W, g.C),
+             w=w if w is not None else z(g.Co, g.kT, g.kH, g.kW, cig),
+             dy=dy if dy is not None else z(g.N, g.To, g.Ho, g.Wo, g.Co))
+    for k, v in (('scale', scale), ('bias', bias), ('residual', residual), ('prev', prev), ('mask', mask),
+                 ('row_scale', row_scale), ('col_scale', col_scale)):
+        if v is not None:
+            t[k] = v
+            case['epi']['accum' if k == 'prev' else k] = 1
+    if relu:
+        case['epi']['relu'] = 1
+    if tf32:
+        case['epi']['tf32'] = 1
+    return reference(case, t)
+
+
 # ------------------------------------------------------------------------------------------------ running
 def _guarded(shape, device, fill=None):
     n = 1

@@ -253,6 +253,268 @@ def exact_f64(t):
     return t.double()
 
 
+# ----------------------------------------------------------------------------------------------- references
+# Each family's fp64 reference and elementwise bound as a function of the call's inputs (fp64 tensors on any device):
+# the builders below call them on seeded inputs, tests/launch_audit.py on the tensors of a real step.  The derivation of
+# every bound is at the family's builder.
+def axpby_ref(x, a, y, b):
+    ref = a * x + b * y
+    return ref, sum_bound(0, (a * x).abs() + (b * y).abs())
+
+
+def sigmoid_ref(x):
+    ref = torch.sigmoid(x)
+    return ref, ref * (1 - ref) * (C_EXP * 2.0 ** -22 + C_ARG * x.abs() * U) + 3 * U * ref
+
+
+def softmax_fwd_ref(x, scale, tf32_out):
+    cols = x.shape[-1]
+    sx = scale * x
+    z = sx - sx.max(-1, keepdim=True).values
+    ref = torch.softmax(z, -1)
+    e = C_ARG * (z.abs() + sx.abs()) * U
+    zbar = (ref * e).sum(-1, keepdim=True)
+    bound = ref * (C_SUM * (cols + 4) * U + C_EXP * 2.0 ** -22 + e + zbar)
+    if tf32_out:
+        bound = bound + ulp_tf32(ref)
+    return ref, bound
+
+
+def softmax_bwd_refb(p, dp, scale, tf32_out):
+    cols = p.shape[-1]
+    ref = softmax_bwd_ref(p, dp, scale)
+    bound = sum_bound(cols, scale * p * (dp.abs() + (p * dp).abs().sum(-1, keepdim=True)), k=4)
+    if tf32_out:
+        bound = bound + ulp_tf32(ref)
+    return ref, bound
+
+
+def layernorm_fwd_ref(x, eps):
+    """x [rows, cols] -> (y, y bound, mean, mean bound, std, std bound), the statistics as [rows, 1]."""
+    cols = x.shape[1]
+    mu = x.mean(1, keepdim=True)
+    dv = x - mu
+    var = (dv * dv).mean(1, keepdim=True)
+    sd = (var + eps).sqrt()
+    ref = dv / sd
+    n = -(-cols // 32) + 5
+    dmu = sum_bound(n, x.abs().mean(1, keepdim=True)) + U * mu.abs()
+    dvar = sum_bound(n, var) + 2 * dmu * dv.abs().mean(1, keepdim=True) + dmu ** 2
+    dsd = sd * (0.5 * dvar / (var + eps) + 2 * U)
+    bound = (dmu + U * dv.abs()) / sd + ref.abs() * (dsd / sd + 2 * U)
+    return ref, bound, mu, dmu, sd, dsd
+
+
+def layernorm_bwd_refb(dy, y, sd):
+    cols = dy.shape[1]
+    ref = layernorm_bwd_ref(dy, y, sd)
+    mag = (dy.abs() + dy.abs().mean(1, keepdim=True) + y.abs() * (dy * y).abs().mean(1, keepdim=True)) / sd
+    return ref, sum_bound(cols, mag, k=6)
+
+
+def colsum_ref(xs, prev, n):
+    """xs [rows, cols] fp64, prev [cols] or None (accumulate), n = terms of one fp32 chain."""
+    ref, mag = xs.sum(0), xs.abs().sum(0)
+    if prev is not None:
+        ref, mag = ref + prev, mag + prev.abs()
+    return ref, sum_bound(n, mag)
+
+
+def maxpool_bwd_refb(g, arg, dy, keep=None, prev=None, tf32_out=False):
+    """scatter form: prev = the finite contents dx starts from; gather form: keep = y > 0 (or None)."""
+    nk = g['kT'] * g['kH'] * g['kW']
+    ref, mag = _scatter_windows(g, arg, dy, keep)
+    if prev is not None:
+        ref, mag = ref + prev, mag + prev.abs()
+    bound = sum_bound(nk, mag)
+    if tf32_out:
+        bound = bound + ulp_tf32(ref)
+    return ref, bound
+
+
+def avgpool_fwd_ref(x, g):
+    import torch.nn.functional as F
+    nk = g['kT'] * g['kH'] * g['kW']
+    pool = lambda t: F.avg_pool3d(_nc(t, g), (g['kT'], g['kH'], g['kW']), (g['sT'], g['sH'], g['sW'])).permute(0, 2, 3, 4, 1)
+    return pool(x), sum_bound(nk, pool(x.abs()), k=3)
+
+
+def avgpool_bwd_refb(dy, g, prev=None):
+    nk = g['kT'] * g['kH'] * g['kW']
+    ref, mag = avgpool_bwd_ref(dy, g), avgpool_bwd_ref(dy.abs(), g)
+    if prev is not None:
+        ref, mag = ref + prev, mag + prev.abs()
+    return ref, sum_bound(nk, mag, k=3)
+
+
+def affine_ref(x, s, b):
+    ref = x * s + b
+    return ref, sum_bound(0, (x * s).abs() + b.abs())
+
+
+def roi_align_fwd_ref(M, nmax, feat2):
+    """M, nmax = roi_matrix(...); feat2 [N H W, C] fp64 -> [R PH PW, C]."""
+    return M @ feat2, sum_bound(nmax, M.abs() @ feat2.abs())
+
+
+def roi_align_bwd_ref(M, dout2, prev):
+    """dout2 [R PH PW, C], prev [N H W, C] (the finite contents the atomics add to)."""
+    ref = M.t() @ dout2 + prev
+    mag = M.abs().t() @ dout2.abs() + prev.abs()
+    terms = int((M != 0).sum(0).max()) + 1 if M.numel() else 1
+    return ref, sum_bound(terms, mag)
+
+
+def sigmoid_ce_fwd_ref(x, t, scale):
+    valid = t != -1
+    cnt = max(float(valid.sum()), 1e-5)
+    l = torch.nn.functional.binary_cross_entropy_with_logits(x, t.clamp(min=0).double(), reduction='none')
+    l = torch.where(valid, l, torch.zeros_like(l))
+    ref = (scale * l.sum() / cnt).view(1)
+    mag = (l.abs() + torch.where(valid, x.abs() + 2, torch.zeros_like(x)) * 2.0 ** -21).sum()
+    return ref, (sum_bound(x.numel(), mag, k=3) * abs(scale) / cnt).view(1)
+
+
+def sigmoid_ce_bwd_ref(x, t, scale, dl):
+    valid = t != -1
+    cnt = max(float(valid.sum()), 1e-5)
+    k = scale * dl / cnt
+    sg = torch.sigmoid(x)
+    ref = torch.where(valid, k * (sg - t.double()), torch.zeros_like(x))
+    bound = abs(k) * (sg * (1 - sg) * (C_EXP * 2.0 ** -22 + C_ARG * x.abs() * U) + 4 * U * (sg + t.double().abs()))
+    return ref, bound
+
+
+def sgd_ref(pd, gd, md, lr, mu, wd, nesterov):
+    """{'p', 'g', 'm'}: (value after the step, bound)."""
+    g2 = gd + wd * pd
+    eg = 2 * U * (gd.abs() + wd * pd.abs())
+    m2 = mu * md + lr * g2
+    em = 2 * U * (mu * md.abs() + lr * g2.abs()) + lr * eg
+    if nesterov:
+        st = (1 + mu) * m2 - mu * md
+        es = 3 * U * ((1 + mu) * m2.abs() + mu * md.abs()) + (1 + mu) * em
+    else:
+        st, es = m2, em
+    p2 = pd - st
+    ep = 2 * U * (pd.abs() + st.abs()) + es
+    return dict(p=(p2, ep), g=(st, es), m=(m2, em))
+
+
+def fbo_tau(L, dA, d, dB, nl):
+    return C_SUM * (dA + d + dB + L + 8) * U * nl
+
+
+def fbo_bound(ref, tau):
+    """The FBO stack's mixed bound: tau times the element's magnitude plus its row's mean magnitude."""
+    r = ref.detach()
+    m = r.abs().reshape(r.shape[0], -1).mean(1).view((-1,) + (1,) * (r.dim() - 1)) if r.dim() > 1 else r.abs().mean()
+    return tau * (r.abs() + m)
+
+
+def fbo_b_phi_bound(theta, aff_grad, tau):
+    """Bound of the phi bias gradient, theta_o sum_j dscore_j: exactly 0, up to the cancellation of the sum."""
+    return tau * theta.detach().abs().t() @ (aff_grad.abs().sum(1))
+
+
+def bn_infer_ref(x, s, b, rm, rv, eps):
+    fs = s / (rv + eps).sqrt()
+    ref = (x - rm) * fs + b
+    return ref, 6 * U * ((x - rm).abs() * fs.abs() + b.abs())
+
+
+def bn_fwd_ref(x, s, b, n, eps, rm=None, rv=None, mom=None):
+    """x [rows, C]; n = terms of one fp32 chain.  {'y', 'sm', 'siv' (, 'rm', 'rv')}: (ref, bound)."""
+    rows = x.shape[0]
+    x0 = x[0]
+    dev_ = x - x0
+    d = dev_.mean(0)
+    mean = x0 + d
+    E2 = (dev_ * dev_).mean(0)
+    var = (x - mean).pow(2).mean(0)
+    dd = sum_bound(n, dev_.abs().mean(0))
+    dmean = dd + U * mean.abs()
+    dvar = sum_bound(n, E2, k=3) + 2 * d.abs() * dd + dd ** 2
+    inv = 1.0 / (var + eps).sqrt()
+    dinv = inv * 0.5 * dvar / (var + eps)
+    fs = s * inv
+    dfs = s.abs() * dinv + U * fs.abs()
+    ref = (x - mean) * fs + b
+    bound = fs.abs() * (dmean + U * (x - mean).abs()) + (x - mean).abs() * dfs + 2 * U * ((x - mean).abs() * fs.abs() + b.abs())
+    out = dict(y=(ref, bound), sm=(mean, dmean), siv=(inv, dinv + U * inv))
+    if rm is not None:
+        unb = var * rows / (rows - 1) if rows > 1 else var
+        dunb = dvar * rows / (rows - 1) if rows > 1 else dvar
+        rm_ref, rv_ref = rm * mom + mean * (1 - mom), rv * mom + unb * (1 - mom)
+        out['rm'] = (rm_ref, (1 - mom) * dd + 2 * U * (rm_ref.abs() + rm.abs()))
+        out['rv'] = (rv_ref, (1 - mom) * dunb + 2 * U * (rv_ref.abs() + rv.abs()))
+    return out
+
+
+def bn_bwd_refb(dy, x, s, sm, siv, n, ds_prev=None, db_prev=None):
+    """{'dx' (, 'ds', 'db')}: (ref, bound); ds_prev / db_prev = the accumulated gradients' contents (None: not
+    computed)."""
+    m = x.shape[0]
+    s1, s2 = dy.sum(0), (dy * (x - sm)).sum(0)
+    ds1 = sum_bound(n, dy.abs().sum(0))
+    ds2 = sum_bound(n, (dy * (x - sm)).abs().sum(0), k=3)
+    A, B = s * siv, -s * siv ** 3 * s2 / m
+    Cc = -A * s1 / m - B * sm
+    dA = U * A.abs()
+    dB = s.abs() * siv ** 3 / m * ds2 + U * B.abs()
+    dC = A.abs() * ds1 / m + dA * s1.abs() / m + sm.abs() * dB + U * ((A * s1 / m).abs() + (B * sm).abs()) * 2
+    ref = bn_bwd_ref(dy, x, s, sm, siv)
+    bound = dy.abs() * dA + x.abs() * dB + dC + 3 * U * ((A * dy).abs() + (B * x).abs() + Cc.abs())
+    out = dict(dx=(ref, bound))
+    if ds_prev is not None:
+        out['ds'] = (ds_prev + s2 * siv, siv * ds2 + 2 * U * (ds_prev.abs() + (s2 * siv).abs()))
+    if db_prev is not None:
+        out['db'] = (db_prev + s1, ds1 + 2 * U * (db_prev.abs() + s1.abs()))
+    return out
+
+
+def softmax_ce_bwd_ref(pd, labd, scale):
+    rows = pd.shape[0]
+    onehot = torch.zeros_like(pd).scatter_(1, labd.view(-1, 1), 1.0)
+    return (pd - onehot) * scale / rows, 3 * U * (pd + onehot) * abs(scale) / rows
+
+
+def softmax_ce_fwd_ref(xd, labd, scale):
+    """{'prob', 'loss'}: (ref, bound)."""
+    rows, cols = xd.shape
+    n = -(-cols // 256) + 10
+    mx = xd.max(1, keepdim=True).values
+    z = xd - mx
+    ref = torch.softmax(xd, 1)
+    e = C_ARG * (z.abs() + xd.abs()) * U
+    rs = C_SUM * (n + 4) * U + C_EXP * 2.0 ** -22 + (ref * e).sum(1, keepdim=True)
+    logs = torch.logsumexp(z, 1)
+    lr = logs - z.gather(1, labd.view(-1, 1)).view(-1)
+    dl = 2.0 ** -21 + 4 * U * logs.abs() + rs.view(-1) + 2 * U * (xd.gather(1, labd.view(-1, 1)).view(-1).abs() + mx.view(-1).abs())
+    loss_ref = (scale * lr.sum() / rows).view(1)
+    lb = abs(scale) / rows * (dl.sum() + sum_bound(rows, lr.abs().sum(), k=3))
+    return dict(prob=(ref, ref * (rs + e)), loss=(loss_ref, lb.view(1)))
+
+
+def bank_scan_ref(bd, qd, scale, S, bf16, tf32_out):
+    """bd [R, L, D], qd [R, D] fp64, S = the split of a RoI's rows over CTAs.  {'out', 'prob'}: (ref, bound)."""
+    R, L, D = bd.shape
+    tiles = -(-(-(-L // S)) // scan_rows(D, bf16)) + 1
+    zs = scale * torch.einsum('rd,rld->rl', qd, bd)
+    p = torch.softmax(zs, 1)
+    z = zs - zs.max(1, keepdim=True).values
+    ds = sum_bound(D // 256 + 13, abs(scale) * torch.einsum('rd,rld->rl', qd.abs(), bd.abs()))
+    rng = zs.max(1, keepdim=True).values - zs.min(1, keepdim=True).values
+    rel = (ds + (p * ds).sum(1, keepdim=True) + tiles * (C_EXP * 2.0 ** -22 + 2 * U) * 2 + C_ARG * U * (z.abs() + rng) * 2
+           + C_SUM * (L + S + 4) * U)
+    ref = torch.einsum('rl,rld->rd', p, bd)
+    pb = p.unsqueeze(2) * bd.abs()
+    bound = torch.einsum('rl,rld->rd', rel, pb) + C_SUM * (L + S + 4) * U * pb.sum(1)
+    if tf32_out:
+        bound = bound + ulp_tf32(ref)
+    return dict(out=(ref, bound), prob=(p, p * rel))
+
+
 # ----------------------------------------------------------------------------------------------- builders
 BUILD = {}
 
@@ -300,8 +562,7 @@ def _ew(P, gen):
         if X['y'] is None:                  # y = NULL needs b = 0
             s1 = 0.0
         yv = torch.zeros((), dtype=torch.float64, device=P.dev) if X['y'] is None else f(X['y']).double()
-        ref = s0 * f(X['x']).double() + s1 * yv
-        bound = sum_bound(0, (s0 * f(X['x']).double()).abs() + (s1 * yv).abs())
+        ref, bound = axpby_ref(f(X['x']).double(), s0, yv, s1)
     elif fn == 'fill':
         ref = torch.full(tuple(shape), v, device=P.dev)
     elif fn == 'round_tf32':
@@ -318,9 +579,7 @@ def _ew(P, gen):
     elif fn == 'relu_bwd_tf32':
         ref = torch.where(f(X['y']) > 0, tf32_round(f(X['dy'])), torch.zeros((), device=P.dev))
     else:
-        x = f(X['x']).double()
-        ref = torch.sigmoid(x)
-        bound = ref * (1 - ref) * (C_EXP * 2.0 ** -22 + C_ARG * x.abs() * U) + 3 * U * ref
+        ref, bound = sigmoid_ref(f(X['x']).double())
     alias = c.get('alias')
     if alias:                   # out is one of the inputs: its buffer is that input's
         n = int(np.prod(shape))
@@ -465,14 +724,7 @@ def _softmax_fwd(P, gen):
     cols = a['x']['shape'][-1]
     scale = c.get('scale', 0.125)
     x = randn(a['x']['shape'], gen, c.get('spread', 3.0))
-    sx = scale * x.double().to(P.dev)
-    z = sx - sx.max(-1, keepdim=True).values
-    ref = torch.softmax(z, -1)
-    e = C_ARG * (z.abs() + sx.abs()) * U
-    zbar = (ref * e).sum(-1, keepdim=True)
-    bound = ref * (C_SUM * (cols + 4) * U + C_EXP * 2.0 ** -22 + e + zbar)
-    if a['tf32_out']:
-        bound = bound + ulp_tf32(ref)
+    ref, bound = softmax_fwd_ref(x.double().to(P.dev), scale, a['tf32_out'])
     p = place(P, 'p', a['p']['shape'], ref, bound, tol=6e-4 if a['tf32_out'] else 2e-5)
     xd = inp(P, x)
     P.call = lambda K: K.softmax_fwd(xd, p, scale, a['tf32_out'])
@@ -496,10 +748,7 @@ def _softmax_bwd(P, gen):
     p = torch.softmax(z, -1)
     dp = randn(a['dp']['shape'], gen)
     pd, dpd = p.double().to(P.dev), dp.double().to(P.dev)
-    ref = softmax_bwd_ref(pd, dpd, scale)
-    bound = sum_bound(cols, scale * pd * (dpd.abs() + (pd * dpd).abs().sum(-1, keepdim=True)), k=4)
-    if a['tf32_out']:
-        bound = bound + ulp_tf32(ref)
+    ref, bound = softmax_bwd_refb(pd, dpd, scale, a['tf32_out'])
     dx = place(P, 'dx', a['dx']['shape'], ref, bound, tol=6e-4 if a['tf32_out'] else 1e-4)
     p_, dp_ = inp(P, p), inp(P, dp)
     P.call = lambda K: K.softmax_bwd(p_, dp_, dx, scale, a['tf32_out'])
@@ -521,17 +770,7 @@ def _layernorm_fwd(P, gen):
     if c.get('content') == 'const_and_offset':             # constant rows (std = sqrt(eps)) and mean >> std rows
         x[0::3] = x[0::3, :1]
         x[1::3] = x[1::3] * 0.01 + 300.0
-    xd = x.double().to(P.dev)
-    mu = xd.mean(1, keepdim=True)
-    dv = xd - mu
-    var = (dv * dv).mean(1, keepdim=True)
-    sd = (var + eps).sqrt()
-    ref = dv / sd
-    n = -(-cols // 32) + 5
-    dmu = sum_bound(n, xd.abs().mean(1, keepdim=True)) + U * mu.abs()
-    dvar = sum_bound(n, var) + 2 * dmu * dv.abs().mean(1, keepdim=True) + dmu ** 2
-    dsd = sd * (0.5 * dvar / (var + eps) + 2 * U)
-    bound = (dmu + U * dv.abs()) / sd + ref.abs() * (dsd / sd + 2 * U)
+    ref, bound, mu, dmu, sd, dsd = layernorm_fwd_ref(x.double().to(P.dev), eps)
     y = place(P, 'y', (rows, cols), ref, bound)
     if c.get('content') == 'const_and_offset':
         # x - mean loses log2(|mean| / std) ~ 15 bits on the mean >> std rows, so their error is ~1e-3 of |y| (inside the
@@ -563,9 +802,8 @@ def _layernorm_bwd(P, gen):
     dy = randn((rows, cols), gen)
     sd = torch.rand(rows, generator=gen) + 0.5
     yd, dyd, sdd = y.double().to(P.dev), dy.double().to(P.dev), sd.double().to(P.dev).view(-1, 1)
-    ref = layernorm_bwd_ref(dyd, yd, sdd)
-    mag = (dyd.abs() + dyd.abs().mean(1, keepdim=True) + yd.abs() * (dyd * yd).abs().mean(1, keepdim=True)) / sdd
-    dx = place(P, 'dx', (rows, cols), ref, sum_bound(cols, mag, k=6), tol=1e-4)
+    ref, bound = layernorm_bwd_refb(dyd, yd, sdd)
+    dx = place(P, 'dx', (rows, cols), ref, bound, tol=1e-4)
     y_, dy_, sd_ = inp(P, y), inp(P, dy), inp(P, sd)
     P.call = lambda K: K.layernorm_bwd(dy_, y_, sd_, dx, cols)
     P.det = True
@@ -589,15 +827,10 @@ def _colsum(P, gen):
     rows, cols, ld = a['rows'], a['cols'], a['ld']
     x = randn(a['x']['shape'], gen)
     xs = x.reshape(-1)[:rows * ld].view(rows, ld)[:, :cols].double().to(P.dev)
-    ref = xs.sum(0)
-    mag = xs.abs().sum(0)
-    prev = None
-    if a['accumulate']:
-        prev = randn((cols,), gen).to(P.dev)
-        ref = ref + prev.double()
-        mag = mag + prev.double().abs()
+    prev = randn((cols,), gen).to(P.dev) if a['accumulate'] else None
     n, _, _ = colsum_terms(rows, cols)
-    out = place(P, 'out', a['out']['shape'], ref, sum_bound(n, mag), prev=prev, tol=2e-5)
+    ref, bound = colsum_ref(xs, None if prev is None else prev.double(), n)
+    out = place(P, 'out', a['out']['shape'], ref, bound, prev=prev, tol=2e-5)
     x_ = inp(P, x)
     P.call = lambda K: K.colsum(x_, ld, out, rows, cols, a['accumulate'])
 
@@ -680,22 +913,17 @@ def _maxpool_bwd(P, gen):
     xd = x.to(P.dev)
     y, arg = maxpool_ref(xd, g)
     dy = randn(a['dy']['shape'], gen).to(P.dev)
-    nk = g['kT'] * g['kH'] * g['kW']
     go = _conv_geom_obj(g)
     arg_ = inp(P, arg)
     dy_ = inp(P, dy)
     if c['fn'] == 'maxpool_bwd':
-        v, m = _scatter_windows(g, arg, dy)
         prev = randn(a['dx']['shape'], gen).to(P.dev)
-        ref, mag = v + prev.double(), m + prev.double().abs()
-        dx = place(P, 'dx', a['dx']['shape'], ref, sum_bound(nk, mag), prev=prev, tol=2e-5)
+        ref, bound = maxpool_bwd_refb(g, arg, dy, prev=prev.double())
+        dx = place(P, 'dx', a['dx']['shape'], ref, bound, prev=prev, tol=2e-5)
         P.call = lambda K: K.maxpool_bwd(dy_, arg_, dx, go)
         return
     keep = (y > 0) if a['y'] is not None else None
-    ref, mag = _scatter_windows(g, arg, dy, keep)
-    bound = sum_bound(nk, mag)
-    if a['tf32_out']:
-        bound = bound + ulp_tf32(ref)
+    ref, bound = maxpool_bwd_refb(g, arg, dy, keep, tf32_out=a['tf32_out'])
     dx = place(P, 'dx', a['dx']['shape'], ref, bound, tol=6e-4 if a['tf32_out'] else 2e-5)
     y_ = inp(P, y.float()) if a['y'] is not None else None
     P.call = lambda K: K.maxpool_bwd_gather(dy_, arg_, y_, dx, go, a['tf32_out'])
@@ -719,27 +947,21 @@ def avgpool_bwd_ref(dy, g, drop_window=False):
 def _avgpool(P, gen):
     """A sum of n = kT kH kW terms times fp32(1/n): C_SUM (n + 3) u sum |terms| (k = 3: the reciprocal, the product and
     the accumulate flag's addition of |prev|)."""
-    import torch.nn.functional as F
     c = P.case
     a = c['args']
     g = a['g']
-    nk = g['kT'] * g['kH'] * g['kW']
     go = _conv_geom_obj(g)
     if c['fn'] == 'avgpool_fwd':
         x = randn((g['N'], g['T'], g['H'], g['W'], g['C']), gen).to(P.dev)
-        pool = lambda t: F.avg_pool3d(_nc(t, g), (g['kT'], g['kH'], g['kW']), (g['sT'], g['sH'], g['sW'])).permute(0, 2, 3, 4, 1)
-        ref, mag = pool(x.double()), pool(x.double().abs())
-        y = place(P, 'y', a['y']['shape'], ref, sum_bound(nk, mag, k=3))
+        ref, bound = avgpool_fwd_ref(x.double(), g)
+        y = place(P, 'y', a['y']['shape'], ref, bound)
         x_ = inp(P, x)
         P.call = lambda K: K.avgpool_fwd(x_, y, go)
     else:
         dy = randn(a['dy']['shape'], gen).to(P.dev)
-        ref, mag = avgpool_bwd_ref(dy, g), avgpool_bwd_ref(dy.abs(), g)
-        prev = None
-        if a['accumulate']:
-            prev = randn(a['dx']['shape'], gen).to(P.dev)
-            ref, mag = ref + prev.double(), mag + prev.double().abs()
-        dx = place(P, 'dx', a['dx']['shape'], ref, sum_bound(nk, mag, k=3), prev=prev)
+        prev = randn(a['dx']['shape'], gen).to(P.dev) if a['accumulate'] else None
+        ref, bound = avgpool_bwd_refb(dy, g, None if prev is None else prev.double())
+        dx = place(P, 'dx', a['dx']['shape'], ref, bound, prev=prev)
         dy_ = inp(P, dy)
         P.call = lambda K: K.avgpool_bwd(dy_, dx, go, a['accumulate'])
     P.det = True
@@ -754,8 +976,7 @@ def _affine(P, gen):
     s = randn(a['s']['shape'], gen)
     b = randn(a['b']['shape'], gen) if c['fn'] == 'affine_fwd' else torch.zeros(a['s']['shape'])
     xd, sd, bd = x.double().to(P.dev), s.double().to(P.dev), b.double().to(P.dev)
-    ref = xd * sd + bd
-    bound = sum_bound(0, (xd * sd).abs() + bd.abs())
+    ref, bound = affine_ref(xd, sd, bd)
     x_, s_ = inp(P, x), inp(P, s)
     if c['fn'] == 'affine_fwd':
         y, b_ = place(P, 'y', a['y']['shape'], ref, bound), inp(P, b)
@@ -834,8 +1055,8 @@ def _roi_align(P, gen):
     if c['fn'] == 'roi_align_fwd':
         feat = randn((N, H, W, C), gen).to(P.dev)
         f2 = feat.double().view(N * H * W, C)
-        ref, mag = (M @ f2).view(R, PH, PW, C), (M.abs() @ f2.abs()).view(R, PH, PW, C)
-        out = place(P, 'out', a['out']['shape'], ref, sum_bound(nmax, mag))
+        ref, bound = roi_align_fwd_ref(M, nmax, f2)
+        out = place(P, 'out', a['out']['shape'], ref.view(R, PH, PW, C), bound.view(R, PH, PW, C))
         feat_ = inp(P, feat)
         P.call = lambda K: K.roi_align_fwd(feat_, rois_, out, scale, sr)
         P.det = True
@@ -843,10 +1064,8 @@ def _roi_align(P, gen):
         dout = randn((R, PH, PW, C), gen).to(P.dev)
         d2 = dout.double().view(R * PH * PW, C)
         prev = randn((N, H, W, C), gen).to(P.dev)
-        ref = (M.t() @ d2).view(N, H, W, C) + prev.double()
-        mag = (M.abs().t() @ d2.abs()).view(N, H, W, C) + prev.double().abs()
-        terms = int((M != 0).sum(0).max()) + 1
-        dfeat = place(P, 'dfeat', a['dfeat']['shape'], ref, sum_bound(terms, mag), prev=prev)
+        ref, bound = roi_align_bwd_ref(M, d2, prev.double().view(N * H * W, C))
+        dfeat = place(P, 'dfeat', a['dfeat']['shape'], ref.view(N, H, W, C), bound.view(N, H, W, C), prev=prev)
         dout_ = inp(P, dout)
         P.call = lambda K: K.roi_align_bwd(dout_, rois_, dfeat, scale, sr)
 
@@ -867,22 +1086,14 @@ def _sigmoid_ce(P, gen):
     if c.get('content') == 'all_ignored':
         t[:] = -1
     xd, td = x.double().to(P.dev), t.to(P.dev)
-    valid = td != -1
-    cnt = max(float(valid.sum()), 1e-5)
     x_, t_ = inp(P, x), inp(P, t)
     if c['fn'] == 'sigmoid_ce_fwd':
-        l = torch.nn.functional.binary_cross_entropy_with_logits(xd, td.clamp(min=0).double(), reduction='none')
-        l = torch.where(valid, l, torch.zeros_like(l))
-        ref = (scale * l.sum() / cnt).view(1)
-        mag = (l.abs() + torch.where(valid, xd.abs() + 2, torch.zeros_like(xd)) * 2.0 ** -21).sum()
-        loss = place(P, 'loss', (1,), ref, (sum_bound(int(np.prod(shape)), mag, k=3) * abs(scale) / cnt).view(1))
+        ref, bound = sigmoid_ce_fwd_ref(xd, td, scale)
+        loss = place(P, 'loss', (1,), ref, bound)
         P.call = lambda K: K.sigmoid_ce_fwd(x_, t_, loss, scale)
     else:
         dl = 0.5 if a['dloss'] is not None else 1.0
-        k = scale * dl / cnt
-        sg = torch.sigmoid(xd)
-        ref = torch.where(valid, k * (sg - td.double()), torch.zeros_like(xd))
-        bound = abs(k) * (sg * (1 - sg) * (C_EXP * 2.0 ** -22 + C_ARG * xd.abs() * U) + 4 * U * (sg + td.double().abs()))
+        ref, bound = sigmoid_ce_bwd_ref(xd, td, scale, dl)
         dx = place(P, 'dlogits', shape, ref, bound)
         dl_ = inp(P, torch.tensor([dl])) if a['dloss'] is not None else None
         P.call = lambda K: K.sigmoid_ce_bwd(x_, t_, dl_, dx, scale)
@@ -900,17 +1111,8 @@ def _sgd(P, gen):
     mu, wd, lr = (float(np.float32(v)) for v in (0.9, 1e-4, 0.01))      # the fp32 values the kernel uses
     p, g, m = randn(n, gen), randn(n, gen, 0.1), randn(n, gen, 0.05)
     pd, gd, md = p.double().to(P.dev), g.double().to(P.dev), m.double().to(P.dev)
-    g2 = gd + wd * pd
-    eg = 2 * U * (gd.abs() + wd * pd.abs())
-    m2 = mu * md + lr * g2
-    em = 2 * U * (mu * md.abs() + lr * g2.abs()) + lr * eg
-    if a['nesterov']:
-        st = (1 + mu) * m2 - mu * md
-        es = 3 * U * ((1 + mu) * m2.abs() + mu * md.abs()) + (1 + mu) * em
-    else:
-        st, es = m2, em
-    p2 = pd - st
-    ep = 2 * U * (pd.abs() + st.abs()) + es
+    r = sgd_ref(pd, gd, md, lr, mu, wd, a['nesterov'])
+    (p2, ep), (st, es), (m2, em) = r['p'], r['g'], r['m']
     pb, gb, mb = (_buffer(int(np.prod(n)), P.dev) for _ in range(3))
     idx = torch.arange(int(np.prod(n)), device=P.dev).view(n) + GUARD
     for b_, v in ((pb, p), (gb, g), (mb, m)):
@@ -982,12 +1184,8 @@ def _fbo_nl(P, gen):
     b64 = bp.double().to(P.dev).requires_grad_(True)
     W64 = [dict((k, v.double().to(P.dev).requires_grad_(True)) for k, v in W.items()) for W in Ws]
     A_ref, outs = fbo_ref(a64, b64, W64, scale, cf['pre_act_ln'], keeps, inv)
-    tau = C_SUM * (dA + d + dB + L + 8) * U * nl
-
-    def bnd(ref):
-        r = ref.detach()
-        m = r.abs().reshape(r.shape[0], -1).mean(1).view((-1,) + (1,) * (r.dim() - 1)) if r.dim() > 1 else r.abs().mean()
-        return tau * (r.abs() + m)
+    tau = fbo_tau(L, dA, d, dB, nl)
+    bnd = lambda ref: fbo_bound(ref, tau)
     dev = lambda t: inp(P, t.float())
     lay = []
     for i, W in enumerate(Ws):
@@ -1030,7 +1228,7 @@ def _fbo_nl(P, gen):
             grad = W64[i][k].grad.detach()
             b_ = bnd(grad)
             if k == 'b_phi':        # exactly 0: theta_o sum_j dscore_j, where the sum cancels to rounding noise
-                b_ = tau * o['theta'].detach().abs().t() @ (o['aff'].grad.abs().sum(1))
+                b_ = fbo_b_phi_bound(o['theta'], o['aff'].grad, tau)
             ld['g' + k] = place(P, 'L%d.g%s' % (i, k), tuple(Ws[i][k].shape), grad + 0.25, b_ + 2 * U * 0.25,
                                 prev=prev, tol=1e-4)
     da0 = place(P, 'da0', (R, dA), a64.grad.detach(), bnd(a64.grad), tol=5e-5)
@@ -1074,40 +1272,21 @@ def _bn_fwd(P, gen):
     rmd, rvd = rm0.double().to(P.dev), rv0.double().to(P.dev)
     x_, s_, b_ = inp(P, x.view(a['x']['shape'])), inp(P, s), inp(P, b)
     if c['fn'] == 'spatial_bn_infer':
-        fs = sd_ / (rvd + eps).sqrt()
-        ref = (xd - rmd) * fs + bd
-        bound = 6 * U * ((xd - rmd).abs() * fs.abs() + bd.abs())
+        ref, bound = bn_infer_ref(xd, sd_, bd, rmd, rvd, eps)
         y = place(P, 'y', a['y']['shape'], ref.view(a['y']['shape']), bound.view(a['y']['shape']))
         rm_, rv_ = inp(P, rm0), inp(P, rv0)
         P.call = lambda K: K.spatial_bn_infer(x_, s_, b_, rm_, rv_, y, eps)
         P.det = True
         return
-    n = bn_chain(rows, C)
-    x0 = xd[0]
-    dev_ = xd - x0
-    d = dev_.mean(0)
-    mean = x0 + d
-    E2 = (dev_ * dev_).mean(0)
-    var = (xd - mean).pow(2).mean(0)
-    dd = sum_bound(n, dev_.abs().mean(0))
-    dmean = dd + U * mean.abs()
-    dvar = sum_bound(n, E2, k=3) + 2 * d.abs() * dd + dd ** 2
-    inv = 1.0 / (var + eps).sqrt()
-    dinv = inv * 0.5 * dvar / (var + eps)
-    fs = sd_ * inv
-    dfs = sd_.abs() * dinv + U * fs.abs()
-    ref = (xd - mean) * fs + bd
-    bound = fs.abs() * (dmean + U * (xd - mean).abs()) + (xd - mean).abs() * dfs + 2 * U * ((xd - mean).abs() * fs.abs() + bd.abs())
+    r = bn_fwd_ref(xd, sd_, bd, bn_chain(rows, C), eps, *((rmd, rvd, mom) if a['rm'] is not None else ()))
+    ref, bound = r['y']
     y = place(P, 'y', a['y']['shape'], ref.view(a['y']['shape']), bound.view(a['y']['shape']))
-    sm = place(P, 'saved_mean', (C,), mean, dmean)
-    siv = place(P, 'saved_inv_std', (C,), inv, dinv + U * inv)
+    sm = place(P, 'saved_mean', (C,), *r['sm'])
+    siv = place(P, 'saved_inv_std', (C,), *r['siv'])
     rm = rv = None
     if a['rm'] is not None:
-        unb = var * rows / (rows - 1) if rows > 1 else var
-        dunb = dvar * rows / (rows - 1) if rows > 1 else dvar
-        rm_ref, rv_ref = rmd * mom + mean * (1 - mom), rvd * mom + unb * (1 - mom)
-        rm = place(P, 'running_mean', (C,), rm_ref, (1 - mom) * dd + 2 * U * (rm_ref.abs() + rmd.abs()), prev=rm0.to(P.dev))
-        rv = place(P, 'running_var', (C,), rv_ref, (1 - mom) * dunb + 2 * U * (rv_ref.abs() + rvd.abs()), prev=rv0.to(P.dev))
+        rm = place(P, 'running_mean', (C,), *r['rm'], prev=rm0.to(P.dev))
+        rv = place(P, 'running_var', (C,), *r['rv'], prev=rv0.to(P.dev))
     P.call = lambda K: K.spatial_bn_fwd(x_, s_, b_, rm, rv, sm, siv, y, eps, mom)
     P.det = True
 
@@ -1138,26 +1317,16 @@ def _bn_bwd(P, gen):
     siv = (1.0 / (x.double().var(0, unbiased=False) + 1e-5).sqrt()).float()
     xd, dyd, sd_ = x.double().to(P.dev), dy.double().to(P.dev), s.double().to(P.dev)
     smd, sivd = sm.double().to(P.dev), siv.double().to(P.dev)
-    n = bn_chain(rows, C)
-    m = rows
-    s1, s2 = dyd.sum(0), (dyd * (xd - smd)).sum(0)
-    ds1 = sum_bound(n, dyd.abs().sum(0))
-    ds2 = sum_bound(n, (dyd * (xd - smd)).abs().sum(0), k=3)
-    A, B = sd_ * sivd, -sd_ * sivd ** 3 * s2 / m
-    Cc = -A * s1 / m - B * smd
-    dA = U * A.abs()
-    dB = sd_.abs() * sivd ** 3 / m * ds2 + U * B.abs()
-    dC = A.abs() * ds1 / m + dA * s1.abs() / m + smd.abs() * dB + U * ((A * s1 / m).abs() + (B * smd).abs()) * 2
-    ref = bn_bwd_ref(dyd, xd, sd_, smd, sivd)
-    bound = dyd.abs() * dA + xd.abs() * dB + dC + 3 * U * ((A * dyd).abs() + (B * xd).abs() + Cc.abs())
-    dx = place(P, 'dx', a['dx']['shape'], ref.view(a['dx']['shape']), bound.view(a['dx']['shape']))
     p_s, p_b = randn((C,), gen).to(P.dev), randn((C,), gen).to(P.dev)
+    r = bn_bwd_refb(dyd, xd, sd_, smd, sivd, bn_chain(rows, C), p_s.double() if a['ds'] is not None else None,
+                    p_b.double() if a['db'] is not None else None)
+    ref, bound = r['dx']
+    dx = place(P, 'dx', a['dx']['shape'], ref.view(a['dx']['shape']), bound.view(a['dx']['shape']))
     ds = db = None
     if a['ds'] is not None:
-        ds = place(P, 'dscale', (C,), p_s.double() + s2 * sivd,
-                   sivd * ds2 + 2 * U * (p_s.double().abs() + (s2 * sivd).abs()), prev=p_s)
+        ds = place(P, 'dscale', (C,), *r['ds'], prev=p_s)
     if a['db'] is not None:
-        db = place(P, 'dbias', (C,), p_b.double() + s1, ds1 + 2 * U * (p_b.double().abs() + s1.abs()), prev=p_b)
+        db = place(P, 'dbias', (C,), *r['db'], prev=p_b)
     x_, dy_, s_, sm_, siv_ = (inp(P, t) for t in (x.view(a['x']['shape']), dy.view(a['dy']['shape']), s, sm, siv))
     P.call = lambda K: K.spatial_bn_bwd(dy_, x_, s_, sm_, siv_, dx, ds, db)
     P.det = True
@@ -1180,28 +1349,15 @@ def _softmax_ce(P, gen):
     labd = lab.long().to(P.dev)
     if c['fn'] == 'softmax_ce_bwd':
         prob = torch.softmax(x, 1)
-        pd = prob.double().to(P.dev)
-        onehot = torch.zeros_like(pd).scatter_(1, labd.view(-1, 1), 1.0)
-        ref = (pd - onehot) * scale / rows
-        dx = place(P, 'dlogits', (rows, cols), ref, 3 * U * (pd + onehot) * abs(scale) / rows)
+        ref, bound = softmax_ce_bwd_ref(prob.double().to(P.dev), labd, scale)
+        dx = place(P, 'dlogits', (rows, cols), ref, bound)
         p_ = inp(P, prob)
         P.call = lambda K: K.softmax_ce_bwd(p_, lab_, dx, scale)
         P.det = True
         return
-    n = -(-cols // 256) + 10
-    xd = x.double().to(P.dev)
-    mx = xd.max(1, keepdim=True).values
-    z = xd - mx
-    ref = torch.softmax(xd, 1)
-    e = C_ARG * (z.abs() + xd.abs()) * U
-    rs = C_SUM * (n + 4) * U + C_EXP * 2.0 ** -22 + (ref * e).sum(1, keepdim=True)
-    prob = place(P, 'prob', (rows, cols), ref, ref * (rs + e))
-    logs = torch.logsumexp(z, 1)
-    lr = logs - z.gather(1, labd.view(-1, 1)).view(-1)
-    dl = 2.0 ** -21 + 4 * U * logs.abs() + rs.view(-1) + 2 * U * (xd.gather(1, labd.view(-1, 1)).view(-1).abs() + mx.view(-1).abs())
-    loss_ref = (scale * lr.sum() / rows).view(1)
-    lb = abs(scale) / rows * (dl.sum() + sum_bound(rows, lr.abs().sum(), k=3))
-    loss = place(P, 'loss', (1,), loss_ref, lb.view(1))
+    r = softmax_ce_fwd_ref(x.double().to(P.dev), labd, scale)
+    prob = place(P, 'prob', (rows, cols), *r['prob'])
+    loss = place(P, 'loss', (1,), *r['loss'])
     x_ = inp(P, x)
     P.call = lambda K: K.softmax_ce_fwd(x_, lab_, prob, loss, scale)
     P.det = True
@@ -1247,22 +1403,9 @@ def _bank_scan(P, gen):
     q = randn((R, D), gen)
     S = scan_splits(R, L, D, bf16)
     P.splits = S
-    tiles = -(-(-(-L // S)) // scan_rows(D, bf16)) + 1
-    bd, qd = bank.double().to(P.dev), q.double().to(P.dev)
-    zs = scale * torch.einsum('rd,rld->rl', qd, bd)
-    p = torch.softmax(zs, 1)
-    z = zs - zs.max(1, keepdim=True).values
-    ds = sum_bound(D // 256 + 13, abs(scale) * torch.einsum('rd,rld->rl', qd.abs(), bd.abs()))
-    rng = zs.max(1, keepdim=True).values - zs.min(1, keepdim=True).values
-    rel = (ds + (p * ds).sum(1, keepdim=True) + tiles * (C_EXP * 2.0 ** -22 + 2 * U) * 2 + C_ARG * U * (z.abs() + rng) * 2
-           + C_SUM * (L + S + 4) * U)
-    ref = torch.einsum('rl,rld->rd', p, bd)
-    pb = p.unsqueeze(2) * bd.abs()
-    bound = torch.einsum('rl,rld->rd', rel, pb) + C_SUM * (L + S + 4) * U * pb.sum(1)
-    if a['tf32_out']:
-        bound = bound + ulp_tf32(ref)
-    out = place(P, 'out', (R, D), ref, bound, tol=6e-4 if a['tf32_out'] else 1e-4)
-    prob = place(P, 'prob', (R, L), p, p * rel) if a['prob'] is not None else None
+    r = bank_scan_ref(bank.double().to(P.dev), q.double().to(P.dev), scale, S, bf16, a['tf32_out'])
+    out = place(P, 'out', (R, D), *r['out'], tol=6e-4 if a['tf32_out'] else 1e-4)
+    prob = place(P, 'prob', (R, L), *r['prob']) if a['prob'] is not None else None
     b_, q_ = inp(P, bank), inp(P, q)
     P.call = lambda K: K.fbo_bank_scan(b_, q_, out, scale, prob, a['tf32_out'])
     P.det = True
