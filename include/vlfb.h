@@ -87,7 +87,8 @@ typedef struct {
                                * rejected with VLFB_E_BADARG, not evaluated as D = epi(0) */
   int batch;                  /* >= 1 (DENSE only)                           */
   int taps;                   /* wgrad: number of temporal taps kT (z-slices), else 1 */
-  int split_k;                /* >= 1 (>1 needs VLFB_EPI_ATOMIC); 0 = the library picks it with the tile width */
+  int split_k;                /* >= 1 (>1 needs VLFB_EPI_ATOMIC); 0 = the library picks it with the tile width (1
+                               * without VLFB_EPI_ATOMIC) */
   float* d;                   /* output rows: d + batch*d_batch_stride + m*ldd + n (+ tap*d_tap_stride) */
   int64_t ldd, d_batch_stride, d_tap_stride;
   float alpha;                /* applied first                               */

@@ -32,12 +32,17 @@ GUARD = 64                     # floats of NaN on each side of every output
 CASES = []
 
 
-def _case(name, dir, shape, co, groups, k=(1, 3, 3), s=(1, 1, 1), p=None, d=(1, 1, 1), family=None, seed=0, **epi):
+def make_case(name, dir, shape, co, groups, k=(1, 3, 3), s=(1, 1, 1), p=None, d=(1, 1, 1), family=None, seed=0, **epi):
+    """One case dict.  epi: the epilogue fields (scale, bias, ...) and det = 1 for a deterministic call."""
     n, t, h, w, c = shape
     if p is None:
         p = tuple(dd * (kk // 2) for kk, dd in zip(k, d))
-    CASES.append(dict(name=name, dir=dir, N=n, T=t, H=h, W=w, C=c, Co=co, groups=groups, k=tuple(k), s=tuple(s),
-                      p=tuple(p), d=tuple(d), family=family or dir, seed=seed, epi=epi))
+    return dict(name=name, dir=dir, N=n, T=t, H=h, W=w, C=c, Co=co, groups=groups, k=tuple(k), s=tuple(s),
+                p=tuple(p), d=tuple(d), family=family or dir, seed=seed, epi=epi)
+
+
+def _case(*a, **kw):
+    CASES.append(make_case(*a, **kw))
 
 
 # widths: Cig = Cog of 4, 8, 16, 32, 64 in every direction, plus Cig != Cog
@@ -354,6 +359,7 @@ def prepare(case, t, out, bits):
     else:
         p = _params_wgrad(K, case, t, out, g, G)
     p.alpha = float(e.get('alpha', 1.0))
+    p.deterministic = int(e.get('det', 0))
     return p, (mask, mbits)
 
 
@@ -463,7 +469,9 @@ def compare(case, t, buf, got, bits, ref, bound):
                     max_err=float(err.max()) if finite else float('inf'))
 
 
-def run_case(case, device='cuda'):
+def run_case(case, device='cuda', keep_out=False):
+    """Runs the case once; returns its stats (with keep_out, also 'out': the guarded output buffer and the sign bits as
+    int32 bits, for a bitwise comparison of two runs)."""
     t = make_tensors(case, device)
     ref, bound = reference(case, t)
     buf, out = _guarded(t['out_shape'], device, t.get('prev'))
@@ -484,6 +492,8 @@ def run_case(case, device='cuda'):
     st['record'] = rec
     st['record_ok'] = rec is not None and all(rec.get(k) == v for k, v in want.items())
     st['ok'] = ok and st['record_ok']
+    if keep_out:
+        st['out'] = torch.cat([buf.view(torch.int32)] + ([bits] if bits is not None else [])).cpu()
     return st
 
 

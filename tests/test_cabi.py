@@ -45,6 +45,29 @@ def test_argument_validation_without_gpu():
     assert lib.vlfb_relu_fwd(None, None, 4, None) == -1
 
 
+def test_split_k_zero_on_a_stored_output_means_one_split():
+    """include/vlfb.h: split_k = 0 lets the library pick the split, which is 1 without VLFB_EPI_ATOMIC -- so a stored
+    output with a residual and TF32 rounding is accepted (validation goes on to the next rule, here an unknown operand
+    kind), while an explicit split without VLFB_EPI_ATOMIC stays rejected, on both engines."""
+    from vlfb import libvlfb as L
+    lib = L.load()
+    p = L.GemmParams()
+    p.a.ptr = p.b.ptr = p.d = p.residual = 256              # never dereferenced: validation fails first
+    p.M, p.N, p.K, p.batch, p.taps, p.ldd = 128, 128, 4096, 1, 1, 128
+    p.flags = L.EPI_TF32
+    p.a.kind = 99
+    for engine in (L.ENGINE_TCGEN05, L.ENGINE_SIMT):
+        p.engine = engine
+        p.split_k = 0
+        assert lib.vlfb_gemm(ctypes.byref(p), None) == -1 and b'unknown operand kind' in lib.vlfb_last_error()
+        p.split_k = 2
+        assert lib.vlfb_gemm(ctypes.byref(p), None) == -1 and b'VLFB_EPI_ATOMIC' in lib.vlfb_last_error()
+        p.deterministic = 1                                 # a deterministic call: 0 is still one split
+        p.split_k = 0
+        assert lib.vlfb_gemm(ctypes.byref(p), None) == -1 and b'unknown operand kind' in lib.vlfb_last_error()
+        p.deterministic = 0
+
+
 def test_struct_layout_matches_header(tmp_path):
     """sizeof / offsetof of the C structs, as the C compiler sees include/vlfb.h, equal the ctypes mirror."""
     import subprocess

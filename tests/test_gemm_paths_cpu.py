@@ -41,58 +41,15 @@ def test_case_table_is_well_formed():
     assert all(any(cfg in c['runs'] for c in GP.CASES) for cfg in GP.CONFIGS)
 
 
-def _abi_errors(c):
-    """The rules of validate_gemm (csrc/api.cu) for the call the case makes, plus the conditions that keep it on the
-    tensor-core engine (a SIMT fallback would have no path record)."""
-    d = GP.describe(c)
-    f = d['flags']
-    ak, bk = d['kinds']
-    M, N, K = d['M'], d['N'], d['K']
-    e = c.get('epi', {})
-    err = []
-    if not (M > 0 and N > 0 and K > 0):
-        err.append('M, N, K must be > 0')
-    if K > GP.KMAX:
-        err.append('K above the range of the table')
-    if f['split_k'] != 1 and not f['atomic']:
-        err.append('split_k != 1 needs VLFB_EPI_ATOMIC')
-    if f['split_k'] != 1 and (f['residual'] or f['mask'] or f['relu'] or f['tf32']):
-        err.append('split-K with a non-linear epilogue')
-    if e.get('bits') and not (f['relu'] and not f['atomic'] and N % 32 == 0):
-        err.append('relu_bits_out needs RELU, no atomic, N % 32 == 0')
-    if f['mask'] and not ((ak, bk) in ((GP.OP_DGRAD_K, GP.OP_DENSE_K), (GP.OP_DENSE_K, GP.OP_DENSE_K))):
-        err.append('relu_mask on other kinds than DGRAD_K/DENSE_K x DENSE_K')
-    g = c.get('geom')
-    if g is not None:
-        kT, kH, kW = g['ker']
-        To, Ho, Wo = GP.out_dims(g)
-        if ak == GP.OP_CONV_K and not (g['C'] % 32 == 0 and K == kT * kH * kW * g['C']):
-            err.append('CONV_K needs C % 32 == 0')
-        if ak == GP.OP_DGRAD_K and not (g['Co'] % 32 == 0 and K == kT * kH * kW * g['Co']):
-            err.append('DGRAD_K needs Co % 32 == 0')
-        if bk == GP.OP_CONV_MN and not (N == kH * kW * g['C'] and g['C'] % 4 == 0 and d['taps'] == kT and kH <= 8 and kW <= 8):
-            err.append('CONV_MN extents')
-        if GP.OP_STEM_K in (ak, bk) or GP.OP_STEM_MN in (ak, bk):
-            if not (g['C'] == 4 and kW <= 8 and tuple(g['dil']) == (1, 1, 1)):
-                err.append('stem geometry')
-            if bk == GP.OP_STEM_MN and not (N == 32 * kH and kH <= 8 and d['taps'] == kT):
-                err.append('STEM_MN extents')
-            if ak == GP.OP_STEM_K and K != kT * kH * 32:
-                err.append('STEM_K extents')
-    else:
-        if not c['a_mn'] and K % 4:
-            err.append('DENSE_K operand with K % 4 != 0 runs on the SIMT engine')
-        if (c['a_mn'] and M % 4) or (c['b_mn'] and N % 4):
-            err.append('DENSE_MN operand with an extent % 4 != 0 runs on the SIMT engine')
-    if c.get('opts', {}).get('tile_n') not in (None, 0, 32, 64, 96, 128):
-        err.append('tile_n')
-    return err
-
-
 @pytest.mark.parametrize('name', [c['name'] for c in GP.CASES])
 def test_case_is_a_legal_tensor_core_call(name):
     c = GP.case_by_name(name)
-    assert _abi_errors(c) == []
+    assert GP.abi_errors(c) == []
+    # (a SIMT fallback would have no path record to check against the declared path; only a case that asks for the
+    # SIMT engine runs there)
+    assert GP.engine(c) == c.get('engine', 'tc')
+    assert GP.describe(c)['K'] <= GP.KMAX
+    assert c.get('opts', {}).get('tile_n', 0) in (0, 32, 64, 96, 128)
     # ... and the host-only plan query accepts its extents
     from vlfb import libvlfb as L
     lib = L.load()

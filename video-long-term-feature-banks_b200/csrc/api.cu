@@ -23,7 +23,7 @@ static int validate_gemm(const vlfb_gemm_params_t& p, bool& tc_ok) {
   tc_ok = true;
   VLFB_CHECK_ARG(p.a.ptr && p.b.ptr && p.d);
   VLFB_CHECK_ARG(p.M > 0 && p.N > 0 && p.K > 0);      // K = 0 (an empty sum) is rejected by both engines alike
-  VLFB_CHECK_ARG(p.batch >= 1 && p.taps >= 1 && p.split_k >= 0);          // split_k 0 = chosen by the library
+  VLFB_CHECK_ARG(p.batch >= 1 && p.taps >= 1 && p.split_k >= 0);          // split_k 0 (atomic) = chosen by the library
   VLFB_CHECK_ARG(!(p.taps > 1 && p.batch > 1));
   VLFB_CHECK_ARG(p.engine == VLFB_ENGINE_TCGEN05 || p.engine == VLFB_ENGINE_SIMT);
   VLFB_CHECK_ARG(p.tile_n == 0 || (p.tile_n >= 32 && p.tile_n <= 256 && p.tile_n % 32 == 0));
@@ -207,19 +207,23 @@ int vlfb_gemm(const vlfb_gemm_params_t* p, void* stream) {
     const int rc = validate_gconv(*p);
     return rc != VLFB_OK ? rc : gconv(*p, static_cast<cudaStream_t>(stream));
   }
+  // split_k = 0 is the library's choice: a split for atomic epilogues, none for a stored output (each engine would
+  // otherwise pick its own split, and a stored split overwrites its partial sums)
+  vlfb_gemm_params_t q = *p;
+  if (q.split_k == 0 && !(q.flags & VLFB_EPI_ATOMIC)) q.split_k = 1;
   bool tc_ok = true;
-  int rc = validate_gemm(*p, tc_ok);
+  int rc = validate_gemm(q, tc_ok);
   if (rc != VLFB_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (p->engine == VLFB_ENGINE_SIMT || !tc_ok) {
+  if (q.engine == VLFB_ENGINE_SIMT || !tc_ok) {
     // the cross-check engine stores element by element: the sign bits are a second pass over the dense output
-    vlfb_gemm_params_t q = *p;
+    uint32_t* bits = q.relu_bits_out;
     q.relu_bits_out = nullptr;
     rc = gemm_simt(q, s);
-    if (rc == VLFB_OK && p->relu_bits_out) rc = relu_bits(p->d, p->relu_bits_out, (int64_t)p->M * p->N, s);
+    if (rc == VLFB_OK && bits) rc = relu_bits(q.d, bits, (int64_t)q.M * q.N, s);
     return rc;
   }
-  return gemm_tc(*p, s);
+  return gemm_tc(q, s);
 }
 
 }  // extern "C"

@@ -1779,8 +1779,10 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
         else { L.par = 0; continue; }   // not addressable: plan again for the cp.async gather path (any geometry)
       }
       if (AK == VLFB_OP_STEM_K && p.a.ld > 0) {
-        // patch tiles need the lean epilogue's row mapping: whole 16-column blocks, 16-byte addressable rows, no mask
-        const bool fast_ok = (p.N & 15) == 0 && (p.ldd & 3) == 0 && (p.d_batch_stride & 3) == 0 && (p.d_tap_stride & 3) == 0 &&
+        // patch tiles need the lean epilogue's row mapping: a TMA-only build (B by TMA too: a cp.async build stores
+        // through the general epilogue, which maps tile rows linearly), whole 16-column blocks, 16-byte addressable
+        // rows, no mask
+        const bool fast_ok = L.tma_b && (p.N & 15) == 0 && (p.ldd & 3) == 0 && (p.d_batch_stride & 3) == 0 && (p.d_tap_stride & 3) == 0 &&
                              (reinterpret_cast<uintptr_t>(p.d) & 15) == 0 && !p.relu_mask && !MASK &&
                              (!p.residual || ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && !(p.flags & VLFB_EPI_ACCUM)));
         L.stem_patch = 0;
