@@ -10,18 +10,14 @@ import torch.nn.functional as F
 
 from vlfb import libvlfb as L
 from vlfb.kernels import conv_geom, out_shape, _is_pointwise  # noqa: F401  (pure python helpers)
+from util import pack_sign_bits, tf32_round
 
 
 EMULATE_TF32 = False     # True: perform the TF32 roundings of the CUDA path (in whatever dtype the tensors have)
 
 
-def _rt(t):
-    i = t.detach().to(torch.float32).contiguous().view(torch.int32)
-    return ((i + 0x1000) & ~0x1FFF).view(torch.float32).to(t.dtype)
-
-
 def _q(t, on=True):
-    return _rt(t) if (EMULATE_TF32 and on) else t
+    return tf32_round(t.detach()) if (EMULATE_TF32 and on) else t
 
 
 def set_gemm_backend(name):
@@ -44,19 +40,13 @@ def _stem_w(w, g):
     return w[:, :, :, :g.kW, :3].permute(0, 4, 1, 2, 3)
 
 
-def _pack_bits(x, bits):
-    b = (x.reshape(-1, 32) > 0).to(torch.int64)
-    v = (b << torch.arange(32, dtype=torch.int64)).sum(1)
-    bits.copy_(torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32))
-
-
 def _unpack_bits(bits, shape):
     v = bits.to(torch.int64) & 0xFFFFFFFF
     return ((v.view(-1, 1) >> torch.arange(32, dtype=torch.int64)) & 1).reshape(shape) > 0
 
 
 def relu_bits(x, bits):
-    _pack_bits(x, bits)
+    bits.copy_(pack_sign_bits(x))
 
 
 def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_out=False, relu_bits=None):
@@ -76,7 +66,7 @@ def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_
     y.copy_(_q(o, tf32_out))
     if relu_bits is not None:
         assert relu
-        _pack_bits(y, relu_bits)
+        relu_bits.copy_(pack_sign_bits(y))
 
 
 def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, tf32_out=False, relu_mask_bits=None):
@@ -328,7 +318,7 @@ def fill(x, v):
 
 def round_tf32(x, y):
     if EMULATE_TF32:
-        y.copy_(_rt(x))
+        y.copy_(tf32_round(x.detach()))
     elif y.data_ptr() != x.data_ptr():
         y.copy_(x)
 

@@ -24,6 +24,8 @@ import sys
 import torch
 import torch.nn.functional as F
 
+from util import capture_fd2, compare, guard_touched, nan_buffer, pack_sign_bits, parse_record, tf32_round
+
 U32 = 2.0 ** -24
 TF32_ULP = 2.0 ** -10
 GUARD = 64                     # floats of NaN on each side of every output
@@ -180,12 +182,6 @@ def check_table():
 
 
 # ------------------------------------------------------------------------------------------------ reference
-def _rt(t):
-    """cvt.rna.tf32.f32 of an fp32 tensor."""
-    i = t.contiguous().view(torch.int32)
-    return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
-
-
 def _nc(x):
     return x.permute(0, 4, 1, 2, 3)
 
@@ -205,9 +201,9 @@ def make_tensors(case, device):
 
     kt, kh, kw = case['k']
     t = {}
-    t['x'] = _rt(rnd(g.N, g.T, g.H, g.W, g.C))
-    t['w'] = _rt(rnd(g.Co, kt, kh, kw, g.C // G, scale=0.2))
-    t['dy'] = _rt(rnd(g.N, g.To, g.Ho, g.Wo, g.Co))
+    t['x'] = tf32_round(rnd(g.N, g.T, g.H, g.W, g.C))
+    t['w'] = tf32_round(rnd(g.Co, kt, kh, kw, g.C // G, scale=0.2))
+    t['dy'] = tf32_round(rnd(g.N, g.To, g.Ho, g.Wo, g.Co))
     e = case['epi']
     d = case['dir']
     ncols = g.Co if d == 'fwd' else (g.C if d == 'dgrad' else kh * kw * (g.C // G))
@@ -250,7 +246,7 @@ def reference(case, t):
         wsc = w64
         if e.get('scale'):           # the dgrad B operand arrives with the affine scale folded (weight_transpose)
             wsc = w64 * t['scale'].double().view(-1, 1, 1, 1, 1)
-            wsc = _rt(wsc.float()).double()
+            wsc = tf32_round(wsc.float()).double()
         acc = dgrad(dy64, wsc)
         mag = dgrad(dy64.abs(), wsc.abs())
     else:
@@ -327,22 +323,6 @@ def reference_of_call(dir, g, groups, x=None, w=None, dy=None, wt=None, scale=No
 
 
 # ------------------------------------------------------------------------------------------------ running
-def _guarded(shape, device, fill=None):
-    n = 1
-    for s in shape:
-        n *= s
-    buf = torch.full((n + 2 * GUARD,), float('nan'), dtype=torch.float32, device=device)
-    if fill is not None:
-        buf[GUARD:GUARD + n] = fill.reshape(-1)
-    return buf, buf[GUARD:GUARD + n].view(shape)
-
-
-def _pack_bits(x):
-    b = (x.reshape(-1, 32) > 0).to(torch.int64)
-    v = (b << torch.arange(32, dtype=torch.int64, device=x.device)).sum(1)
-    return torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32)
-
-
 def prepare(case, t, out, bits):
     """The vlfb_gemm parameter block of the case (dgrad: the grouped wt is built here) and the tensors it reads."""
     from vlfb import kernels as K
@@ -351,7 +331,7 @@ def prepare(case, t, out, bits):
     G = case['groups']
     d = case['dir']
     mask = t.get('mask') if e.get('mask') == 'float' else None
-    mbits = _pack_bits(t['mask']) if e.get('mask') == 'bits' else None
+    mbits = pack_sign_bits(t['mask']) if e.get('mask') == 'bits' else None
     if d == 'fwd':
         p = _params_fwd(K, case, t, out, g, G, mask, mbits, bits)
     elif d == 'dgrad':
@@ -451,42 +431,45 @@ def _params_wgrad(K, case, t, out, g, G):
     return p
 
 
-def compare(case, t, buf, got, bits, ref, bound):
-    """(ok, stats dict)."""
-    n = got.numel()
-    head, tail = buf[:GUARD], buf[GUARD + n:]
-    guard_ok = bool(torch.isnan(head).all()) and bool(torch.isnan(tail).all())
-    gd = got.double()
-    err = (gd - ref).abs()
-    finite = bool(torch.isfinite(gd).all())
-    ratio = float((err / bound.clamp(min=1e-300)).max()) if finite else float('inf')
-    ok = finite and guard_ok and bool((err <= bound).all())
-    bits_ok = True
-    if bits is not None:
-        bits_ok = torch.equal(bits.cpu(), _pack_bits(got.reshape(-1).cpu()))
-        ok = ok and bits_ok
-    return ok, dict(ratio=ratio, guard_ok=guard_ok, bits_ok=bits_ok, finite=finite,
-                    max_err=float(err.max()) if finite else float('inf'))
+def verdict(buf, got, bits, ref, bound):
+    """(ok, stats dict) of one launch's output `got` (inside the guarded `buf`) and its sign bits."""
+    cmp = compare(got, ref, bound)
+    guard_ok = guard_touched(buf, torch.arange(GUARD, GUARD + got.numel(), device=buf.device)) == 0
+    bits_ok = bits is None or torch.equal(bits.cpu(), pack_sign_bits(got.reshape(-1).cpu()))
+    return cmp['ok'] and guard_ok and bits_ok, dict(ratio=cmp['worst_ratio'], guard_ok=guard_ok, bits_ok=bits_ok,
+                                                    finite=cmp['nonfinite'] == 0)
+
+
+def _setup(case, device):
+    """The case's tensors, fp64 reference and bound, and its output: GUARD elements of NaN on each side of it in
+    `buf`, starting from the case's prev (or zero for a wgrad, which accumulates)."""
+    t = make_tensors(case, device)
+    ref, bound = reference(case, t)
+    n = 1
+    for s in t['out_shape']:
+        n *= s
+    buf = nan_buffer(n + 2 * GUARD, device)
+    out = buf[GUARD:GUARD + n].view(t['out_shape'])
+    if 'prev' in t:
+        out.copy_(t['prev'])
+    elif case['dir'] == 'wgrad':
+        out.zero_()
+    bits = torch.zeros(n // 32, dtype=torch.int32, device=device) if case['epi'].get('bits') else None
+    return t, ref, bound, buf, out, bits
 
 
 def run_case(case, device='cuda', keep_out=False):
     """Runs the case once; returns its stats (with keep_out, also 'out': the guarded output buffer and the sign bits as
     int32 bits, for a bitwise comparison of two runs)."""
-    t = make_tensors(case, device)
-    ref, bound = reference(case, t)
-    buf, out = _guarded(t['out_shape'], device, t.get('prev'))
-    if case['dir'] == 'wgrad' and not case['epi'].get('accum'):
-        out.zero_()
-    bits = torch.zeros(out.numel() // 32, dtype=torch.int32, device=device) if case['epi'].get('bits') else None
-    import gemm_paths as GP
+    t, ref, bound, buf, out, bits = _setup(case, device)
 
     def go():
         keep = launch(case, t, out, bits)
         torch.cuda.synchronize()
         return keep
-    _, text = GP.capture_fd2(go)
-    ok, st = compare(case, t, buf, out, bits, ref, bound)
-    rec = parse_record(text)
+    _, text = capture_fd2(go)
+    ok, st = verdict(buf, out, bits, ref, bound)
+    rec = next((r for r in (parse_record(l, 'gconv') for l in text.splitlines()) if r is not None), None)
     G = case['groups']
     want = dict(path='gconv', dir=case['dir'], groups=str(G), cig=str(case['C'] // G), cog=str(case['Co'] // G))
     st['record'] = rec
@@ -495,14 +478,6 @@ def run_case(case, device='cuda', keep_out=False):
     if keep_out:
         st['out'] = torch.cat([buf.view(torch.int32)] + ([bits] if bits is not None else [])).cpu()
     return st
-
-
-def parse_record(text):
-    for line in text.splitlines():
-        m = re.search(r'vlfb gconv:\s*(.*)$', line.strip())
-        if m:
-            return dict(tok.split('=', 1) for tok in m.group(1).split())
-    return None
 
 
 # ------------------------------------------------------------------------------------------------ CPU emulation
@@ -529,7 +504,7 @@ def emulate(case, t, buf, out, bits, plant=None):
         if e.get('bias'):
             v = v + t['bias']
     elif d == 'dgrad':
-        ws = w if not e.get('scale') else _rt(w * t['scale'].view(-1, 1, 1, 1, 1))
+        ws = w if not e.get('scale') else tf32_round(w * t['scale'].view(-1, 1, 1, 1, 1))
         xs = torch.zeros_like(x, requires_grad=True)
         F.conv3d(xs, ws, **conv).backward(dy)
         v = _cl(xs.grad) * float(e.get('alpha', 1.0))
@@ -554,7 +529,7 @@ def emulate(case, t, buf, out, bits, plant=None):
     if e.get('mask') and d != 'wgrad':
         v = torch.where(t['mask'] > 0, v, torch.zeros_like(v))
     if e.get('tf32'):
-        v = _rt(v.contiguous())
+        v = tf32_round(v.contiguous())
     if plant == 'missing_border_row':
         v = v.clone()
         v[:, :, -1] = 0
@@ -562,18 +537,13 @@ def emulate(case, t, buf, out, bits, plant=None):
     if plant == 'guard_write':
         buf[GUARD + out.numel()] = 0.0
     if bits is not None:
-        bits.copy_(_pack_bits(out.reshape(-1)))
+        bits.copy_(pack_sign_bits(out.reshape(-1)))
 
 
 def run_case_cpu(case, plant=None):
-    t = make_tensors(case, 'cpu')
-    ref, bound = reference(case, t)
-    buf, out = _guarded(t['out_shape'], 'cpu', t.get('prev'))
-    if case['dir'] == 'wgrad' and not case['epi'].get('accum'):
-        out.zero_()
-    bits = torch.zeros(out.numel() // 32, dtype=torch.int32) if case['epi'].get('bits') else None
+    t, ref, bound, buf, out, bits = _setup(case, 'cpu')
     emulate(case, t, buf, out, bits, plant)
-    return compare(case, t, buf, out, bits, ref, bound)
+    return verdict(buf, out, bits, ref, bound)
 
 
 def _by_name(name):
@@ -665,6 +635,7 @@ def main():
         for c in CASES:
             if args.only and not re.search(args.only, c['name']):
                 continue
+            print('[gconv_cases] %s' % c['name'], flush=True)
             st = run_case(c)
             st.update(name=c['name'], family=c['family'])
             f.write(json.dumps(st) + '\n')

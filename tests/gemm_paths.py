@@ -8,7 +8,9 @@ configuration runs in its own process:
     python tests/gemm_paths.py --config NAME --out FILE
 
 writes one JSON record per case that lists NAME among its configurations.  tests/test_gpu_gemm_paths.py drives it;
-tests/test_gemm_paths_cpu.py checks the table and the comparison itself without a GPU.
+tests/test_gemm_paths_cpu.py checks the table and the comparison itself without a GPU.  Besides the path cases, the
+default configuration runs the weight gradient at every production geometry of tests/wgrad_cases.py, the wide-tile
+forms and the conv1 column mask.
 
 Every output lives inside a NaN-filled buffer with a guard band (a lead-in, rows past M, ldd > N where the caller
 controls ldd, gaps between batches): after the call each in-range element must be finite and within the bound of
@@ -17,9 +19,7 @@ controls ldd, gaps between batches): after the call each in-range element must b
 import argparse
 import json
 import os
-import re
 import sys
-import tempfile
 
 import torch
 import torch.nn.functional as F
@@ -30,7 +30,9 @@ for _p in (os.path.join(ROOT, 'video-long-term-feature-banks_b200', 'lib'), HERE
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
-from util import tf32_round  # noqa: E402
+import wgrad_cases as WC  # noqa: E402
+from util import (capture_fd2, compare, guard_touched, nan_buffer, pack_sign_bits, parse_record,  # noqa: E402,F401
+                  tf32_round, ulp_tf32)
 
 # Tolerance of the accumulation, relative to sum_k |A[m,k]| |B[n,k]| (the operands are TF32-exact, so every product
 # is exact and only the fp32 additions err).  The wgmma accumulator adds each k8 step to the running fp32 sum with at
@@ -40,7 +42,9 @@ from util import tf32_round  # noqa: E402
 # tile shifts an element by ~sqrt(32) times a typical |A||B| term, far above tau(K) sum |A||B| (test_gemm_paths_cpu.py
 # shows the check rejects it at the largest K of the table).
 TAU_SAFETY = 4.0
-KMAX = 16000                   # the table's K stays in the range the worker's fp64 references handle quickly
+# The table's K stays in the range the worker's fp64 references handle quickly, and where the suite's global relative
+# check holds; only the weight gradients marked long_k (the production geometries, K = N To Ho Wo) go beyond it.
+KMAX = 16000
 
 
 def tau(K):
@@ -48,7 +52,6 @@ def tau(K):
 
 # the fp32 epilogue (scale, bias, residual, accumulate) rounds a few times: 2^-22 of the magnitudes it adds
 EPS32 = 2.0 ** -22
-NAN_BITS = 0x7FC00000          # torch.full(..., nan) fills this pattern
 GUARD = 64                     # lead-in guard floats (keeps d 16-byte aligned)
 
 CONFIGS = {
@@ -58,29 +61,11 @@ CONFIGS = {
     'nopatch': {'VLFB_NO_PATCH': '1'},
     'nopar': {'VLFB_NO_PAR': '1'},
 }
-# every environment override of the GEMM (a configuration sets some of them; the rest must be unset)
-SWITCHES = ('VLFB_TMA', 'VLFB_IM2COL', 'VLFB_NO_PATCH', 'VLFB_NO_PAR', 'VLFB_BN', 'VLFB_STAGES', 'VLFB_LAG', 'VLFB_SK',
-            'VLFB_DEBUG')
 
 OP_DENSE_K, OP_DENSE_MN, OP_CONV_K, OP_DGRAD_K, OP_CONV_MN, OP_STEM_K, OP_STEM_MN = range(7)
 
 
 # ----------------------------------------------------------------------------------------------- path records
-def parse_record(line):
-    """One VLFB_DEBUG line of gemm_tc launch() -> dict (None if the line is not one).  Values are ints; 'kinds' and
-    'tma' are (a, b) tuples."""
-    m = re.search(r'vlfb gemm_tc:\s*(.*)$', line.strip())
-    if not m:
-        return None
-    rec = {}
-    for tok in m.group(1).split():
-        if '=' not in tok:
-            continue
-        k, v = tok.split('=', 1)
-        rec[k] = tuple(int(x) for x in v.split(',')) if ',' in v else int(v)
-    return rec
-
-
 def matches(rec, expect):
     """Fields of `expect` that the record contradicts ([] = it took the declared path).  An expected value '>N'
     means greater than N."""
@@ -264,6 +249,81 @@ _add('raw_split0_stored_residual_tf32_simt', 'raw', 34, Z=1, M=200, N=96, K=4096
      split_k=0, engine='simt', epi=dict(residual=True, tf32=True),
      runs={'default': {}})
 
+
+# ---- weight gradients at every production geometry of R50-I3D-NL at 2 clips (tests/wgrad_cases.py) and at small ragged
+# ones: K (positions) not a multiple of 64, Co = 4, 32, 64 and 68, N tails, stream-K / split-K of each operand form.
+# These launches stage both operands by cp.async and publish each chunk by the completion of its copies
+# (cp.async.mbarrier.arrive), so the producers run ahead of the MMAs by the whole ring.  A case with Co <= 64 runs
+# 64 x 2bn wide tiles, warpgroup w computing columns [w bn, (w + 1) bn) of the 64 rows (csrc/gemm_tc.cu, Launch::wide).
+def _wgrad(name, seed, shape, co, ker, st=(1, 1, 1), pd=(0, 0, 0), dil=(1, 1, 1), opts=None, epi=None, long_k=False,
+           col_mask=False, **expect):
+    """A conv_wgrad case run under the default configuration only (check_case compares the record's kinds with
+    describe() for every case).  long_k: K = N To Ho Wo may exceed KMAX.  col_mask: conv1 with the optimiser's 32-lane
+    column mask."""
+    n, t, h, w, c = shape
+    run = dict(tma=(0, 0), cp=1)
+    if c == 4:
+        run['patch'] = 0
+    run.update(expect)
+    _add(name, 'conv_wgrad', seed, {'default': run}, opts=opts or {}, epi=epi or {}, long_k=long_k, col_mask=col_mask,
+         geom=G(n, t, h, w, c, co, tuple(ker), st=tuple(st), pd=tuple(pd), dil=tuple(dil)))
+
+
+_RS = dict(row_scale=True)
+for _i, (_label, _shape, _co, _ker, _st, _pd, _dil, _) in enumerate(WC.PRODUCTION):
+    _wgrad('wgrad prod ' + _label, 500 + _i, _shape, _co, _ker, _st, _pd, _dil, long_k=True)
+_wgrad('wgrad ragged M=4 3x3', 601, (1, 2, 6, 6, 32), 4, (1, 3, 3), pd=(0, 1, 1))
+_wgrad('wgrad ragged M=32 3x3 N tail', 602, (2, 3, 5, 7, 64), 32, (1, 3, 3), pd=(0, 1, 1))
+_wgrad('wgrad ragged M=64 3x1x1', 603, (1, 3, 10, 10, 32), 64, (3, 1, 1), pd=(1, 0, 0))
+_wgrad('wgrad ragged M=68 1x1', 604, (2, 2, 9, 9, 64), 68, (1, 1, 1))
+_wgrad('wgrad ragged M=68 3x3 N tail', 605, (1, 3, 7, 9, 32), 68, (1, 3, 3), pd=(0, 1, 1))
+_wgrad('wgrad ragged stem 5x7x7', 606, (1, 3, 20, 20, 4), 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3))
+# stream-K (atomic, no fix-up) of each operand form
+_wgrad('wgrad stream-K 3x3', 611, (2, 8, 14, 14, 128), 128, (1, 3, 3), pd=(0, 1, 1), opts=dict(stream_k=1), sk=1, fix=0)
+_wgrad('wgrad stream-K 1x1', 612, (2, 16, 14, 14, 256), 128, (1, 1, 1), opts=dict(stream_k=1), sk=1, fix=0)
+_wgrad('wgrad stream-K stem', 613, (1, 4, 36, 64, 4), 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3), opts=dict(stream_k=1),
+       sk=1, fix=0)
+# wide tiles: every Co = 64 production geometry, and one Co = 128 that stays narrow
+for _i, (_label, _shape, _co, _ker, _st, _pd, _dil, _) in enumerate(WC.PRODUCTION):
+    if _co <= 64 or _label == 'res3_x_2b 1x3x3 128->128':
+        _wgrad('wide prod ' + _label, 700 + _i, _shape, _co, _ker, _st, _pd, _dil, long_k=True, wide=int(_co <= 64))
+# M against the 64-row wide tile (Co % 4 == 0: 16-byte dY rows)
+_wgrad('wide M=4 3x3', 801, (1, 2, 6, 6, 32), 4, (1, 3, 3), pd=(0, 1, 1), epi=_RS, wide=1)
+_wgrad('wide M=32 3x3', 802, (2, 3, 5, 7, 64), 32, (1, 3, 3), pd=(0, 1, 1), wide=1)
+_wgrad('wide M=60 3x1x1 N=32', 803, (1, 3, 8, 8, 32), 60, (3, 1, 1), pd=(1, 0, 0), epi=_RS, wide=1)
+_wgrad('wide M=64 1x1', 804, (2, 2, 9, 9, 64), 64, (1, 1, 1), wide=1)
+_wgrad('wide M=68 3x3', 805, (1, 3, 7, 9, 32), 68, (1, 3, 3), pd=(0, 1, 1), wide=0)
+# N tails against bn and 2 bn, with the tile width forced
+_wgrad('wide N=96 <= bn=128 1x1', 811, (2, 2, 8, 8, 96), 64, (1, 1, 1), opts=dict(tile_n=128), epi=_RS, wide=1, bn=128)
+_wgrad('wide bn=64 < N=108 < 128 3x3', 812, (1, 3, 6, 6, 12), 48, (1, 3, 3), pd=(0, 1, 1), opts=dict(tile_n=64), wide=1,
+       bn=64)
+_wgrad('wide N=144 = 2 x 64 + 16, bn=32 1x1', 813, (1, 4, 6, 6, 144), 64, (1, 1, 1), opts=dict(tile_n=32), epi=_RS,
+       wide=1, bn=32)
+_wgrad('wide N=144 = 128 + 16, bn=64 3x3', 814, (1, 3, 6, 6, 16), 64, (1, 3, 3), pd=(0, 1, 1), opts=dict(tile_n=64),
+       wide=1, bn=64)
+_wgrad('wide N=224 bn=128 stem', 815, (1, 3, 20, 20, 4), 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3),
+       opts=dict(tile_n=128), wide=1, bn=128)
+# split-K (few wide tiles, long K) and stream-K (atomic, no fix-up) for each B operand kind
+_wgrad('wide split-K CONV_MN', 821, (2, 8, 14, 14, 64), 64, (1, 3, 3), pd=(0, 1, 1), epi=_RS, wide=1, split='>1', sk=0)
+_wgrad('wide split-K STEM_MN', 822, (1, 4, 36, 64, 4), 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3), wide=1, split='>1',
+       sk=0)
+_wgrad('wide split-K DENSE_MN', 823, (2, 8, 14, 14, 64), 64, (1, 1, 1), wide=1, split='>1', sk=0)
+_wgrad('wide stream-K CONV_MN', 831, (2, 8, 14, 14, 64), 64, (1, 3, 3), pd=(0, 1, 1), opts=dict(stream_k=1), wide=1,
+       sk=1, fix=0)
+_wgrad('wide stream-K STEM_MN', 832, (1, 4, 36, 64, 4), 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3),
+       opts=dict(stream_k=1), epi=_RS, wide=1, sk=1, fix=0)
+_wgrad('wide stream-K DENSE_MN', 833, (2, 16, 28, 28, 64), 64, (1, 1, 1), opts=dict(stream_k=1), long_k=True, wide=1,
+       sk=1, fix=0)
+# conv1 with the optimiser's column mask (padding lanes px >= kW and the fourth channel zeroed) and a row scale
+_wgrad('wide stem col_mask', 841, (1, 4, 36, 64, 4), 64, (5, 7, 7), st=(1, 2, 2), pd=(2, 3, 3), epi=_RS, col_mask=True,
+       wide=1)
+# transposed x transposed matmul, M <= 64, plain stores with ACCUM (read-modify-write of D by exactly one warp: no
+# reduction across warpgroups)
+_add('wide raw MNxMN M=48 accum', 'raw', 851, Z=2, M=48, N=200, K=300, a_mn=True, b_mn=True, gn=4, gm=2,
+     epi=dict(accum=True, scale=True, bias=True, row_scale=True),
+     runs={'default': dict(kinds=(OP_DENSE_MN, OP_DENSE_MN), tma=(0, 0), cp=1, wide=1, sk=0, split=1)})
+
+
 def case_by_name(name):
     return next(c for c in CASES if c['name'] == name)
 
@@ -401,12 +461,6 @@ def engine(c):
 
 
 # ----------------------------------------------------------------------------------------------- comparison
-def ulp_tf32(x):
-    """One TF32 ulp (10 explicit mantissa bits) of |x|, elementwise; 0 at 0."""
-    m, e = torch.frexp(x.abs())
-    return torch.where(x == 0, torch.zeros_like(x), torch.ldexp(torch.ones_like(x), e - 11))
-
-
 def finish(acc, mag, epi, K):
     """fp64 epilogue of vlfb_gemm (common.cuh epilogue_store, element by element) and the error bound of each element.
     acc / mag: [Z, M, N] sum_k A B and sum_k |A| |B| over the call's K; epi: alpha, cs [N], cb [N], rs [M],
@@ -437,39 +491,6 @@ def finish(acc, mag, epi, K):
         v = v + after
         bound = bound + EPS32 * after.abs()
     return v, bound.expand_as(v)
-
-
-def compare(d, ref, bound):
-    """Elementwise check: d finite and |d - ref| <= bound everywhere; plus the suite's global max|d-ref| / max|ref| <
-    2e-5 (looser where the result is stored TF32-rounded).  Returns a dict: ok, worst ratio |d-ref|/bound, where, and
-    the global relative error."""
-    d = d.double()
-    diff = (d - ref).abs()
-    finite = torch.isfinite(d)
-    ratio = torch.where(finite, diff / bound.clamp(min=1e-300), torch.full_like(diff, float('inf')))
-    ratio = torch.where(diff == 0, torch.zeros_like(ratio), ratio)
-    worst = int(ratio.reshape(-1).argmax())
-    rel = float(diff[finite].max() / (ref.abs().max() + 1e-30)) if bool(finite.any()) else float('inf')
-    nbad = int((ratio > 1).sum())
-    at = [int(i) for i in torch.unravel_index(torch.tensor(worst), tuple(ref.shape))]
-    return dict(ok=nbad == 0 and bool(finite.all()), nbad=nbad, nonfinite=int((~finite).sum()),
-                worst_ratio=float(ratio.reshape(-1)[worst]), worst_at=at, rel_err=rel)
-
-
-def guard_intact(buf, index):
-    """Every element of the fp32 buffer `buf` outside the flat offsets `index` still holds the NaN fill, bit for bit.
-    Returns the number of touched guard elements."""
-    bits = buf.reshape(-1).view(torch.int32)
-    guard = torch.ones(bits.numel(), dtype=torch.bool, device=buf.device)
-    guard[index.reshape(-1)] = False
-    return int((bits[guard] != NAN_BITS).sum())
-
-
-def pack_sign_bits(x):
-    """bit e & 31 of word e >> 5 = x.flat[e] > 0 (vlfb_gemm_params_t.relu_bits_out / relu_mask_bits)."""
-    b = (x.reshape(-1, 32) > 0).to(torch.int64)
-    v = (b << torch.arange(32, dtype=torch.int64, device=x.device)).sum(1)
-    return torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32)
 
 
 # ----------------------------------------------------------------------------------------------- case inputs / references
@@ -521,6 +542,15 @@ def conv_refs(c, x, w, dy, dev):
             r = r.reshape(kT, g['Co'], -1)
         res.append(r.detach())
     return res[0], res[1]
+
+
+def _col_mask(kH):
+    """conv1's column mask over the kH x 32 lanes of a wgrad row: lane px * 4 + ch is real when px < kW (7) and
+    ch < 3.  conv_wgrad takes the first 32 lanes and repeats them."""
+    m = torch.zeros(32)
+    for px in range(7):
+        m[px * 4:px * 4 + 3] = 1
+    return m.repeat(kH)
 
 
 class Prepared:
@@ -578,6 +608,8 @@ def prepare(c, dev):
     epi = dict(alpha=e.get('alpha', 1.0), relu=e.get('relu', False), tf32=e.get('tf32', False))
     if e.get('scale'):
         epi['cs'] = (torch.rand(N, generator=gen) + 0.5).double()
+    if c.get('col_mask'):
+        epi['cs'] = _col_mask(c['geom']['ker'][1]).double()
     if e.get('bias'):
         epi['cb'] = (torch.randn(N, generator=gen) * e.get('bias_scale', 1.0)).double()
     if e.get('row_scale'):
@@ -629,7 +661,7 @@ def run_case(K, P, dev):
     c = P.case
     e = c.get('epi', {})
     Z, M, N = P.ref.shape
-    buf = torch.full((P.layout['size'],), float('nan'), device=dev)
+    buf = nan_buffer(P.layout['size'], dev)
     flat = buf.view(-1)
     if 'prev' in P.epi:
         flat[P.index.reshape(-1)] = P.epi['prev'].reshape(-1).float()
@@ -679,7 +711,8 @@ def run_case(K, P, dev):
                 x = _stem_input(K, P, dev) if g['C'] == 4 else _to_cl(P.x).to(dev)
                 dw = out.view((g['Co'],) + tuple(g['ker'][:2]) + (8 if g['C'] == 4 else g['ker'][2], g['C']))
                 wgrad = K.conv_wgrad_det if c.get('deterministic') else K.conv_wgrad
-                wgrad(_to_cl(P.dy).to(dev), x, dw, geo, row_scale=rs)
+                mask = P.epi['cs'][:32].float() if c.get('col_mask') else None
+                wgrad(_to_cl(P.dy).to(dev), x, dw, geo, row_scale=rs, col_mask=mask)
         elif c['op'] == 'matmul':
             A = P.A.to(dev)
             if c.get('b_weight'):
@@ -779,24 +812,6 @@ def _run_raw(K, L, ctypes, P, flat, cs, cb, rs, dev):
     return bits
 
 
-def capture_fd2(fn):
-    """Runs fn() with file descriptor 2 redirected to a temporary file (the library writes its VLFB_DEBUG records with
-    fprintf(stderr)); returns (fn's result, the captured text)."""
-    sys.stderr.flush()
-    with tempfile.TemporaryFile() as tmp:
-        saved = os.dup(2)
-        os.dup2(tmp.fileno(), 2)
-        try:
-            out = fn()
-        finally:
-            sys.stderr.flush()
-            os.dup2(saved, 2)
-            os.close(saved)
-        tmp.seek(0)
-        text = tmp.read().decode('utf-8', 'replace')
-    return out, text
-
-
 def check_case(K, c, config, dev, declared=True):
     """Runs one case under the current process's configuration; returns its JSON record.  The launch must take the
     engine abi_errors / engine() predict (one gemm_tc record, or none on the SIMT engine) and, with `declared`, the
@@ -839,9 +854,11 @@ def check_case(K, c, config, dev, declared=True):
         # a drawn call may sum up to KMAX products, most of them zero taps: its rounding grows like sqrt(K) against the
         # largest output (the elementwise bound above stays the rigorous check)
         tol *= max(1.0, (P.K / 2048.0) ** 0.5)
-    if not cmp['rel_err'] < tol:
+    # beyond KMAX the fp32 accumulation error of a K-long sum grows with K: the elementwise bound above is the check
+    # that scales
+    if P.K <= KMAX and not cmp['rel_err'] < tol:
         rec['errors'].append('global rel_err %.3g >= %g' % (cmp['rel_err'], tol))
-    touched = guard_intact(buf, P.index)
+    touched = guard_touched(buf, P.index)
     if touched:
         rec['errors'].append('%d guard elements overwritten' % touched)
     if bits is not None:
@@ -883,6 +900,7 @@ def main(argv=None):
                 rec = dict(case=c['name'], config=args.config, ok=False, paths=[], errors=['%s: %s' % (type(ex).__name__, ex)])
             f.write(json.dumps(rec) + '\n')
             f.flush()
+            torch.cuda.empty_cache()
     print('[gemm_paths] config=%s done' % args.config, flush=True)
 
 

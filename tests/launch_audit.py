@@ -41,6 +41,7 @@ import gconv_cases as GC  # noqa: E402
 import gemm_paths as GP  # noqa: E402
 import streaming_cases as SC  # noqa: E402
 from streaming_cases import U, C_SUM, sum_bound  # noqa: E402
+from util import capture_fd2, compare, pack_sign_bits, parse_record, tf32_round  # noqa: E402
 
 GEMM_WRAPPERS = ('conv_fwd', 'conv_dgrad', 'conv_wgrad', 'conv_wgrad_det', 'matmul', 'matmul_det')
 DET_WRAPPERS = ('colsum_det', 'spatial_bn_fwd_det', 'spatial_bn_bwd_det', 'roi_align_bwd_det')
@@ -67,12 +68,6 @@ class NoReference(Exception):
 # ----------------------------------------------------------------------------------------------- small helpers
 def _bits(t):
     return t.contiguous().view({4: torch.int32, 8: torch.int64, 2: torch.int16, 1: torch.uint8}[t.element_size()])
-
-
-def tf32_rna(t):
-    """cvt.rna.tf32.f32 of the fp32 value of t, returned in t's dtype (the CPU stand-in runs in fp64)."""
-    i = t.float().contiguous().view(torch.int32)
-    return ((i + 0x1000) & ~0x1FFF).view(torch.float32).to(t.dtype).view(t.shape)
 
 
 def tf32_trunc(t):
@@ -270,7 +265,7 @@ def _conv_fwd(c):
 def _with_bits(c, out):
     if c.b['relu_bits'] is not None:
         bits = c.a['relu_bits']
-        out.append(('relu_bits', bits, SC.pack_sign_bits(c.a['y'].reshape(-1)).view(bits.shape), None))
+        out.append(('relu_bits', bits, pack_sign_bits(c.a['y'].reshape(-1)).view(bits.shape), None))
     return out
 
 
@@ -363,7 +358,7 @@ def _wt_ref(w, s):
     w3 = w.reshape(co, -1, ci)
     if s is not None:
         w3 = w3 * s.view(-1, 1, 1)             # one rounding in the tensors' dtype, as the kernel's product
-    return tf32_rna(w3.permute(2, 1, 0).contiguous())
+    return tf32_round(w3.permute(2, 1, 0).contiguous())
 
 
 @ref('weight_transpose_multi')
@@ -389,17 +384,17 @@ def _fill(c):
 
 @ref('round_tf32')
 def _round_tf32(c):
-    return [('y', c.a['y'], tf32_rna(c.b['x']).view(c.a['y'].shape), None)]
+    return [('y', c.a['y'], tf32_round(c.b['x']).view(c.a['y'].shape), None)]
 
 
 @ref('add_tf32')
 def _add_tf32(c):
-    return [('out', c.a['out'], tf32_rna(c.b['x'] + c.b['y']).view(c.a['out'].shape), None)]
+    return [('out', c.a['out'], tf32_round(c.b['x'] + c.b['y']).view(c.a['out'].shape), None)]
 
 
 @ref('relu_tf32')
 def _relu_tf32(c):
-    return [('y', c.a['y'], tf32_rna(c.b['x'].clamp(min=0)).view(c.a['y'].shape), None)]
+    return [('y', c.a['y'], tf32_round(c.b['x'].clamp(min=0)).view(c.a['y'].shape), None)]
 
 
 @ref('relu_fwd')
@@ -418,12 +413,12 @@ def _relu_bwd(c):
 
 @ref('relu_bwd_tf32')
 def _relu_bwd_tf32(c):
-    return [('dx', c.a['dx'], _where_pos(c.b['y'], tf32_rna(c.b['dy'])).view(c.a['dx'].shape), None)]
+    return [('dx', c.a['dx'], _where_pos(c.b['y'], tf32_round(c.b['dy'])).view(c.a['dx'].shape), None)]
 
 
 @ref('add_relu_bwd_tf32')
 def _add_relu_bwd_tf32(c):
-    s = tf32_rna(c.b['a'] + c.b['b'])
+    s = tf32_round(c.b['a'] + c.b['b'])
     if c.b['y'] is not None:
         s = _where_pos(c.b['y'], s)
     return [('out', c.a['out'], s.view(c.a['out'].shape), None)]
@@ -431,7 +426,7 @@ def _add_relu_bwd_tf32(c):
 
 @ref('relu_bits')
 def _relu_bits(c):
-    return [('bits', c.a['bits'], SC.pack_sign_bits(c.b['x'].reshape(-1)).view(c.a['bits'].shape), None)]
+    return [('bits', c.a['bits'], pack_sign_bits(c.b['x'].reshape(-1)).view(c.a['bits'].shape), None)]
 
 
 @ref('sigmoid_fwd')
@@ -496,7 +491,7 @@ def _nc_to_cl(c):
     v = torch.zeros((n, inner, cpad), dtype=b['src'].dtype, device=b['src'].device)
     v[:, :, :C_] = b['src'].reshape(n, C_, inner).permute(0, 2, 1)
     if b['tf32_out']:
-        v = tf32_rna(v)
+        v = tf32_round(v)
     dst = a['dst']
     pitch = int(b.get('pitch', 0) or 0)
     if pitch:
@@ -661,7 +656,7 @@ def _sgd(c):
     out = [(k, a[k], *r[k]) for k in ('p', 'g', 'm')]
     if b['p_tf32'] is not None:
         # exactly the TF32 rounding of the stored p
-        out.append(('p_tf32', a['p_tf32'], tf32_rna(a['p']), None))
+        out.append(('p_tf32', a['p_tf32'], tf32_round(a['p']), None))
     return out
 
 
@@ -728,7 +723,7 @@ def _lfb_gather(c):
     r = torch.where(ok.view(-1, 1), rows[i.clamp(0, rows.shape[0] - 1)], torch.zeros((), dtype=rows.dtype,
                                                                                      device=rows.device))
     if b['tf32_out']:
-        r = tf32_rna(r)
+        r = tf32_round(r)
     return [('out', a['out'], r.view(a['out'].shape), None)]
 
 
@@ -827,32 +822,6 @@ def _roi_table(c):
     raise NoReference('roi_align_table (the executor does not call it)')
 
 
-# ----------------------------------------------------------------------------------------------- comparison
-def compare(got, r, bound):
-    """(number of elements outside the bound, number not finite, worst |got - ref| / bound, index of the worst)."""
-    if bound is None:
-        if got.dtype.is_floating_point:
-            same = _bits(got.to(got.dtype)) == _bits(r.to(got.dtype).reshape(got.shape))
-            # -0.0 and +0.0 are the same value
-            same = same | ((got == 0) & (r.to(got.dtype).reshape(got.shape) == 0))
-        else:
-            same = got == r.to(got.dtype).reshape(got.shape)
-        bad = ~same
-        nf = int((~torch.isfinite(got)).sum()) if got.dtype.is_floating_point else 0
-        nbad = int(bad.sum())
-        at = int(bad.reshape(-1).nonzero()[0]) if nbad else -1
-        return nbad, nf, (float('inf') if nbad else 0.0), at
-    g = got.double().reshape(r.shape)
-    diff = (g - r).abs()
-    fin = torch.isfinite(g)
-    ratio = torch.where(diff == 0, torch.zeros_like(diff), diff / bound.clamp(min=1e-300))
-    ratio = torch.where(fin, ratio, torch.full_like(ratio, float('inf')))
-    if ratio.numel() == 0:
-        return 0, 0, 0.0, -1
-    worst = int(ratio.reshape(-1).argmax())
-    return int((ratio > 1).sum()), int((~fin).sum()), float(ratio.reshape(-1)[worst]), worst
-
-
 # ----------------------------------------------------------------------------------------------- the interposer
 def _wrapper_signature(name):
     from vlfb import kernels
@@ -923,10 +892,10 @@ class Audit:
         snaps = self._snapshots(name, a)
         text = ''
         if name in GEMM_WRAPPERS and os.environ.get('VLFB_DEBUG') and not self.engine.startswith('fake'):
-            ret, text = GP.capture_fd2(lambda: self._run(f, args, kwargs))
+            ret, text = capture_fd2(lambda: self._run(f, args, kwargs))
             rec['paths'] = [dict((k, list(v) if isinstance(v, tuple) else v) for k, v in r.items())
-                            for r in (GP.parse_record(l) for l in text.splitlines()) if r is not None]
-            rec['paths'] += [dict(r, path='gconv') for r in (GC.parse_record(l) for l in text.splitlines())
+                            for r in (parse_record(l) for l in text.splitlines()) if r is not None]
+            rec['paths'] += [dict(r, path='gconv') for r in (parse_record(l, 'gconv') for l in text.splitlines())
                              if r is not None]
         else:
             ret = self._run(f, args, kwargs)
@@ -990,13 +959,17 @@ class Audit:
         results = REF[name](c)
         written = {}
         for oname, got, r, bnd in results:
-            nbad, nf, worst, at = compare(got, r, bnd)
-            rec['outputs'][oname] = dict(worst=worst if bnd is not None or nbad else 0.0, exact=bnd is None)
-            if nbad or nf:
+            if bnd is None and got.dtype.is_floating_point:          # -0.0 and +0.0 are the same value
+                r = r.reshape(got.shape)
+                r = torch.where((got == 0) & (r == 0), got.to(r.dtype), r)
+            cmp = compare(got, r, bnd)
+            rec['outputs'][oname] = dict(worst=cmp['worst_ratio'], exact=bnd is None)
+            if not cmp['ok']:
+                at = int(np.ravel_multi_index(cmp['worst_at'], r.shape)) if cmp['worst_at'] else -1
                 g, rr = got.reshape(-1)[at] if at >= 0 else None, r.reshape(-1)[at] if at >= 0 else None
                 rec['errors'].append('%s: %s: %d elements outside the bound (%d not finite), worst %.3g x bound at flat '
-                                     '%d (got %r, ref %r)' % (self._where(rec), oname, nbad, nf, worst, at,
-                                                             None if g is None else float(g),
+                                     '%d (got %r, ref %r)' % (self._where(rec), oname, cmp['nbad'], cmp['nonfinite'],
+                                                             cmp['worst_ratio'], at, None if g is None else float(g),
                                                              None if rr is None else float(rr)))
             key = (got.untyped_storage().data_ptr(), got.dtype)
             written.setdefault(key, []).append(_offsets(got).reshape(-1))
@@ -1122,6 +1095,7 @@ def run_net(audit, name, runs=None, rois_per_clip=2, seed=2):
             workspace.RunNet(model.net.Proto().name)
             audit.install()
         for r in range(runs):
+            print('[launch_audit] net=%s run=%d' % (name, r + 1), flush=True)
             audit.run = r + 1
             workspace.RunNet(model.net.Proto().name)
     finally:

@@ -85,7 +85,7 @@ def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_
     y.copy_(FK._q(o, tf32_out))
     if relu_bits is not None:
         assert relu
-        FK._pack_bits(y, relu_bits)
+        relu_bits.copy_(FK.pack_sign_bits(y))
 
 
 def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, tf32_out=False, relu_mask_bits=None,

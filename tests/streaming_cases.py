@@ -32,6 +32,8 @@ for _p in (os.path.join(ROOT, 'video-long-term-feature-banks_b200', 'lib'), HERE
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from util import BITS, compare, guard_touched, nan_buffer, pack_sign_bits, tf32_round, ulp_tf32  # noqa: E402,F401
+
 # ----------------------------------------------------------------------------------------------- launch signatures
 # The wrappers of vlfb.kernels that launch a streaming kernel (the GEMM wrappers conv_fwd / conv_dgrad / conv_wgrad /
 # matmul are tests/gemm_paths.py's).
@@ -99,7 +101,6 @@ U = 2.0 ** -24
 C_SUM = 2.0
 C_EXP = 2.0
 C_ARG = 2.0
-NAN_BITS = 0x7FC00000          # torch.full(..., nan) fills this pattern; int32 outputs are filled with the same bits
 GUARD = 64                     # lead-in guard elements (keeps an unshifted output 16-byte aligned)
 TAIL = 64
 # stream_grid (common.cuh) caps a grid at 132 * 16 blocks: above CAP_ITEMS work items of 256-thread blocks (one item per
@@ -119,28 +120,10 @@ def geom(N, T_, H, W, C, ker, st, pd):
                 sH=st[1], sW=st[2], pT=pd[0], pH=pd[1], pW=pd[2], dT=1, dH=1, dW=1)
 
 
-def tf32_round(t):
-    """cvt.rna.tf32.f32 (round to nearest, ties away) of an fp32 tensor."""
-    i = t.contiguous().view(torch.int32)
-    return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
-
-
-def ulp_tf32(x):
-    """One TF32 ulp (10 explicit mantissa bits) of |x|, elementwise; 0 at 0."""
-    _, e = torch.frexp(x.abs())
-    return torch.where(x == 0, torch.zeros_like(x), torch.ldexp(torch.ones_like(x), e - 11))
-
-
 def bf16_rne(t):
     """fp32 -> bf16 bits (round to nearest even) as int32, the rule of vlfb_cast_f32_to_bf16."""
     i = t.contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
     return ((i + 0x7FFF + ((i >> 16) & 1)) >> 16).to(torch.int32)
-
-
-def pack_sign_bits(x):
-    b = (x.reshape(-1, 32) > 0).to(torch.int64)
-    v = (b << torch.arange(32, dtype=torch.int64, device=x.device)).sum(1)
-    return torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32)
 
 
 # ----------------------------------------------------------------------------------------------- Philox4x32-10 (numpy)
@@ -187,12 +170,6 @@ class Prepared:
         self.keep = []
 
 
-def _buffer(n, dev, dtype=torch.float32, lead=GUARD, tail=TAIL):
-    if dtype in (torch.float32, torch.bfloat16):
-        return torch.full((lead + n + tail,), float('nan'), dtype=dtype, device=dev)
-    return torch.full((lead + n + tail,), NAN_BITS, dtype=dtype, device=dev)
-
-
 # The global check of the older suite, max|got - ref| / max|ref| < tol, kept beside the elementwise bound: TOL unless a
 # case states its own (the TF32-rounded outputs: one TF32 ulp, 6e-4).
 TOL = 1e-4
@@ -201,7 +178,7 @@ TOL = 1e-4
 def place(P, name, shape, ref, bound=None, dtype=torch.float32, off=0, prev=None, tol=None):
     """A contiguous output of `shape` at GUARD + off of a NaN buffer; `prev` = its finite starting contents."""
     n = int(np.prod(shape)) if len(shape) else 1
-    buf = _buffer(n + off, P.dev, dtype)
+    buf = nan_buffer(GUARD + n + off + TAIL, P.dev, dtype)
     index = torch.arange(n, device=P.dev).view(shape) + GUARD + off
     if prev is not None:
         buf[index.reshape(-1)] = prev.reshape(-1).to(dtype)
@@ -583,7 +560,7 @@ def _ew(P, gen):
     alias = c.get('alias')
     if alias:                   # out is one of the inputs: its buffer is that input's
         n = int(np.prod(shape))
-        buf = _buffer(n + off, P.dev)
+        buf = nan_buffer(GUARD + n + off + TAIL, P.dev)
         index = torch.arange(n, device=P.dev).view(shape) + GUARD + off
         buf[index.reshape(-1)] = X[alias].reshape(-1).to(P.dev)
         T_ = {alias: buf[GUARD + off:GUARD + off + n].view(shape)}
@@ -636,7 +613,7 @@ def _copy2d(P, gen):
     sidx = so + r_ * lds + c_
     didx = GUARD + do + r_ * ldd + c_
     v = src.reshape(-1)[sidx]
-    buf = _buffer(nd, P.dev)
+    buf = nan_buffer(GUARD + nd + TAIL, P.dev)
     if a['accumulate']:
         prev = randn((rows, cols), gen)
         buf[didx.reshape(-1).to(P.dev)] = prev.reshape(-1).to(P.dev)
@@ -678,7 +655,7 @@ def _layout(P, gen):
             index = (base.view(-1, 1) + torch.arange(cpad).view(1, -1)).view(n, inner, cpad)
         else:
             index = GUARD + torch.arange(n * inner * cpad).view(n, inner, cpad)
-        buf = _buffer(nd, P.dev)
+        buf = nan_buffer(GUARD + nd + TAIL, P.dev)
         add_out(P, 'dst', buf, index.to(P.dev), v.to(P.dev))
         dst = buf[GUARD:GUARD + nd].view(a['dst']['shape'])
         sd = inp(P, src.view(a['src']['shape']))
@@ -1113,7 +1090,7 @@ def _sgd(P, gen):
     pd, gd, md = p.double().to(P.dev), g.double().to(P.dev), m.double().to(P.dev)
     r = sgd_ref(pd, gd, md, lr, mu, wd, a['nesterov'])
     (p2, ep), (st, es), (m2, em) = r['p'], r['g'], r['m']
-    pb, gb, mb = (_buffer(int(np.prod(n)), P.dev) for _ in range(3))
+    pb, gb, mb = (nan_buffer(GUARD + int(np.prod(n)) + TAIL, P.dev) for _ in range(3))
     idx = torch.arange(int(np.prod(n)), device=P.dev).view(n) + GUARD
     for b_, v in ((pb, p), (gb, g), (mb, m)):
         b_[idx.reshape(-1)] = v.reshape(-1).to(P.dev)
@@ -1731,40 +1708,6 @@ def prepare(c, dev):
     return P
 
 
-_BITS = {torch.float32: torch.int32, torch.bfloat16: torch.int16}
-
-
-def compare(got, ref, bound, tol=None, tol_rows=None):
-    """Elementwise: bit-exact (bound None) or finite and |got - ref| <= bound; plus the global max|got - ref| /
-    max|ref| < tol.  Returns a dict: ok, nbad, worst ratio |got - ref| / bound, rel_err."""
-    if bound is None:
-        g, r = got.contiguous(), ref.to(got.dtype).contiguous()
-        if g.dtype in _BITS:
-            g, r = g.view(_BITS[g.dtype]), r.view(_BITS[g.dtype])
-        nbad = int((g != r).sum())
-        return dict(ok=nbad == 0, nbad=nbad, worst_ratio=0.0 if nbad == 0 else float('inf'), rel_err=0.0)
-    d = got.double()
-    diff = (d - ref).abs()
-    finite = torch.isfinite(d)
-    ratio = torch.where(finite, diff / bound.clamp(min=1e-300), torch.full_like(diff, float('inf')))
-    ratio = torch.where(diff == 0, torch.zeros_like(ratio), ratio)
-    nbad = int((ratio > 1).sum())
-    sel = finite if tol_rows is None else finite & tol_rows
-    rel = float(diff[sel].max() / (ref[sel].abs().max() + 1e-30)) if bool(sel.any()) else 0.0
-    ok = nbad == 0 and bool(finite.all()) and (tol is None or rel < tol)
-    return dict(ok=ok, nbad=nbad, worst_ratio=float(ratio.max()) if ratio.numel() else 0.0, rel_err=rel)
-
-
-def guard_touched(buf, index):
-    """Elements of the buffer outside `index` that no longer hold the NaN fill bits."""
-    bits = buf.view(_BITS[buf.dtype]) if buf.dtype in _BITS else buf
-    fill = _buffer(0, 'cpu', buf.dtype, 1, 0)
-    fill = int((fill.view(_BITS[buf.dtype]) if buf.dtype in _BITS else fill)[0])
-    guard = torch.ones(bits.numel(), dtype=torch.bool, device=buf.device)
-    guard[index.reshape(-1)] = False
-    return int((bits[guard] != fill).sum())
-
-
 def _results(P):
     return [o['buf'].view(-1)[o['index'].reshape(-1)].view(o['ref'].shape) for o in P.outs]
 
@@ -1793,7 +1736,7 @@ def check_case(K, c, dev):
         P2.call(K)
         torch.cuda.synchronize()
         for o, a_, b_ in zip(P.outs, got, _results(P2)):
-            bits = lambda t: t.contiguous().view(-1).view(_BITS[t.dtype]) if t.dtype in _BITS else t
+            bits = lambda t: t.contiguous().view(-1).view(BITS[t.dtype]) if t.dtype in BITS else t
             if not torch.equal(bits(a_), bits(b_)):
                 rec['errors'].append('%s differs between two runs' % o['name'])
     rec['ok'] = not rec['errors']

@@ -129,7 +129,7 @@ def test_planted_faults_are_rejected_at_drawn_shapes(k):
     # one guard element written
     buf = torch.full((P.layout['size'],), float('nan'))
     buf[P.index.reshape(-1)] = P.ref.reshape(-1).float()
-    assert GP.guard_intact(buf, P.index) == 0
+    assert GP.guard_touched(buf, P.index) == 0
     inside = set(P.index.reshape(-1).tolist())
     for pos in (P.layout['d0'] - 1, int(P.index.max()) + 1,
                 next((j for j in range(int(P.index.min()), int(P.index.max())) if j not in inside), None)):
@@ -137,4 +137,4 @@ def test_planted_faults_are_rejected_at_drawn_shapes(k):
             continue
         b = buf.clone()
         b[pos] = 0.0
-        assert GP.guard_intact(b, P.index) == 1, pos
+        assert GP.guard_touched(b, P.index) == 1, pos

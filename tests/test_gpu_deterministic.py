@@ -9,7 +9,6 @@ Model level: the same sequence of steps (eager runs, graph replays, SGD) from th
 losses, gradients and parameters; deterministic and default mode agree; a checkpoint resumes exactly.
 """
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -22,6 +21,7 @@ for _p in (HERE, os.path.dirname(HERE), os.path.join(os.path.dirname(HERE), 'vid
         sys.path.insert(0, _p)
 
 import harness as H  # noqa: E402
+from util import capture_fd2, parse_record, run_worker  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -49,13 +49,11 @@ def _twice(fn, out):
 
 
 def _gemm_records(text):
-    import gemm_paths as GP
-    recs = [GP.parse_record(l) for l in text.splitlines()]
+    recs = [parse_record(l) for l in text.splitlines()]
     return [r for r in recs if r]
 
 
 def _check_wgrad(K, label, shape, co, ker, st, pd, dil, tol, expect=None):
-    import gemm_paths as GP
     dev = 'cuda'
     gen = torch.Generator(device='cpu').manual_seed(7)
     g = K.conv_geom(shape, co, ker, st, pd, dil)
@@ -71,7 +69,7 @@ def _check_wgrad(K, label, shape, co, ker, st, pd, dil, tol, expect=None):
     else:
         dw = torch.zeros((co, g.kT, g.kH, g.kW, g.C), device=dev)
         mask = None
-    (a, b), text = GP.capture_fd2(lambda: _twice(lambda: K.conv_wgrad_det(dyr, xr, dw, g, col_mask=mask), dw))
+    (a, b), text = capture_fd2(lambda: _twice(lambda: K.conv_wgrad_det(dyr, xr, dw, g, col_mask=mask), dw))
     assert torch.equal(a, b), label
     recs = [r for r in _gemm_records(text) if r.get('det') == 1]
     assert recs, (label, text[-500:])
@@ -92,7 +90,7 @@ def _check_wgrad(K, label, shape, co, ker, st, pd, dil, tol, expect=None):
                                           padding=(g.pT, g.pH, g.pW), dilation=(g.dT, g.dH, g.dW))
         got = a.permute(0, 4, 1, 2, 3).double()
     err = _rel(got, ref)
-    print('wgrad %-32s rel %.2e  %s' % (label, err, ' '.join('cp=%d sk=%d fix=%d bn=%d wide=%d' % (
+    print('[deterministic] wgrad %-32s rel %.2e  %s' % (label, err, ' '.join('cp=%d sk=%d fix=%d bn=%d wide=%d' % (
         r['cp'], r['sk'], r['fix'], r['bn'], r.get('wide', 0)) for r in recs)))
     assert err < tol, (label, err)
     return recs
@@ -100,7 +98,6 @@ def _check_wgrad(K, label, shape, co, ker, st, pd, dil, tol, expect=None):
 
 def kernel_checks():
     from vlfb import kernels as K
-    import gemm_paths as GP
     import wgrad_cases as WC
     dev = 'cuda'
     gen = torch.Generator(device='cpu').manual_seed(3)
@@ -116,12 +113,12 @@ def kernel_checks():
         ar, br = a.clone(), b.clone()
         K.round_tf32(a, ar), K.round_tf32(b, br)
         d = torch.empty((1, M, N), device=dev)
-        (x, y), text = GP.capture_fd2(lambda: _twice(lambda: K.matmul_det(ar, br, d, tf32_out=tf32), d))
+        (x, y), text = capture_fd2(lambda: _twice(lambda: K.matmul_det(ar, br, d, tf32_out=tf32), d))
         assert torch.equal(x, y)
         for r in _gemm_records(text):
             assert r['split'] == 1 and (r['sk'] == 0 or r['fix'] == 1), r
         err = _rel(x, ar.double() @ br.double())
-        print('matmul_det %dx%dx%d tf32=%d rel %.2e' % (M, N, Kd, tf32, err))
+        print('[deterministic] matmul_det %dx%dx%d tf32=%d rel %.2e' % (M, N, Kd, tf32, err))
         assert err < (1e-3 if tf32 else 1e-4)
     # bias gradients
     for rows, cols in [(100352, 64), (40, 2048), (7, 80)]:
@@ -131,7 +128,7 @@ def kernel_checks():
         a, b = _twice(lambda: K.colsum_det(x, cols, out, rows, cols, accumulate=True), out)
         assert torch.equal(a, b)
         err = _rel(a - o0, x.double().sum(0))
-        print('colsum_det %dx%d rel %.2e' % (rows, cols, err))
+        print('[deterministic] colsum_det %dx%d rel %.2e' % (rows, cols, err))
         assert err < 1e-5
     # RoIAlign backward against the fp64 sample-table reference of tests/streaming_cases.py: the res5 width (C 2048)
     # with boxes on the map's edges, 100 random boxes, and 32 identical boxes (every sample collides)
@@ -153,7 +150,7 @@ def kernel_checks():
         a, b = _twice(lambda: K.roi_align_bwd_det(dout, rois_d, dfeat, scale, sr), dfeat)
         assert torch.equal(a, b)
         excess = float(((a.double() - ref).abs() - terms * 2.0 ** -23 * 2 * mag).max())
-        print('roi_align_bwd_det %s R=%d C=%d: max |err| - bound %.2e' % (kind, R, C, excess))
+        print('[deterministic] roi_align_bwd_det %s R=%d C=%d: max |err| - bound %.2e' % (kind, R, C, excess))
         assert excess <= 0, kind
     # SpatialBN statistics
     rows, C = 2 * 8 * 28 * 28, 128
@@ -175,14 +172,14 @@ def kernel_checks():
     yr = (xr - xr.mean(0)) / torch.sqrt(xr.var(0, unbiased=False) + 1e-5) * s.double() + bb.double()
     yr.backward(dy.double())
     assert _rel(a, xr.grad) < 1e-4, _rel(a, xr.grad)
-    print('spatial_bn det fwd / bwd ok')
+    print('[deterministic] spatial_bn det fwd / bwd ok')
     # grouped weight gradient (ResNeXt branch2b), split over positions into workspace slabs
     import gconv_cases as GC  # noqa: F401  (the grouped geometries' conventions)
     g = K.conv_geom((2, 8, 28, 28, 256), 256, (3, 3, 3), (1, 1, 1), (1, 1, 1))
     x = torch.randn((2, 8, 28, 28, 256), generator=gen).to(dev)
     dy = torch.randn((2, g.To, g.Ho, g.Wo, 256), generator=gen).to(dev)
     dw = torch.zeros((256, 3, 3, 3, 8), device=dev)
-    (a, b), text = GP.capture_fd2(lambda: _twice(lambda: K.conv_wgrad_det(dy, x, dw, g, groups=32), dw))
+    (a, b), text = capture_fd2(lambda: _twice(lambda: K.conv_wgrad_det(dy, x, dw, g, groups=32), dw))
     assert torch.equal(a, b)
     rec = [l for l in text.splitlines() if 'vlfb gconv:' in l and 'dir=wgrad' in l]
     assert rec and 'det=1' in rec[-1], text[-300:]
@@ -191,7 +188,7 @@ def kernel_checks():
     ref = torch.nn.grad.conv3d_weight(x.double().permute(0, 4, 1, 2, 3), (256, 8, 3, 3, 3),
                                       dy.double().permute(0, 4, 1, 2, 3), padding=(1, 1, 1), groups=32)
     err = _rel(a.permute(0, 4, 1, 2, 3), ref)
-    print('grouped wgrad det rel %.2e' % err)
+    print('[deterministic] grouped wgrad det rel %.2e' % err)
     assert err < 1e-5
     print('KERNEL CHECKS OK')
 
@@ -211,22 +208,18 @@ def forced_cp_checks():
     print('FORCED CP CHECKS OK')
 
 
-def _worker(args, extra_env, ok):
-    env = dict(os.environ)
-    env['VLFB_DEBUG'] = '1'
-    env.update(extra_env)
-    r = subprocess.run([sys.executable, os.path.abspath(__file__)] + args, env=env, capture_output=True, text=True,
-                       cwd=os.path.dirname(HERE))
+def _worker(args, ok):
+    r, _ = run_worker('test_gpu_deterministic.py', args, timeout=1800, tag='deterministic', jsonl=False)
     print(r.stdout[-6000:])
     assert r.returncode == 0 and ok in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
 
 
 def test_deterministic_kernels():
-    _worker([], {}, 'KERNEL CHECKS OK')
+    _worker([], 'KERNEL CHECKS OK')
 
 
 def test_deterministic_wgrad_fixup_on_128_row_cp_async_tiles():
-    _worker(['--forced-cp'], {}, 'FORCED CP CHECKS OK')
+    _worker(['--forced-cp'], 'FORCED CP CHECKS OK')
 
 
 # ------------------------------------------------------------------------------------------------ model level
@@ -386,6 +379,8 @@ def test_full_size_benchmark_config_is_bitwise_reproducible(ws):
 
 
 if __name__ == '__main__':
+    if os.environ.get('VLFB_DEBUG') != '1':
+        raise SystemExit('the path records need VLFB_DEBUG=1')
     if '--forced-cp' in sys.argv:
         forced_cp_checks()
     else:

@@ -1,11 +1,6 @@
 """Grouped convolution on the GPU (csrc/gconv.cu through vlfb_gemm with groups > 1): the case table of
 tests/gconv_cases.py elementwise against fp64, and ResNeXt-50 32x4d (RESNETS.NUM_GROUPS 32, WIDTH_PER_GROUP 4) nets
 through the builder API against the fp64 oracle, with the tolerances of tests/test_gpu_model.py."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -13,23 +8,18 @@ import torch
 import harness as H
 import resnext_oracle as RO
 from test_gpu_model import FULL, TINY, _oracle, _train_case, ws  # noqa: F401  (ws: the fixture)
+from util import run_worker
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 RESNEXT = ['RESNETS.NUM_GROUPS', 32, 'RESNETS.WIDTH_PER_GROUP', 4]
 
 
-def test_case_table(tmp_path):
+def test_case_table():
     """Every case of the table in its own process (VLFB_DEBUG is read once per process): bound, guard bands, sign
     bits and the path record.  Prints each case's bound ratio (max |got - ref| / bound) and the worst per family."""
-    out = str(tmp_path / 'gconv_cases.jsonl')
-    env = dict(os.environ, VLFB_DEBUG='1')
-    cmd = [sys.executable] + (['-s'] if sys.flags.no_user_site else []) + [os.path.join(HERE, 'gconv_cases.py'),
-                                                                             '--out', out]
-    proc = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=1800)
+    proc, recs = run_worker('gconv_cases.py', [], timeout=1800)
     assert proc.returncode == 0, proc.stderr[-4000:]
-    recs = [json.loads(line) for line in open(out)]
     import gconv_cases as GC
     assert len(recs) == len(GC.CASES)
     worst = {}

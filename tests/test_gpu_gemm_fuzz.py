@@ -4,64 +4,27 @@ Each (configuration, seed) runs tests/gemm_fuzz.py once in its own process with 
 its fp64 reference elementwise, leave its guard band and stream-K counters untouched, run on the engine the ABI
 predicts and, when deterministic, give the same bits twice.  A coverage floor keeps the generator at the edges: each
 named cell must be reached by at least FLOOR passing draws."""
-import json
-import os
-import subprocess
-import sys
-
 import pytest
 
 import gemm_fuzz as GF
 import gemm_paths as GP
+from util import run_worker
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 TIMEOUT = 900            # seconds per worker; a worker that times out fails its tests and is not started again
 RUNS = GF.RUNS
 FLOOR = 3
-_RESULTS = {}
 
 
-def _launch(cfg, seed, count, tmp_dir):
-    out = os.path.join(tmp_dir, 'gemm_fuzz_%s_%d.jsonl' % (cfg, seed))
-    env = dict((k, v) for k, v in os.environ.items() if k not in GP.SWITCHES)
-    env.update(GP.CONFIGS[cfg])
-    env['VLFB_DEBUG'] = '1'
-    cmd = [sys.executable] + (['-s'] if sys.flags.no_user_site else []) + [
-        os.path.join(HERE, 'gemm_fuzz.py'), '--config', cfg, '--seed', str(seed), '--count', str(count), '--out', out]
-    try:
-        proc = subprocess.run(cmd, env=env, cwd=os.path.dirname(HERE), capture_output=True, text=True, timeout=TIMEOUT)
-    except subprocess.TimeoutExpired as ex:
-        so = ex.stdout.decode() if isinstance(ex.stdout, bytes) else (ex.stdout or '')
-        last = [l for l in so.splitlines() if l.startswith('[gemm_fuzz]')]
-        return dict(timeout=last[-1] if last else '(none)')
-    recs = []
-    if os.path.exists(out):
-        with open(out) as f:
-            recs = [json.loads(l) for l in f if l.strip()]
-    return dict(proc=proc, recs=recs)
-
-
-def _run(cfg, seed, count, tmp_dir):
-    key = (cfg, seed)
-    if key not in _RESULTS:
-        _RESULTS[key] = _launch(cfg, seed, count, tmp_dir)
-    r = _RESULTS[key]
-    if 'timeout' in r:
-        pytest.fail('configuration %s seed %d timed out after %d s; last progress line: %s' % (cfg, seed, TIMEOUT,
-                                                                                               r['timeout']))
-    return r['proc'], r['recs']
-
-
-@pytest.fixture(scope='module')
-def tmp_dir(tmp_path_factory):
-    return str(tmp_path_factory.mktemp('gemm_fuzz'))
+def _run(cfg, seed, count):
+    return run_worker('gemm_fuzz.py', ['--config', cfg, '--seed', str(seed), '--count', str(count)],
+                      env=GP.CONFIGS[cfg], timeout=TIMEOUT)
 
 
 @pytest.mark.parametrize('cfg,seed,count', RUNS)
-def test_every_draw_matches_fp64(cfg, seed, count, tmp_dir):
-    proc, recs = _run(cfg, seed, count, tmp_dir)
+def test_every_draw_matches_fp64(cfg, seed, count):
+    proc, recs = _run(cfg, seed, count)
     assert proc.returncode == 0, 'worker exit %d\n%s\n%s' % (proc.returncode, proc.stdout[-3000:], proc.stderr[-3000:])
     assert [r['index'] for r in recs] == list(range(count))
     bad = ['seed %d index %d (%s): %s\n    %s' % (seed, r['index'], r['family'], '; '.join(r['errors']), r['reproducer'])
@@ -124,12 +87,12 @@ def coverage_cells():
     return cells
 
 
-def test_coverage_floor(tmp_dir):
+def test_coverage_floor():
     """Each cell is reached by at least FLOOR passing draws (over every configuration and seed)."""
     counts = dict((k, 0) for k in coverage_cells())
     cells = coverage_cells()
     for cfg, seed, count in RUNS:
-        _, recs = _run(cfg, seed, count, tmp_dir)
+        _, recs = _run(cfg, seed, count)
         for r in recs:
             if not r['ok']:
                 continue

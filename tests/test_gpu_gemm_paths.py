@@ -4,61 +4,24 @@ Every configuration of the library's switches runs tests/gemm_paths.py in its ow
 process).  Each case must match its fp64 reference elementwise, leave its guard band untouched and take the path it
 declares; together the configurations must cover every instantiation, loader, tile width, schedule and special form of
 the kernel, each named in the failure message when it is missing."""
-import json
-import os
-import subprocess
-import sys
-
 import pytest
 
 import gemm_paths as GP
+from util import run_worker
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-TIMEOUT = 900            # seconds per configuration; the child is killed when it expires
-_RESULTS = {}
+# seconds per configuration; the default one also runs the production weight gradients
+TIMEOUT = dict(default=4500)
 
 
-def _launch(cfg, tmp_dir):
-    """Runs the worker of one configuration ONCE; the outcome (records, or the timeout) is kept for every later test."""
-    out = os.path.join(tmp_dir, 'gemm_paths_%s.jsonl' % cfg)
-    env = dict((k, v) for k, v in os.environ.items() if k not in GP.SWITCHES)
-    env.update(GP.CONFIGS[cfg])
-    env['VLFB_DEBUG'] = '1'
-    cmd = [sys.executable] + (['-s'] if sys.flags.no_user_site else []) + [
-        os.path.join(HERE, 'gemm_paths.py'), '--config', cfg, '--out', out]
-    try:
-        proc = subprocess.run(cmd, env=env, cwd=os.path.dirname(HERE), capture_output=True, text=True, timeout=TIMEOUT)
-    except subprocess.TimeoutExpired as ex:
-        so = ex.stdout.decode() if isinstance(ex.stdout, bytes) else (ex.stdout or '')
-        last = [l for l in so.splitlines() if l.startswith('[gemm_paths]')]
-        return dict(timeout=last[-1] if last else '(none)')
-    recs = []
-    if os.path.exists(out):
-        with open(out) as f:
-            recs = [json.loads(l) for l in f if l.strip()]
-    return dict(proc=proc, recs=recs)
-
-
-def _run(cfg, tmp_dir):
-    """(process, records) of a configuration; fails -- without starting it again -- if its worker timed out."""
-    if cfg not in _RESULTS:
-        _RESULTS[cfg] = _launch(cfg, tmp_dir)
-    r = _RESULTS[cfg]
-    if 'timeout' in r:
-        pytest.fail('configuration %s timed out after %d s; last progress line: %s' % (cfg, TIMEOUT, r['timeout']))
-    return r['proc'], r['recs']
-
-
-@pytest.fixture(scope='module')
-def tmp_dir(tmp_path_factory):
-    return str(tmp_path_factory.mktemp('gemm_paths'))
+def _run(cfg):
+    return run_worker('gemm_paths.py', ['--config', cfg], env=GP.CONFIGS[cfg], timeout=TIMEOUT.get(cfg, 900))
 
 
 @pytest.mark.parametrize('cfg', sorted(GP.CONFIGS))
-def test_gemm_paths_match_fp64_and_declared_path(cfg, tmp_dir):
-    proc, recs = _run(cfg, tmp_dir)
+def test_gemm_paths_match_fp64_and_declared_path(cfg):
+    proc, recs = _run(cfg)
     want = [c['name'] for c in GP.CASES if cfg in c['runs']]
     assert proc.returncode == 0, 'worker exit %d\n%s\n%s' % (proc.returncode, proc.stdout[-3000:], proc.stderr[-3000:])
     assert [r['case'] for r in recs] == want
@@ -74,11 +37,11 @@ def _strided(case_name):
     return g is not None and tuple(g['st']) != (1, 1, 1)
 
 
-def test_gemm_path_coverage(tmp_dir):
+def test_gemm_path_coverage():
     """The union over all configurations reaches every path of the kernel (checked on passing cases only)."""
     seen = []
     for cfg in sorted(GP.CONFIGS):
-        _, recs = _run(cfg, tmp_dir)
+        _, recs = _run(cfg)
         for r in recs:
             if r['ok'] and len(r['paths']) == 1:
                 p = dict(r['paths'][0])
@@ -129,16 +92,32 @@ def test_gemm_path_coverage(tmp_dir):
         'K == 32 (one chunk)': lambda: any_(lambda n, f, p: p['K'] == 32),
         'batch > 1': lambda: any_(lambda n, f, p: p['z'] > 1 and p['kinds'][1] in (0, 1) and p['kinds'][0] in (0, 1)),
         'taps > 1': lambda: any_(lambda n, f, p: p['z'] > 1 and p['kinds'][1] in (4, 6)),
+        'wide tiles N <= bn': lambda: any_(lambda n, f, p: p.get('wide') == 1 and p['N'] <= p['bn']),
+        'wide tiles bn < N < 2 bn': lambda: any_(lambda n, f, p: p.get('wide') == 1 and p['bn'] < p['N'] < 2 * p['bn']),
+        'wide tiles N = 2 bn q + 16': lambda: any_(lambda n, f, p: p.get('wide') == 1 and p['N'] >= 2 * p['bn'] and
+                                                   p['N'] % (2 * p['bn']) == 16),
     })
+    for bn in (32, 64, 128):
+        need['wide tiles bn=%d' % bn] = lambda bn=bn: any_(lambda n, f, p: p.get('wide') == 1 and p['bn'] == bn)
+    # every B operand of a weight gradient under both multi-CTA schedules, on 128-row and on 64 x 2bn wide tiles
+    # (conv1 has Co = 64: its STEM_MN launches are always wide)
+    scheds = {'stream-K': lambda p: p['sk'] == 1, 'split-K > 1': lambda p: p['sk'] == 0 and p['split'] > 1}
+    for bk, wides in ((GP.OP_CONV_MN, (0, 1)), (GP.OP_DENSE_MN, (0, 1)), (GP.OP_STEM_MN, (1,))):
+        for sname, sched in scheds.items():
+            for wide in wides:
+                need['wgrad B kind %d %s on %s tiles' % (bk, sname, 'wide' if wide else 'narrow')] = \
+                    (lambda bk=bk, sched=sched, wide=wide:
+                     any_(lambda n, f, p: p['kinds'][0] == GP.OP_DENSE_MN and p['kinds'][1] == bk and sched(p) and
+                          p.get('wide', 0) == wide))
     missing = [name for name, pred in need.items() if not pred()]
     assert not missing, 'not covered by any passing case: ' + '; '.join(missing)
 
 
-def test_mn_major_operands_are_staged_by_cp_async(tmp_dir):
+def test_mn_major_operands_are_staged_by_cp_async():
     """Every launch record, in every configuration: an MN-major operand has no TMA loader and runs in a cp.async build."""
     bad = []
     for cfg in sorted(GP.CONFIGS):
-        _, recs = _run(cfg, tmp_dir)
+        _, recs = _run(cfg)
         for r in recs:
             for p in r['paths']:
                 ak, bk = p['kinds']

@@ -6,7 +6,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from util import rel_err, stem_pack, tf32_round, to_cl, to_nc, w_to_cl
+from util import pack_sign_bits, rel_err, stem_pack, tf32_round, to_cl, to_nc, w_to_cl
 
 pytestmark = pytest.mark.gpu
 
@@ -72,13 +72,6 @@ def test_matmul_layouts(K, backend, ta, tb, B, M, N, K_):
     if M % 4 == 0 and N % 4 == 0:
         torch.cuda.synchronize()
         assert rel_err(dt.transpose(1, 2), ref + 1.0) < 2e-5
-
-
-def pack_sign_bits(x):
-    """Reference bit layout of vlfb_gemm_params_t.relu_mask_bits / relu_bits_out: bit e & 31 of word e >> 5 = x.flat[e] > 0."""
-    b = (x.reshape(-1, 32) > 0).to(torch.int64)
-    v = (b << torch.arange(32, dtype=torch.int64, device=x.device)).sum(1)
-    return torch.where(v >= 2 ** 31, v - 2 ** 32, v).to(torch.int32)
 
 
 def test_relu_bits_kernel(K):

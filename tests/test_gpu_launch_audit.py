@@ -5,20 +5,14 @@ engine.  Each net runs in its own process with VLFB_DEBUG set, so every GEMM rec
 
 The full-size config-2 step (the benchmarked one) runs once unaudited, then once audited, every call, within a
 ten-minute budget."""
-import json
-import os
-import subprocess
-import sys
 import time
 
 import pytest
 
-import gemm_paths as GP
 import launch_audit as LA
+from util import run_worker
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 GPU_NETS = ['ava_train', 'ava_train_simt', 'ava_train_dropout', 'charades_train', 'charades_softmax_train',
             'ava_val_fold_f32', 'ava_val_fold_bf16', 'ava_lfb_infer_only', 'ava_train_det', 'ava_train_capacity',
@@ -28,20 +22,13 @@ BUDGET_S = dict(config2_train=600.0)
 
 
 @pytest.mark.parametrize('net', GPU_NETS)
-def test_every_launch_of_a_tiny_net_matches_fp64(net, tmp_path):
-    out = tmp_path / ('%s.jsonl' % net)
-    env = dict(os.environ, VLFB_DEBUG='1')
-    for k in GP.SWITCHES:
-        if k != 'VLFB_DEBUG':
-            env.pop(k, None)
+def test_every_launch_of_a_tiny_net_matches_fp64(net):
     t0 = time.time()
-    p = subprocess.run([sys.executable, os.path.join(HERE, 'launch_audit.py'), '--net', net, '--out', str(out)],
-                       env=env, capture_output=True, text=True, timeout=1200)
+    p, recs = run_worker('launch_audit.py', ['--net', net], timeout=1200)
     wall = time.time() - t0
     print('\n[%s] wall %.1f s\n%s' % (net, wall, p.stdout[-4000:]))
     assert p.returncode == 0, p.stderr[-4000:]
-    recs = [json.loads(l) for l in out.read_text().splitlines() if l.strip()]
-    tail = recs.pop()
+    *recs, tail = recs
     assert not tail['missing'], 'wrappers the net never reached: %s' % tail['missing']
     bad = [r for r in recs if not r['ok']]
     assert not bad, '\n'.join(e for r in bad[:20] for e in r['errors'])

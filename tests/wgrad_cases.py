@@ -1,6 +1,6 @@
 """The weight-gradient convolutions of one training step of R50-I3D-NL at 2 clips of 32 x 224^2 (the benchmarked network),
-one entry per distinct geometry, with the number of its launches per step.  Shared by tests/test_gpu_wgrad_pipeline.py
-and scripts/bench_wgrad.py.
+one entry per distinct geometry, with the number of its launches per step.  Shared by tests/gemm_paths.py (the
+production cases of its table), tests/test_gpu_deterministic.py and scripts/bench_wgrad.py.
 
 Entry: (label, in_shape (N, T, H, W, C), Co, kernel, strides, pads, dilations, launches per step).  conv1 has C = 4 (RGB
 plus the zero pad channel the library's stem path expects)."""
