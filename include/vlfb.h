@@ -138,12 +138,22 @@ typedef struct {
    * partial-tile area and a second pass adds them to d in split order.  SIMT engine: split 1 (each element is then
    * written by one thread).  Without VLFB_EPI_ATOMIC every element is stored once anyway and the field changes nothing. */
   int deterministic;
+  /* ---- product precision (VLFB_PREC_*) ----
+   * VLFB_PREC_TF32 (0): the tensor core multiplies TF32 x TF32 and truncates fp32 operands to TF32, so callers that want
+   * round-to-nearest operands round them where they are produced (VLFB_EPI_TF32, vlfb_round_tf32, ...).
+   * VLFB_PREC_X3 (1): split TF32.  Each operand x = hi + lo (hi = x truncated to TF32, lo = x - hi, exact) and every
+   * product is hi*hi + hi*lo + lo*hi: three MMAs per product, within about 3 * 2^-20 of |a b| of the fp32 product, for
+   * unrounded fp32 operands.  The SIMT engine and the grouped convolutions (groups > 1) multiply in fp32 already: for
+   * them the field changes nothing, and fp32 accuracy only needs operands that were not rounded to TF32. */
+  int precision;
 } vlfb_gemm_params_t;
 
 enum { VLFB_ENGINE_TCGEN05 = 0, VLFB_ENGINE_SIMT = 1 };
+enum { VLFB_PREC_TF32 = 0, VLFB_PREC_X3 = 1 };
 
 /* What vlfb_gemm would do for `p` (host-only, no launch; not defined for groups > 1).  With p->deterministic and
- * VLFB_EPI_ATOMIC, split_k is 1 and stream_k = 1 only when the workspace fields allow the fix-up. */
+ * VLFB_EPI_ATOMIC, split_k is 1 and stream_k = 1 only when the workspace fields allow the fix-up.  The plan is that of
+ * p->precision: a VLFB_PREC_X3 plan takes no tile width that would leave fewer than 3 pipeline stages. */
 typedef struct {
   int tile_n;                 /* output-tile width */
   int split_k;                /* plain split-K factor (atomic epilogues) */
@@ -391,4 +401,5 @@ int vlfb_lfb_gather(const float* bank, int64_t bank_rows, const int32_t* idx, fl
 #endif
 #include "vlfb_det.h"
 #include "vlfb_live.h"
+#include "vlfb_prec.h"
 #endif /* VLFB_H_ */

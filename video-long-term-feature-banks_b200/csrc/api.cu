@@ -29,6 +29,7 @@ static int validate_gemm(const vlfb_gemm_params_t& p, bool& tc_ok) {
   VLFB_CHECK_ARG(p.tile_n == 0 || (p.tile_n >= 32 && p.tile_n <= 256 && p.tile_n % 32 == 0));
   VLFB_CHECK_ARG(p.split_k == 1 || (p.flags & VLFB_EPI_ATOMIC));
   VLFB_CHECK_ARG(p.deterministic == 0 || p.deterministic == 1);
+  VLFB_CHECK_ARG(p.precision == VLFB_PREC_TF32 || p.precision == VLFB_PREC_X3);
   VLFB_CHECK_ARG(!(p.deterministic && p.split_k > 1));   // a deterministic launch is never split (split_k 0 = 1)
   const bool split = p.deterministic ? p.split_k > 1 : p.split_k != 1;
   VLFB_CHECK_ARG(!(split && (p.residual || p.relu_mask || p.relu_mask_bits || (p.flags & (VLFB_EPI_RELU | VLFB_EPI_TF32)))));
@@ -107,6 +108,7 @@ static int validate_gconv(const vlfb_gemm_params_t& p) {
   VLFB_CHECK_ARG(p.a.ptr && p.b.ptr && p.d);
   VLFB_CHECK_ARG(p.M > 0 && p.N > 0 && p.K > 0);
   VLFB_CHECK_ARG(p.deterministic == 0 || p.deterministic == 1);
+  VLFB_CHECK_ARG(p.precision == VLFB_PREC_TF32 || p.precision == VLFB_PREC_X3);   // fp32 products either way
   GCONV_REQUIRE(p.batch == 1, VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 needs batch == 1");
   GCONV_REQUIRE(p.split_k == 0 || p.split_k == 1, VLFB_E_UNSUPPORTED, "vlfb_gemm: groups > 1 needs split_k <= 1");
   GCONV_REQUIRE(p.a.kind != VLFB_OP_STEM_K && p.a.kind != VLFB_OP_STEM_MN && p.b.kind != VLFB_OP_STEM_K &&
@@ -179,6 +181,7 @@ int vlfb_version(void) { return 100; }
 const char* vlfb_last_error(void) { return g_err; }
 int vlfb_gemm_plan(const vlfb_gemm_params_t* p, int num_sms, vlfb_gemm_plan_t* plan) {
   VLFB_CHECK_ARG(p && plan && p->M > 0 && p->N > 0 && p->K > 0);
+  VLFB_CHECK_ARG(p->precision == VLFB_PREC_TF32 || p->precision == VLFB_PREC_X3);
   if (p->groups > 1) {
     set_error("vlfb_gemm_plan: grouped convolutions (groups > 1) run on CUDA cores and have no tile plan");
     return VLFB_E_UNSUPPORTED;

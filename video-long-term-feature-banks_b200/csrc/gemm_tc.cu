@@ -208,6 +208,10 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
 
+// Split-TF32 (VLFB_PREC_X3): x = hi + lo with hi = x with its low 13 mantissa bits cleared (what the tensor core reads of
+// an fp32 operand: it truncates) and lo = x - hi, which is exact in fp32.
+__device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+
 // Consumer-side rewrite of an MN-major stage tile into the K-major SWIZZLE_128B image [row][128 B] that wgmma reads
 // (tf32 operands in shared memory must be K-major).  Source: `rows` x 32 k as [atom of 32 elements][k-row][128 B]
 // (MNLoader), 16-byte chunk c of k-row k at byte (16 c) ^ (32 (k & 3)), k-rows 128 B and atoms 4 KB apart.
@@ -220,7 +224,9 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 //   loads:  slot = c ^ 2 (k & 3) = kq ^ b ^ 2 r for load r  -> 8 distinct slots;
 //   stores: slot = kq ^ (n % 8) = kq ^ 4 ((kq ^ b) & 1) ^ q  -> kq ^ const on even kq, kq ^ (const ^ 4) on odd kq, a
 //           bijection of 0..7 (bit 0 is kept) -> 8 distinct slots.
-__device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int rows, int ctid) {
+// LO (split TF32, DESIGN.md 4.7): the same pass also writes the lo image of every element to `dst_lo`, in the image's layout.
+template <bool LO = false>
+__device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int rows, int ctid, uint32_t dst_lo = 0) {
   for (int u = ctid; u < rows * 2; u += NEPI) {
     const int kq = u & 7, c = kq ^ ((u >> 3) & 7), atom = u >> 6;
     float v[4][4];
@@ -238,7 +244,23 @@ __device__ __forceinline__ void mn_to_kmajor(uint32_t src, uint32_t dst, int row
       asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};"
                    ::"r"(dst + (uint32_t)(n * 128 + ((kq ^ (n & 7)) << 4))), "f"(v[0][q]), "f"(v[1][q]), "f"(v[2][q]), "f"(v[3][q])
                    : "memory");
+      if constexpr (LO)
+        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};"
+                     ::"r"(dst_lo + (uint32_t)(n * 128 + ((kq ^ (n & 7)) << 4))), "f"(tf32_lo(v[0][q])), "f"(tf32_lo(v[1][q])),
+                       "f"(tf32_lo(v[2][q])), "f"(tf32_lo(v[3][q]))
+                     : "memory");
     }
+  }
+}
+
+// lo image of a K-major stage tile of `bytes` bytes: elementwise, so it keeps the tile's SWIZZLE_128B layout and the
+// wgmma descriptors of the tile address it at the same offsets.  Consecutive 16-byte units per thread: conflict-free.
+__device__ __forceinline__ void kmajor_lo(uint32_t src, uint32_t dst, uint32_t bytes, int ctid) {
+  for (uint32_t o = (uint32_t)ctid * 16u; o < bytes; o += NEPI * 16u) {
+    float v0, v1, v2, v3;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v0), "=f"(v1), "=f"(v2), "=f"(v3) : "r"(src + o) : "memory");
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};"
+                 ::"r"(dst + o), "f"(tf32_lo(v0)), "f"(tf32_lo(v1)), "f"(tf32_lo(v2)), "f"(tf32_lo(v3)) : "memory");
   }
 }
 
@@ -694,712 +716,25 @@ __device__ __forceinline__ bool sched_next(const vlfb_gemm_params_t& p, const La
 // FIX: the stream-K fix-up (a piece of a shared tile through the workspace) is compiled in; only the launches that plan
 // fix-ups use these instantiations.  Its last-arriver decision is per warp, so the K loop must leave no MMA in flight
 // when it ends on any path (ptxas would otherwise serialise every wgmma of the kernel, tests/test_gemm_pipeline_cpu.py).
+// X3: split-TF32 products (gemm_tc3_kernel, DESIGN.md 4.7).  The consumers build a lo image of every operand chunk
+// (double-buffered like the B images) and issue A_hi B_hi + A_hi B_lo + A_lo B_hi per k8 step; the stage tiles and the
+// K-major images of MN-major operands are the hi operands as they stand (the tensor core truncates fp32 to TF32).
 template <int AK, int BK, bool MASK, bool CP, bool FIX>
 __global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc_kernel(const vlfb_gemm_params_t p, const Launch L,
                                                               const __grid_constant__ CUtensorMap tmA,
                                                               const __grid_constant__ CUtensorMap tmB) {
-  static_assert(CP || (!is_mn(AK) && !is_mn(BK)), "MN-major operands are staged by cp.async only");
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int bn = L.bn, S = L.stages;
-  // K-major images of the MN-major operands (wgmma reads tf32 operands K-major only): one for A, two for B (chunk i
-  // uses B image i % 2)
-  constexpr bool TA = is_mn(AK), TB = is_mn(BK);
-  // wide tile (Launch::wide): WM A rows, 2 bn B rows per stage; the images alias the epilogue staging tiles, which are
-  // idle during the K loop (one barrier after the loop's final drain orders the MMAs' reads before the staging stores)
-  const bool wide = CP && TA && TB && L.wide != 0;
-  const int a_rows = wide ? WM : BM, b_rows = bn << (wide ? 1 : 0);
-  const uint32_t a_tile_bytes = (uint32_t)a_rows * KC * 4;
-  const uint32_t b_tile_bytes = (uint32_t)b_rows * KC * 4;
-  const uint32_t stage_bytes = a_tile_bytes + b_tile_bytes;
-  const uint32_t img_base = smem_base + S * stage_bytes;
-  const uint32_t epi_base = img_base + (wide ? 0u : (TA ? a_tile_bytes : 0u) + (TB ? 2 * b_tile_bytes : 0u));   // per-consumer-warp transpose tiles
-  const uint32_t ka_img = wide ? epi_base : img_base;
-  const uint32_t kb_img = ka_img + (TA ? a_tile_bytes : 0u);
-  const uint32_t bar_base = epi_base + EPI_STAGE_BYTES;
-  const uint32_t full0 = bar_base, empty0 = bar_base + 8 * MAX_STAGES;
-
-  constexpr int NPRODT = CP ? NPROD : NPROD_TMA;   // producer threads of this build
-  constexpr int NPWT = NPRODT / 32;
-  const int tid = threadIdx.x;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform role: producer / consumer branches are not divergent
-  const int unit = (int)blockIdx.x;
-  const int nunits = (int)gridDim.x;
-  const bool tma_a = !is_mn(AK) && L.tma_a != 0, tma_b = !is_mn(BK) && L.tma_b != 0;
-  const bool cp_any = CP && !(tma_a && tma_b);
-
-#ifdef VLFB_TRACE
-  if (tid == 0 && L.trace) {
-    unsigned long long gt;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-    L.trace[(size_t)blockIdx.x * 64 + 1] = gt;
-    TR(0);
-  }
-#endif
-  if (tid == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(full0 + 8 * s, (cp_any ? NPROD : 0) + ((tma_a || tma_b) ? 1 : 0));
-      mbar_init(empty0 + 8 * s, NEPI / 128);          // one arrival per consumer warpgroup
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) TR(2);
-
-  if (warp < NPWT) {
-    // ============================ PRODUCERS (8 cp.async warps / one TMA issuer) ============================
-    // The TMA issuer is thread 0: it posts the expected byte count and issues the boxes of every chunk, after waiting for
-    // the free stage like every cp.async thread.
-    const bool issuer = tid == 0;
-    if (cp_any || issuer) {
-      KLoader<is_mn(AK) ? VLFB_OP_DENSE_K : AK, BM / RSTEP> ka;
-      MNLoader<is_mn(AK) ? AK : VLFB_OP_DENSE_MN> ma;
-      KLoader<is_mn(BK) ? VLFB_OP_DENSE_K : BK, BN_MAX / RSTEP> kb;
-      MNLoader<is_mn(BK) ? BK : VLFB_OP_DENSE_MN> mb;
-      const int LAG = L.lag;
-      // Publishing a cp.async chunk.  Both operands MN-major (wgrad): the consumers read the stage tiles only through
-      // their generic-proxy rewrite (mn_to_kmajor), so no proxy fence is needed and each thread's arrival on the stage
-      // barrier is triggered by the completion of its copies (cp.async.mbarrier.arrive): the producers run up to
-      // `stages` chunks ahead of the MMAs.  Otherwise a thread publishes chunk c itself after issuing chunk c + lag
-      // (wait_group, then the proxy fence wgmma's async-proxy reads need).  That ties each publication to a stage the
-      // consumers release, and with lag = stages - 2 producers and consumers take turns chunk by chunk.
-      constexpr bool ASYNC_PUB = CP && is_mn(AK) && is_mn(BK);
-      // compile-time gates keep the im2col state out of the instantiations that cannot use it (registers)
-      const bool im2col_a = (AK == VLFB_OP_CONV_K || AK == VLFB_OP_DGRAD_K) && L.tma_a == 2;
-      // im2col state of the issuing thread: window origin of the tile's first row + filter-tap cursor
-      int ia_w = 0, ia_h = 0, ia_d = 0, ia_n = 0, ic_t = 0, ic_h = 0, ic_w = 0, ic_c = 0, icpt = 1;
-      // conv1 stem rows (tma 3): the 128 tile rows = 8 groups of 16 consecutive output positions (16 | Wo, so a group
-      // never crosses an output row): per group the window origin (wo, hi0 = ho sH - pH, ti0 = to sT - pT, n)
-      const bool stem_a = AK == VLFB_OP_STEM_K && L.tma_a == 3;
-      constexpr int NSG = AK == VLFB_OP_STEM_K ? 8 : 1;
-      int sg_w[NSG], sg_ht[NSG], sg_n[NSG];
-      // chunk counter over the CTA's whole work sequence; ring slot / phase / lagged slot advance
-      // incrementally (S is a run-time value: `it % S` cost three integer divisions per chunk per thread)
-      int it = 0, s = 0, sl = 0;
-      uint32_t ph = 0;
-      Sched sc;
-      sched_init(sc, L, unit);
-      TileInfo ti;
-      int witem = 0;
-      while (sched_next(p, L, sc, unit, nunits, ti)) {
-        if (tid == 0 && witem < 4) TR(8 + 2 * witem);
-        const int nb0 = ti.n0;                           // first D column whose B rows this CTA stages
-        if (cp_any) {
-          // (A is loaded as a 128-row tile also when wide: a compile-time row count keeps the producers' per-chunk issue
-          // loop as short as it was; rows >= M are never copied, and a wide launch has M <= 64, so only its WM-row
-          // A stage tile is written)
-          if (!tma_a) { if (is_mn(AK)) ma.init(p, p.a, ti.m0, BM, p.M, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { ka.init(p, p.a, ti.m0, BM, p.M, ti.batch, L.out, L.in, ti.k_begin / KC); ka.kend = ti.k_end; } }
-          if (!tma_b) { if (is_mn(BK)) mb.init(p, p.b, ti.n0, b_rows, p.N, ti.batch, ti.tap, L.cdiv, L.kwdiv); else { kb.init(p, p.b, ti.n0, bn, p.N, ti.batch, L.out, L.in, ti.k_begin / KC); kb.kend = ti.k_end; } }
-        }
-        const int kc0 = ti.k_begin / KC;
-        // bytes the stage barrier expects
-        const uint32_t tma_bytes = (tma_a ? (uint32_t)A_TILE_BYTES : 0u) + (tma_b ? b_tile_bytes : 0u);
-        if (issuer && stem_a && L.stem_patch) {
-          const vlfb_conv_geom_t& g = p.g;
-          const int mt = ti.m0 / BM;
-          const int wb = mt % L.patch_wb, q = mt / L.patch_wb;
-          const int hb = q % L.patch_hb, rest = q / L.patch_hb;
-          const int to = rest % g.To, n = rest / g.To;
-          sg_w[0] = wb * 16;
-          sg_ht[0] = ((hb * 8 * g.sH - g.pH) << 16) | ((to * g.sT - g.pT) & 0xFFFF);
-          sg_n[0] = n;
-          ic_t = kc0 / g.kH;
-          ic_h = kc0 - ic_t * g.kH;
-        } else if (issuer && stem_a) {
-          const vlfb_conv_geom_t& g = p.g;
-          Pos4 o = decode_pos_fast((uint32_t)ti.m0, L.out);
-#pragma unroll
-          for (int q = 0; q < NSG; ++q) {
-            sg_w[q] = o.w;
-            sg_ht[q] = ((o.h * g.sH - g.pH) << 16) | ((o.t * g.sT - g.pT) & 0xFFFF);
-            sg_n[q] = (ti.m0 + 16 * q < p.M) ? o.n : g.N;          // rows past M: out of bounds in N -> zeros
-            o.w += 16;
-            if (o.w >= g.Wo) { o.w = 0; if (++o.h == g.Ho) { o.h = 0; if (++o.t == g.To) { o.t = 0; ++o.n; } } }
-          }
-          ic_t = kc0 / g.kH;
-          ic_h = kc0 - ic_t * g.kH;
-        }
-        if (issuer && im2col_a) {
-          const vlfb_conv_geom_t& g = p.g;
-          if (AK == VLFB_OP_CONV_K) {
-            const Pos4 o = decode_pos_fast((uint32_t)ti.m0, L.out);
-            ia_w = o.w * g.sW - g.pW; ia_h = o.h * g.sH - g.pH; ia_d = o.t * g.sT - g.pT; ia_n = o.n;
-            icpt = g.C / KC;
-          } else if (L.par) {   // parity class of a strided dgrad: unit-stride gather over dY with the class's taps
-            const Pos4 o = decode_pos_fast((uint32_t)ti.m0, L.sub);
-            ia_w = o.w + L.par_lo[0]; ia_h = o.h + L.par_lo[1];
-            ia_d = o.t + g.pT - (g.kT - 1) * g.dT; ia_n = o.n;
-            icpt = g.Co / KC;
-          } else {  // DGRAD_K, unit strides: dx[i] = sum_tap dy[i + pad - tap*dil] -> origin i + pad - (k-1)*dil
-            const Pos4 o = decode_pos_fast((uint32_t)ti.m0, L.in);
-            ia_w = o.w + g.pW - (g.kW - 1) * g.dW; ia_h = o.h + g.pH - (g.kH - 1) * g.dH;
-            ia_d = o.t + g.pT - (g.kT - 1) * g.dT; ia_n = o.n;
-            icpt = g.Co / KC;
-          }
-          const int tap = kc0 / icpt;
-          ic_c = kc0 - tap * icpt;
-          decode_tap(tap, g.kH, g.kW, ic_t, ic_h, ic_w);     // (par: kc0 = 0 -> all zero; ic_h / ic_w count the class's taps)
-        }
-        for (int i = 0; i < ti.nk; ++i, ++it) {
-          const int s_cur = s;
-          if (it >= S) mbar_wait(empty0 + 8 * s_cur, ph ^ 1u);
-          if (++s == S) { s = 0; ph ^= 1u; }
-          const uint32_t a_tile = smem_base + s_cur * stage_bytes;
-          const uint32_t b_tile = a_tile + a_tile_bytes;
-          const uint32_t fbar = full0 + 8 * s_cur;
-          if (issuer && tma_bytes) {
-            mbar_expect_tx(fbar, tma_bytes);
-            if (stem_a) {
-              const vlfb_conv_geom_t& g = p.g;
-              if (L.stem_patch) {                     // one {128 B x 16 wo x 8 rows (stride sH)} box = the whole A tile
-                tma_load_5d(a_tile, &tmA, 0, sg_w[0], (sg_ht[0] >> 16) + ic_h, (int)(short)(sg_ht[0] & 0xFFFF) + ic_t, sg_n[0], fbar);
-              } else {
-#pragma unroll
-                for (int q = 0; q < NSG; ++q)
-                  tma_load_5d(a_tile + q * 2048, &tmA, 0, sg_w[q], (sg_ht[q] >> 16) + ic_h, (int)(short)(sg_ht[q] & 0xFFFF) + ic_t,
-                              sg_n[q], fbar);
-              }
-              if (++ic_h == g.kH) { ic_h = 0; ++ic_t; }
-            } else if (im2col_a) {
-              const vlfb_conv_geom_t& g = p.g;
-              if (AK == VLFB_OP_CONV_K) {
-                tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, ic_w * g.dW, ic_h * g.dH, ic_t * g.dT, fbar);
-              } else if (AK == VLFB_OP_DGRAD_K && L.par) {
-                // tap (kt, rh + sH ic_h, rw + sW ic_w) of the class: dY offset (taps - 1 - index), weights at the original tap
-                const ParCls& c = L.par_cls[ti.batch];
-                tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, c.nw - 1 - ic_w, c.nh - 1 - ic_h, (g.kT - 1 - ic_t) * g.dT, fbar);
-                const int tap = (ic_t * g.kH + c.rh + g.sH * ic_h) * g.kW + c.rw + g.sW * ic_w;
-                tma_load_3d(b_tile, &tmB, tap * g.Co + ic_c * KC, nb0, 0, fbar);
-                if (++ic_c == icpt) {
-                  ic_c = 0;
-                  if (++ic_w == c.nw) { ic_w = 0; if (++ic_h == c.nh) { ic_h = 0; ++ic_t; } }
-                }
-              } else {
-                tma_load_im2col(a_tile, &tmA, ic_c * KC, ia_w, ia_h, ia_d, ia_n, (g.kW - 1 - ic_w) * g.dW,
-                    (g.kH - 1 - ic_h) * g.dH, (g.kT - 1 - ic_t) * g.dT, fbar);
-              }
-              if (!(AK == VLFB_OP_DGRAD_K && L.par) && ++ic_c == icpt) {
-                ic_c = 0;
-                if (++ic_w == g.kW) { ic_w = 0; if (++ic_h == g.kH) { ic_h = 0; ++ic_t; } }
-              }
-            } else if (tma_a) {
-              tma_load_3d(a_tile, &tmA, (kc0 + i) * KC, ti.m0, ti.batch, fbar);
-            }
-            if (tma_b && !(AK == VLFB_OP_DGRAD_K && L.par)) tma_load_3d(b_tile, &tmB, (kc0 + i) * KC, nb0, ti.batch, fbar);
-          }
-          if (!cp_any) continue;
-          if (!tma_a) {
-            if (is_mn(AK)) ma.issue(p, L.out, ti.k_begin + i * KC, ti.k_end, a_tile);
-            else ka.issue(p, kc0 + i, a_tile);
-          }
-          if (!tma_b) {
-            if (is_mn(BK)) mb.issue(p, L.out, ti.k_begin + i * KC, ti.k_end, b_tile);
-            else kb.issue(p, kc0 + i, b_tile);
-          }
-          if (ASYNC_PUB) {                 // published when its copies land; the producer moves on to the next chunk
-            cp_async_mbar_arrive(fbar);
-            continue;
-          }
-          cp_async_commit();
-          if (it >= LAG) {
-            cp_async_wait_dyn(LAG);
-            fence_proxy_async();
-            mbar_arrive(full0 + 8 * sl);
-            if (++sl == S) sl = 0;
-          }
-        }
-        if (tid == 0 && witem < 4) TR(9 + 2 * witem);
-        ++witem;
-      }
-      if (ASYNC_PUB) {
-        cp_async_wait<0>();              // (no copy may outlive the CTA's producers)
-      } else if (cp_any) {
-        cp_async_wait<0>();
-        fence_proxy_async();
-        for (int c = (it > LAG ? it - LAG : 0); c < it; ++c) {
-          mbar_arrive(full0 + 8 * sl);
-          if (++sl == S) sl = 0;
-        }
-      }
-    }
-  } else {
-    // ============================ CONSUMERS (2 warpgroups: wgmma K loop, then the epilogue) ============================
-    // Warp w of warpgroup g holds accumulator rows [64 g + 16 w, +16) of the tile (wgmma fragment layout; wide tiles: rows
-    // [16 w, +16) of columns [g bn, (g + 1) bn), so every output element still belongs to one warp).  After the K
-    // loop the warp writes them to its padded shared-memory tile (16 x EPITCH), so that the epilogue holds no accumulator
-    // registers and a warp store / residual load / atomic covers 8 rows x 64 contiguous bytes (whole 32-byte sectors).
-    const int ctid = tid - NPRODT;
-    // (from the broadcast warp index: warp-uniform for the compiler, so the wgmma descriptors, which add the warpgroup's
-    // offset, stay in uniform registers)
-    const int ew = warp - NPWT;          // consumer warp 0-7 = 4 wg + (warp % 4)
-    const int wg = ew >> 2;
-    const int wrow = 16 * (wide ? (ew & 3) : ew);   // its first tile row
-    const int wcol = wide ? wg * bn : 0;            // ... and first tile column (a wide tile's halves: one per warpgroup)
-    const int lane = tid & 31;
-    float* stg = reinterpret_cast<float*>(smem_raw + (epi_base - smem_u32(smem_raw))) + ew * EPI_WARP_FLOATS;
-    float* wsc = stg + 16 * EPITCH;      // column scale of the tile's columns, then the bias
-    float* wbi = wsc + BN_MAX;
-    int s = 0;
-    uint32_t ph = 0;
-    int colv_n0 = -1;
-    const size_t ws_tile_floats = (size_t)BM * bn;
-    int tile_iter = 0;
-    Sched sc;
-    sched_init(sc, L, unit);
-    TileInfo ti;
-    while (sched_next(p, L, sc, unit, nunits, ti)) {
-      // ---- K loop, instantiated per tile width so that the width is a compile-time constant of the MMA loop: the MMAs
-      // of chunk i are in flight while chunk i + 1 is issued; a stage goes back to the producers once the MMAs that
-      // read it have completed (the host keeps the cp.async lag <= stages - 2, so that release never waits on itself)
-      auto mma_tile = [&](auto bn_c) {
-        constexpr int BN = decltype(bn_c)::value;
-        float acc[BN / 2];
-#pragma unroll
-        for (int q = 0; q < BN / 2; ++q) acc[q] = 0.f;
-        // chunk i: at its start this warpgroup's MMAs of chunk i - 2 have completed (the wait<1> that ends chunk i - 1),
-        // so B image i % 2, which chunk i - 2 read, may be rewritten once both warpgroups are there; the MMAs of chunk
-        // i - 1, which read the other image, stay in flight meanwhile.  The single A image waits for all MMAs.
-        // Wide tile: both warpgroups read the one WM-row A image, warpgroup w rows [w BN, (w + 1) BN) of the B image.
-        const uint32_t a_wg = wide ? 0u : (uint32_t)wg * (64 * 128), b_wg = (uint32_t)wcol * 128;
-        for (int i = 0; i < ti.nk; ++i) {
-          mbar_wait(full0 + 8 * s, ph);
-          const uint32_t a_tile = smem_base + s * stage_bytes, b_tile = a_tile + a_tile_bytes;
-          const uint32_t b_img = kb_img + (i & 1) * b_tile_bytes;
-          if (TA || TB) {
-            if (TA) wgmma_wait<0>();             // no MMA still reads the A image
-            consumers_sync();                    // both warpgroups are done with chunk i - 2 (TA: i - 1)
-            if (TA) mn_to_kmajor(a_tile, ka_img, a_rows, ctid);
-            if (TB) mn_to_kmajor(b_tile, b_img, b_rows, ctid);
-            fence_proxy_async();                 // generic-proxy writes -> visible to the wgmma (async proxy) reads
-            consumers_sync();                    // images complete
-          }
-          const uint32_t a_src = (TA ? ka_img : a_tile) + a_wg;
-          const uint32_t b_src = (TB ? b_img : b_tile) + b_wg;
-          wgmma_fence();
-#pragma unroll
-          for (int j = 0; j < KC / 8; ++j)      // wgmma K = 8 for tf32: 32 bytes along the swizzled 128-byte rows
-            wgmma_tf32<BN>(acc, make_desc(a_src + 32 * j), make_desc(b_src + 32 * j), (i | j) ? 1u : 0u);
-          wgmma_commit();
-          if (i > 0) {
-            wgmma_wait<1>();
-            if ((ctid & 127) == 0) mbar_arrive(empty0 + 8 * ((s == 0 ? S : s) - 1));   // chunk i - 1's stage
-          }
-          if (++s == S) { s = 0; ph ^= 1u; }
-        }
-        // unconditional: a path that skips this wait (nk == 0) would let ptxas see accumulators in flight after the
-        // loop, and it then serialises every wgmma of the kernel
-        wgmma_wait<0>();
-        if (ti.nk > 0 && (ctid & 127) == 0) mbar_arrive(empty0 + 8 * ((s == 0 ? S : s) - 1));   // the last chunk's stage
-        // wide: the staging tiles below are the images the other warpgroup's MMAs may still read.  (The next tile's
-        // first chunk barrier orders this epilogue before the next rewrite.)
-        if (wide) consumers_sync();
-        // fragment (n8 group j: rows lane / 4 and lane / 4 + 8, columns 8 j + 2 (lane % 4) + {0, 1}) -> stg
-        float* r = stg + (lane >> 2) * EPITCH + 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(r + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(r + 8 * EPITCH + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-        __syncwarp();
-      };
-      switch (bn) {
-        case 32: mma_tile(std::integral_constant<int, 32>{}); break;
-        case 64: mma_tile(std::integral_constant<int, 64>{}); break;
-        case 96: mma_tile(std::integral_constant<int, 96>{}); break;
-        default: mma_tile(std::integral_constant<int, 128>{}); break;
-      }
-      // epilogue switches, read per tile (kernel parameters) rather than held in registers through the K loop
-      const bool vec_ok = ((p.ldd & 3) == 0) && ((p.d_batch_stride & 3) == 0) && ((p.d_tap_stride & 3) == 0) &&
-                          ((reinterpret_cast<uintptr_t>(p.d) & 15) == 0) &&
-                          (!p.residual || (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) &&
-                          (!p.relu_mask || (reinterpret_cast<uintptr_t>(p.relu_mask) & 15) == 0) &&
-                          !(p.residual && (p.flags & VLFB_EPI_ACCUM));
-      const int col = (lane & 3) * 4;
-      const bool want_res = (p.residual != nullptr) || (p.flags & VLFB_EPI_ACCUM);
-      const float* res_src = p.residual ? p.residual : p.d;
-      if (ew == 0 && lane == 0 && tile_iter < 4) TR(24 + 4 * tile_iter);
-      const bool par = AK == VLFB_OP_DGRAD_K && L.par != 0;
-      const int64_t tile_off = par ? 0 : (int64_t)ti.batch * p.d_batch_stride + (int64_t)ti.tap * p.d_tap_stride;
-      if ((want_res || MASK) && !par) {
-        // pull the NEXT tile's residual / mask rows into L2 while this tile is being written out
-        Sched sn = sc;
-        TileInfo tn;
-        if (sched_next(p, L, sn, unit, nunits, tn) && tn.npieces() == 1) {
-          const int64_t noff = (int64_t)tn.batch * p.d_batch_stride + (int64_t)tn.tap * p.d_tap_stride;
-          const int segs = b_rows >> 5;
-          for (int idx = ctid; idx < a_rows * segs; idx += NEPI) {
-            const int row = idx / segs, seg = idx - row * segs;
-            const int m = tn.m0 + row, n = tn.n0 + seg * 32;
-            if (m < p.M && n < p.N) {
-              if (want_res) prefetch_l2(res_src + noff + (int64_t)m * p.ldd + n);
-              if (MASK && p.relu_mask) prefetch_l2(p.relu_mask + noff + (int64_t)m * p.ldd + n);
-            }
-          }
-        }
-      }
-      const int n0w = ti.n0 + wcol;      // first D column of this warp's accumulator
-      if (wide || ti.n0 != colv_n0) {
-        // per-column affine of this warp's blocks -> shared memory, once per N tile (not per block: the
-        // global-load latency used to sit in front of every block's first FFMA); every tile when wide (the K loop's
-        // images overwrite it)
-        colv_n0 = ti.n0;
-        for (int i = lane; i < bn; i += 32) {
-          const int n = n0w + i;
-          wsc[i] = (p.col_scale && n < p.N) ? p.col_scale[n] : 1.f;
-          wbi[i] = (p.col_bias && n < p.N) ? p.col_bias[n] : 0.f;
-        }
-        __syncwarp();
-      }
-      float rs[EROWS];
-#pragma unroll
-      for (int i = 0; i < EROWS; ++i) {
-        const int m = ti.m0 + wrow + (lane >> 2) + 8 * i;
-        rs[i] = (p.row_scale && m < p.M) ? p.row_scale[m] : 1.f;
-      }
-      // One pass over this warp's column blocks.  mode 0: accumulator -> fused epilogue -> D (whole tile here);
-      // mode 1 (stream-K piece): raw accumulator -> this unit's workspace slot; mode 2 (last unit to arrive at a
-      // shared tile): sum of ALL pieces' slots in piece order (deterministic) -> fused epilogue -> D.
-      auto run_blocks = [&](auto mode_c) {
-        constexpr int mode = decltype(mode_c)::value;
-        const bool wres = want_res && mode != 1;
-        // residual / accumulate operands are fetched one column block ahead (register double buffer): with only
-        // 8 epilogue warps per SM the loads must be in flight while the previous block is stored, otherwise the
-        // epilogue is DRAM-latency bound (Little's law) instead of bandwidth bound
-        auto load_res = [&](int c0, float4* r) {
-          const int n = n0w + c0 + col;
-          const bool ok = wres && vec_ok && c0 < bn && n + 3 < p.N;
-#pragma unroll
-          for (int i = 0; i < EROWS; ++i) {
-            const int m = ti.m0 + wrow + (lane >> 2) + 8 * i;
-            r[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (ok && m < p.M) r[i] = ld_nc_f4(res_src + tile_off + (int64_t)m * p.ldd + n);
-          }
-        };
-        // ReLU mask (backward of the ReLU that produced this GEMM's D-shaped input): fetched one block ahead like
-        // the residual, but AFTER the accumulator block has left the registers and packed to 16 bits as soon as
-        // it arrives, so that it never coexists with both residual buffers (register budget).
-        auto load_mask = [&](int c0, float4* mk) {
-          const int n = n0w + c0 + col;
-          const bool ok = mode != 1 && vec_ok && c0 < bn && n + 3 < p.N;
-#pragma unroll
-          for (int i = 0; i < EROWS; ++i) {
-            const int m = ti.m0 + wrow + (lane >> 2) + 8 * i;
-            mk[i] = make_float4(1.f, 1.f, 1.f, 1.f);
-            if (ok && m < p.M) {
-              const int64_t e = tile_off + (int64_t)m * p.ldd + n;
-              if (p.relu_mask) {
-                mk[i] = ld_nc_f4(p.relu_mask + e);
-              } else {                                 // sign bits (n % 4 == 0: the four bits sit in one word)
-                const uint32_t nib = p.relu_mask_bits[e >> 5] >> (e & 31);
-                mk[i] = make_float4((nib & 1u) ? 1.f : 0.f, (nib & 2u) ? 1.f : 0.f, (nib & 4u) ? 1.f : 0.f, (nib & 8u) ? 1.f : 0.f);
-              }
-            }
-          }
-        };
-        auto pack_mask = [](const float4* mk) {
-          uint32_t b = 0;
-#pragma unroll
-          for (int i = 0; i < EROWS; ++i)
-            b |= ((mk[i].x > 0.f ? 1u : 0u) | (mk[i].y > 0.f ? 2u : 0u) | (mk[i].z > 0.f ? 4u : 0u) |
-                  (mk[i].w > 0.f ? 8u : 0u)) << (4 * i);
-          return b;
-        };
-        uint32_t mbits = 0xFFFFu;
-        if (MASK) {
-          float4 mk[EROWS];
-          load_mask(0, mk);
-          mbits = pack_mask(mk);
-        }
-        // MASK instantiations keep one residual buffer (register budget)
-        constexpr bool DB = !MASK;
-        float4 rr[EROWS], rn[EROWS];
-        if (DB) load_res(0, rr);          // independent of the accumulator: issued before the wait
-        for (int c0 = 0; c0 < bn; c0 += EPC) {
-          if (n0w + c0 >= p.N) break;              // warp-uniform (a wide tile's half past N: no block)
-          if (DB) load_res(c0 + EPC, rn);
-          else load_res(c0, rr);                   // L2-resident (tile-ahead prefetch)
-          float4 mk[EROWS];
-          if (MASK) load_mask(c0 + EPC, mk);
-          const int n = n0w + c0 + col;
-          const bool nfull = n + 3 < p.N;
-          const int cvi = c0 + col;
-          const float4 cs = *reinterpret_cast<const float4*>(wsc + cvi);
-          float4 cb = *reinterpret_cast<const float4*>(wbi + cvi);
-          if (mode == 0 && ti.k_begin != 0) cb = make_float4(0.f, 0.f, 0.f, 0.f);      // split-K: bias from the first K slice only
-#pragma unroll
-          for (int i = 0; i < EROWS; ++i) {
-            const int row = (lane >> 2) + 8 * i;
-            const int m = ti.m0 + wrow + row;
-            float4 a4;
-            if (mode == 2) {
-              const size_t wso = (size_t)(wrow + row) * bn + c0 + col;
-              a4 = make_float4(0.f, 0.f, 0.f, 0.f);
-              for (int j = 0; j < ti.npieces(); ++j) {
-                const int sl = (j == 0) ? ti.first_slot() : 0;
-                const float4 w4 = ld_cg_f4(L.ws_tiles + ((size_t)((ti.ufirst() + j) * 2 + sl) ) * ws_tile_floats + wso);
-                a4.x += w4.x; a4.y += w4.y; a4.z += w4.z; a4.w += w4.w;
-              }
-            } else {
-              a4 = *reinterpret_cast<const float4*>(stg + row * EPITCH + c0 + col);
-            }
-            if (mode == 1) {
-              float* const ws_mine = L.ws_tiles + ((size_t)(unit * 2 + ti.slot()) ) * ws_tile_floats;
-              *reinterpret_cast<float4*>(ws_mine + (size_t)(wrow + row) * bn + c0 + col) = a4;
-              continue;
-            }
-            if (m >= p.M || n >= p.N) continue;
-            if (nfull && vec_ok) {
-              float4 o = make_float4(a4.x * p.alpha, a4.y * p.alpha, a4.z * p.alpha, a4.w * p.alpha);
-              o.x = (o.x * cs.x + cb.x) * rs[i]; o.y = (o.y * cs.y + cb.y) * rs[i];
-              o.z = (o.z * cs.z + cb.z) * rs[i]; o.w = (o.w * cs.w + cb.w) * rs[i];
-              const int64_t off = tile_off + (int64_t)m * p.ldd + n;
-              if (want_res) { o.x += rr[i].x; o.y += rr[i].y; o.z += rr[i].z; o.w += rr[i].w; }   // residual or D (ACCUM)
-              if (p.flags & VLFB_EPI_RELU) {
-                o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-              }
-              if (MASK) {
-                const uint32_t mb = mbits >> (4 * i);
-                o.x = (mb & 1u) ? o.x : 0.f; o.y = (mb & 2u) ? o.y : 0.f;
-                o.z = (mb & 4u) ? o.z : 0.f; o.w = (mb & 8u) ? o.w : 0.f;
-              }
-              if (p.flags & VLFB_EPI_TF32) {
-                o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w);
-              }
-              float* dst = p.d + off;
-              if (p.flags & VLFB_EPI_ATOMIC) {
-                atomicAdd(dst, o.x); atomicAdd(dst + 1, o.y); atomicAdd(dst + 2, o.z); atomicAdd(dst + 3, o.w);
-              } else {
-                *reinterpret_cast<float4*>(dst) = o;
-              }
-            } else {
-              const float e4[4] = {a4.x, a4.y, a4.z, a4.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                if (n + e < p.N) epilogue_store(p, ti.batch, ti.tap, m, n + e, e4[e], mode != 0 || ti.k_begin == 0);
-            }
-          }
-          __syncwarp();
-          if (MASK) mbits = pack_mask(mk);
-          if (DB) {
-#pragma unroll
-            for (int i = 0; i < EROWS; ++i) rr[i] = rn[i];
-          }
-        }
-      };
-      // The same pass, lean: for tiles whose rows are 16-byte addressable and whose N extent is a whole number of
-      // 16-column blocks (every layer of the networks).  run_blocks pays per-float4 flag tests, 64-bit address
-      // arithmetic and bounds checks; here every run-time switch is tested once per tile (warp-uniform), rows are
-      // precomputed 32-bit offsets and the column offset is one add per block.
-      auto run_fast = [&](auto mode_c, auto atomic_c, auto wres_c, auto bits_c) {
-        constexpr int mode = decltype(mode_c)::value;
-        constexpr bool ATOMIC = decltype(atomic_c)::value && mode != 1;
-        constexpr bool WRES = decltype(wres_c)::value && mode != 1;
-        constexpr bool BITS = decltype(bits_c)::value && mode != 1 && !ATOMIC;      // emit the ReLU sign bits of the result
-        const int r0 = wrow + (lane >> 2);                         // tile rows r0 + 8 i of this lane
-        const int cbase = 0 + col;
-        const bool patch = AK == VLFB_OP_STEM_K && L.stem_patch != 0;
-        const int mrows = par ? L.par_m : p.M;
-        uint32_t rowok = 0;
-#pragma unroll
-        for (int i = 0; i < EROWS; ++i) rowok |= (patch || ti.m0 + r0 + 8 * i < mrows) ? (1u << i) : 0u;
-        const int ncols = min(bn, p.N - ti.n0);                            // multiple of 16
-        // ONE 32-bit element offset per row, shared by every stream (D, residual, sign bits: same addressing), advanced by
-        // one block (32 columns) per step; 64-bit row pointers per stream cost 24 registers, which the look-ahead
-        // buffers need (the host / fast_tile test guarantees offsets < 2^32)
-        uint32_t eo[EROWS];
-        float* wsp = nullptr;                  // mode 1: this unit's workspace slot (rows 8 bn apart)
-        unsigned short* bout = nullptr;        // relu_bits_out group of tile row r0 + 8 (lane & 3) (this lane stores that row's)
-        constexpr bool emit_bits = BITS;
-        if (mode == 1)
-          wsp = L.ws_tiles + ((size_t)(unit * 2 + ti.slot()) ) * ws_tile_floats + (size_t)r0 * bn + cbase;
-#pragma unroll
-        for (int i = 0; i < EROWS; ++i) {
-          int64_t row = ti.m0 + r0 + 8 * i;
-          if (patch) row = patch_row(p, L, ti.m0 / BM, r0 + 8 * i);      // conv1 patch tile: row -> (ho, wo) of the patch
-          if (par && ((rowok >> i) & 1u)) row = par_row(p, L, ti.batch, ti.m0 + r0 + 8 * i);   // parity class: sub-grid row -> dX row
-          eo[i] = (uint32_t)(tile_off + row * p.ldd + ti.n0 + cbase);
-        }
-        if (emit_bits) {
-          const int rb = r0 + 8 * (lane & 3);
-          int64_t row = ti.m0 + rb;
-          if (patch) row = patch_row(p, L, ti.m0 / BM, rb);
-          bout = reinterpret_cast<unsigned short*>(p.relu_bits_out) + ((tile_off + row * p.ldd + ti.n0 + 0) >> 4);
-        }
-        const unsigned short* mbase = reinterpret_cast<const unsigned short*>(p.relu_mask_bits);
-        const bool relu = (p.flags & VLFB_EPI_RELU) != 0, tf32 = (p.flags & VLFB_EPI_TF32) != 0;
-        const bool has_rs = p.row_scale != nullptr;
-        const bool nobias = mode == 0 && ti.k_begin != 0;                  // split-K: bias from the first K slice only
-        const float alpha = p.alpha;
-        // residual / accumulate / mask operands of the block `ahead` blocks after the current one.  ReLU-backward mask
-        // (MASK builds): the sign bits of the activation that gates this gradient, one 16-bit group per row and block.
-        auto load_ahead = [&](bool valid, int ahead, float4* r, uint32_t* m) {
-#pragma unroll
-          for (int i = 0; i < EROWS; ++i) {
-            const uint32_t e = eo[i] + (uint32_t)(ahead * EPC);
-            if (WRES) {
-              r[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (valid && ((rowok >> i) & 1u)) r[i] = ld_nc_f4(res_src + e);
-            }
-            if (MASK && mode != 1) {
-              m[i] = 0xFFFFu;
-              if (valid && ((rowok >> i) & 1u)) m[i] = ld_nc_u16(mbase + ((e - (uint32_t)col) >> 4));
-            }
-          }
-        };
-        // Residual / mask operands are fetched VLFB_EPI_DEPTH blocks ahead into a ring of register buffers; the loop is
-        // unrolled over the ring so that no buffer is ever copied (a `cur = next` move at the end of an iteration waits
-        // for the load it copies).
-        constexpr int NBUF = VLFB_EPI_DEPTH + 1;
-        float4 rbuf[NBUF][EROWS];
-        uint32_t mbuf[NBUF][EROWS];
-        load_ahead(0 < ncols, 0, rbuf[0], mbuf[0]);
-        if (NBUF == 3) load_ahead(0 + EPC < ncols, 1, rbuf[1], mbuf[1]);
-        // one 32 x 16 block: operands of block c0 in (rc, mc); the block VLFB_EPI_DEPTH ahead is fetched into (rl, ml)
-        auto step = [&](int c0, int cofs, const float4* rc, const uint32_t* mc, float4* rl, uint32_t* ml) {
-          load_ahead(c0 + EPC * VLFB_EPI_DEPTH < ncols, VLFB_EPI_DEPTH, rl, ml);
-          float4 a4[EROWS];
-          uint32_t obits = 0;
-          if (mode != 2) {
-#pragma unroll
-            for (int i = 0; i < EROWS; ++i)
-              a4[i] = *reinterpret_cast<const float4*>(stg + ((lane >> 2) + 8 * i) * EPITCH + c0 + col);
-            __syncwarp();
-            if (par && ti.nk == 0) {                                        // class without taps: dX = finish(0)
-#pragma unroll
-              for (int i = 0; i < EROWS; ++i) a4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < EROWS; ++i) a4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            for (int j = 0; j < ti.npieces(); ++j) {                        // piece order: deterministic sum
-              const int sl = (j == 0) ? ti.first_slot() : 0;
-              const float* w = L.ws_tiles + ((size_t)((ti.ufirst() + j) * 2 + sl) ) * ws_tile_floats +
-                               (size_t)r0 * bn + cbase + cofs;
-#pragma unroll
-              for (int i = 0; i < EROWS; ++i) {
-                const float4 w4 = ld_cg_f4(w + (size_t)i * 8 * bn);
-                a4[i].x += w4.x; a4[i].y += w4.y; a4[i].z += w4.z; a4[i].w += w4.w;
-              }
-            }
-          }
-          if (mode == 1) {
-#pragma unroll
-            for (int i = 0; i < EROWS; ++i) *reinterpret_cast<float4*>(wsp + (size_t)i * 8 * bn) = a4[i];
-            wsp += EPC;
-            return;
-          }
-          const int cvi = c0 + col;
-          float4 cs = *reinterpret_cast<const float4*>(wsc + cvi);
-          float4 cb = *reinterpret_cast<const float4*>(wbi + cvi);
-          cs.x *= alpha; cs.y *= alpha; cs.z *= alpha; cs.w *= alpha;
-          if (nobias) cb = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int i = 0; i < EROWS; ++i) {
-            float4 o;
-            o.x = fmaf(a4[i].x, cs.x, cb.x); o.y = fmaf(a4[i].y, cs.y, cb.y);
-            o.z = fmaf(a4[i].z, cs.z, cb.z); o.w = fmaf(a4[i].w, cs.w, cb.w);
-            if (has_rs) { o.x *= rs[i]; o.y *= rs[i]; o.z *= rs[i]; o.w *= rs[i]; }
-            if (WRES) { o.x += rc[i].x; o.y += rc[i].y; o.z += rc[i].z; o.w += rc[i].w; }
-            if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-            if (MASK) {
-              const uint32_t nib = mc[i] >> ((lane & 3) * 4);
-              o.x = (nib & 1u) ? o.x : 0.f; o.y = (nib & 2u) ? o.y : 0.f;
-              o.z = (nib & 4u) ? o.z : 0.f; o.w = (nib & 8u) ? o.w : 0.f;
-            }
-            if (tf32) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-            if ((rowok >> i) & 1u) {
-              if (ATOMIC) red_add_f4(p.d + eo[i], o);
-              else *reinterpret_cast<float4*>(p.d + eo[i]) = o;
-            }
-            eo[i] += EPC;
-            if (emit_bits) {             // the row's 16 sign bits: 4 lanes x 4 columns (warp-uniform branch)
-              uint32_t nb = (o.x > 0.f ? 1u : 0u) | (o.y > 0.f ? 2u : 0u) | (o.z > 0.f ? 4u : 0u) | (o.w > 0.f ? 8u : 0u);
-              nb <<= (lane & 3) * 4;
-              nb |= __shfl_xor_sync(0xffffffffu, nb, 1);
-              nb |= __shfl_xor_sync(0xffffffffu, nb, 2);
-              if ((lane & 3) == i) obits = nb;
-            }
-          }
-          if (emit_bits) {
-            if ((lane & 3) < EROWS && ((rowok >> (lane & 3)) & 1u)) *bout = (unsigned short)obits;
-            bout += EPC / 16;
-          }
-        };
-        {
-          int c0 = 0, cofs = 0;                                    // cofs: column offset of the block from cbase (mode 2)
-          while (c0 < ncols) {
-#pragma unroll
-            for (int b = 0; b < NBUF; ++b) {
-              if (c0 < ncols) step(c0, cofs, rbuf[b], mbuf[b], rbuf[(b + NBUF - 1) % NBUF], mbuf[(b + NBUF - 1) % NBUF]);
-              c0 += EPC; cofs += EPC;
-            }
-          }
-        }
-      };
-      // run-time epilogue flavour -> compile-time flags (atomic accumulate; residual / D-accumulate stream)
-      auto call_fast = [&](auto mode_c) {
-        using T = std::true_type;
-        using F = std::false_type;
-        const bool atomic = (p.flags & VLFB_EPI_ATOMIC) != 0;
-        if (decltype(mode_c)::value == 1) run_fast(mode_c, F{}, F{}, F{});
-        else if (atomic) { if (want_res) run_fast(mode_c, T{}, T{}, F{}); else run_fast(mode_c, T{}, F{}, F{}); }
-        else if (!MASK && p.relu_bits_out != nullptr) { if (want_res) run_fast(mode_c, F{}, T{}, T{}); else run_fast(mode_c, F{}, F{}, T{}); }
-        else { if (want_res) run_fast(mode_c, F{}, T{}, F{}); else run_fast(mode_c, F{}, F{}, F{}); }
-      };
-      // (cp.async builds take the fix-up path only in the MN x MN instantiations of deterministic atomic launches)
-      const bool split_tile = FIX && ti.npieces() > 1;
-      // cp.async fix-up, first half: a piece is this warp's raw staging rows, copied to its slot (tile row r at r * tile
-      // columns + column, so a wide tile's two warpgroups fill their own column halves).  gemm_fixup_kernel, launched
-      // after this kernel, sums the slots of every shared tile in piece order and applies the epilogue once.  (The
-      // in-kernel reduction of the TMA builds does not fit these 128-register builds without spills.)
-      auto cp_piece = [&]() {
-        const int bq = bn >> 2, tcols = bn << (wide ? 1 : 0);
-        float* slot = L.ws_tiles + (size_t)(unit * 2 + ti.slot()) * (BM * bn);
-        for (int idx = lane; idx < 16 * bq; idx += 32) {
-          const int r = idx / bq, c = (idx - r * bq) * 4;
-          *reinterpret_cast<float4*>(slot + (size_t)(wrow + r) * tcols + wcol + c) =
-              *reinterpret_cast<const float4*>(stg + r * EPITCH + c);
-        }
-        __syncwarp();
-      };
-      // (MASK builds: the lean path reads the mask as sign bits; a float mask takes the general path)
-      const bool bits_ok = (p.ldd & 15) == 0 && (p.d_batch_stride & 15) == 0 && (p.d_tap_stride & 15) == 0;
-      const bool fast_tile = !CP && vec_ok && (p.N & 15) == 0 && span32_ok(p) && !(MASK && (p.relu_mask != nullptr || !bits_ok));
-      if constexpr (!CP) {
-        if (fast_tile) {
-          if (split_tile) call_fast(std::integral_constant<int, 1>{});
-          else call_fast(std::integral_constant<int, 0>{});
-        } else {
-          if (split_tile) run_blocks(std::integral_constant<int, 1>{});
-          else run_blocks(std::integral_constant<int, 0>{});
-        }
-      } else {
-        if (split_tile) cp_piece();
-        else run_blocks(std::integral_constant<int, 0>{});
-      }
-      if (ew == 0 && lane == 0 && tile_iter < 4) TR(25 + 4 * tile_iter);
-      ++tile_iter;
-      if constexpr (FIX && !CP) if (split_tile) {
-        // publish this piece, count it; the warp that arrives last owns the reduction of its sub-blocks
-        __threadfence();
-        __syncwarp();
-        int* cnt = L.ws_cnt + (size_t)ti.tile * (NEPI / 32) + ew;
-        int old = 0;
-        if (lane == 0) old = atomicAdd(cnt, 1);
-        old = __shfl_sync(0xffffffffu, old, 0);
-        if (ew == 0 && lane == 0 && tile_iter <= 4) TR(26 + 4 * (tile_iter - 1));
-        if (old == ti.npieces() - 1) {
-          __threadfence();
-          if (fast_tile) call_fast(std::integral_constant<int, 2>{});
-          else run_blocks(std::integral_constant<int, 2>{});
-          if (lane == 0) *cnt = 0;                 // counters are zero again when the launch ends
-          if (ew == 0 && lane == 0 && tile_iter <= 4) TR(27 + 4 * (tile_iter - 1));
-        }
-      }
-    }
-  }
-  if (tid == 0) TR(3);
+  constexpr bool X3 = false;
+#include "gemm_tc_body.inc"
 }
+// split-TF32 products (VLFB_PREC_X3): the same roles, loaders, schedules and epilogue
+template <int AK, int BK, bool MASK, bool CP, bool FIX>
+__global__ void __launch_bounds__((CP ? NPROD : NPROD_TMA) + NEPI, 1) gemm_tc3_kernel(const vlfb_gemm_params_t p, const Launch L,
+                                                               const __grid_constant__ CUtensorMap tmA,
+                                                               const __grid_constant__ CUtensorMap tmB) {
+  constexpr bool X3 = true;
+#include "gemm_tc_body.inc"
+}
+
 
 // Second half of a cp.async stream-K launch with fix-ups (deterministic atomic MN x MN launches): CTA t sums the
 // workspace slots of tile t's pieces in piece order and applies d = epi(sum) (with VLFB_EPI_ATOMIC: d += epi(sum)) once
@@ -1545,11 +880,25 @@ static const Env& env() {
 // (Fitted to the Co = 64 wgrads of the benchmarked network, that term is worth 20-200 model clocks; with it a wide
 // launch takes the wider tile when both widths pad N alike.)
 // A tile adds a fixed fill + epilogue cost (~8 chunks' worth); a stream-K launch adds the fix-up of the shared tiles.
+// A split-TF32 chunk (x3) issues three times the MMAs and adds the consumers' lo-image pass: the chunk's operand bytes
+// read and written once through shared memory (128 B/clk) between two barriers (the same fixed latency as a wide rewrite).
 // The constants rank tile widths against each other; they are model values, not measurements.
-static double chunk_cost(int bn, bool wide) {
-  const double tensor = 4.0 * bn;
+static double chunk_cost(int bn, bool wide, bool x3 = false) {
+  const double tensor = (x3 ? 12.0 : 4.0) * bn;
   const double port = (wide ? 128.0 * (WM + 2 * bn) : 16384.0 + 128.0 * bn) / 64.0;
-  return (tensor > port ? tensor : port) + (wide ? 128.0 : 0.0);
+  const double lo = x3 ? 2.0 * (wide ? WM + 2 * bn : BM + bn) + (wide ? 0.0 : 128.0) : 0.0;
+  return (tensor > port ? tensor : port) + (wide ? 128.0 : 0.0) + lo;
+}
+
+// Pipeline stages that fit shared memory next to the epilogue staging, the K-major images of MN-major operands (A, 2 x B;
+// a wide launch keeps them in the epilogue staging) and, split-TF32, the lo images (2 x (A + B)); at most 6.
+static int fit_stages(int bn, bool wide, bool ta, bool tb, bool x3) {
+  const int a_tile_bytes = (wide ? WM : BM) * KC * 4, b_tile_bytes = (bn << (wide ? 1 : 0)) * KC * 4;
+  const int stage_bytes = a_tile_bytes + b_tile_bytes;
+  const int img_bytes = wide ? 0 : (ta ? a_tile_bytes : 0) + (tb ? 2 * b_tile_bytes : 0);
+  const int lo_bytes = x3 ? 2 * stage_bytes : 0;
+  const int s = (227 * 1024 - EPI_STAGE_BYTES - img_bytes - lo_bytes - 2048) / stage_bytes;
+  return s > 6 ? 6 : s;
 }
 
 // Wide tiles: both operands MN-major (their K-major images are built by the consumers, so the tile shape is free) and
@@ -1573,6 +922,11 @@ static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool
   if (want_bn > BN_MAX) want_bn = BN_MAX;                                      // wider requests get the widest tile
   if (pow2_only && want_bn == 96) want_bn = 64;                                // (the one width not a power of two)
   const int want_sk = p.stream_k != 0 ? p.stream_k : env().sk;
+  // split-TF32: a width whose lo images would leave fewer than 3 stages is not planned; a narrower tile is
+  const bool x3 = p.precision == VLFB_PREC_X3;
+  const bool ta = is_mn(p.a.kind), tb = is_mn(p.b.kind);
+  if (x3)
+    while (want_bn > 32 && fit_stages(want_bn, wide_tiles(p), ta, tb, true) < 3) want_bn = want_bn == 96 ? 64 : want_bn / 2;
   Plan best, best_sk;
   best.cost = 1e30; best.bn = 32; best.split_k = p.split_k > 0 ? p.split_k : 1; best.pair = 0; best.sk = 0;
   best.tiles = 0; best.units = 0;
@@ -1587,10 +941,11 @@ static Plan make_plan(const vlfb_gemm_params_t& p, int num_sms, bool sk_ok, bool
     const int tn = wide ? 2 * bn : bn;                                          // tile columns
     if (want_bn > 0 ? bn != want_bn : ((bn & (bn - 1)) != 0)) continue;       // 96 only on request
     if (want_bn <= 0 && bn > 32 && p.N <= tn / 2) continue;                   // do not pad N by 2x
+    if (x3 && fit_stages(bn, wide, ta, tb, true) < 3) continue;
     const int tiles_m = wide ? 1 : ceil_div(p.M, BM);
     const int64_t T = (int64_t)tiles_m * ceil_div(p.N, tn) * zbase;
     const int nkt = ceil_div(p.K, KC);
-    const double cc = chunk_cost(bn, wide);
+    const double cc = chunk_cost(bn, wide, x3);
     const double fixed = 8.0 * cc;
     // (a) static tile loop, optional plain split-K (atomic epilogues only)
     const int smax = det ? 1 : p.split_k > 0 ? p.split_k : (atomic && p.K >= 512 ? (p.K / 256 < 128 ? p.K / 256 : 128) : 1);
@@ -1642,20 +997,21 @@ size_t gemm_tc_workspace_bytes() {
   return (size_t)SK_CNT_INTS * 4 + (size_t)MAX_UNITS * 2 * BM * 256 * 4;
 }
 
-template <int AK, int BK, bool MASK, bool CP, bool FIX>
+template <int AK, int BK, bool MASK, bool CP, bool FIX, bool X3>
 static int launch_variant(const cudaLaunchConfig_t& cfg, const vlfb_gemm_params_t& p, const Launch& L, const CUtensorMap& tmA,
                           const CUtensorMap& tmB) {
+  constexpr auto kernel = X3 ? gemm_tc3_kernel<AK, BK, MASK, CP, FIX> : gemm_tc_kernel<AK, BK, MASK, CP, FIX>;
   static bool attr_done = false;
   cudaError_t e;
   if (!attr_done) {
-    e = cudaFuncSetAttribute(gemm_tc_kernel<AK, BK, MASK, CP, FIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(smem): %s", cudaGetErrorString(e));
       return VLFB_E_CUDA;
     }
     attr_done = true;
   }
-  e = cudaLaunchKernelEx(&cfg, gemm_tc_kernel<AK, BK, MASK, CP, FIX>, p, L, tmA, tmB);
+  e = cudaLaunchKernelEx(&cfg, kernel, p, L, tmA, tmB);
   if (e != cudaSuccess) {
     set_error("gemm_tc launch: %s", cudaGetErrorString(e));
     return VLFB_E_CUDA;
@@ -1808,10 +1164,15 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   // (the kernel computes the same stage layout)
   const int a_tile_bytes = (L.wide ? WM : BM) * KC * 4, b_tile_bytes = (L.bn << L.wide) * KC * 4;
   const int stage_bytes = a_tile_bytes + b_tile_bytes;
-  // K-major images: A, 2 x B; a wide launch keeps them in the epilogue staging tiles
+  // K-major images: A, 2 x B; a wide launch keeps them in the epilogue staging tiles.  Split TF32: 2 x (A + B) lo images.
+  const bool x3 = p.precision == VLFB_PREC_X3;
   const int img_bytes = L.wide ? 0 : (is_mn(AK) ? a_tile_bytes : 0) + (is_mn(BK) ? 2 * b_tile_bytes : 0);
-  L.stages = (227 * 1024 - EPI_STAGE_BYTES - img_bytes - 2048) / stage_bytes;
-  if (L.stages > 6) L.stages = 6;
+  const int lo_bytes = x3 ? 2 * stage_bytes : 0;
+  L.stages = fit_stages(L.bn, L.wide != 0, is_mn(AK), is_mn(BK), x3);
+  if (x3 && L.bn == BN_MAX) {          // make_plan rules it out (2 stages at most): the split builds have no such K loop
+    set_error("gemm_tc: split-TF32 launch planned at tile width %d", L.bn);
+    return VLFB_E_UNSUPPORTED;
+  }
   if (ev.stages >= 3 && ev.stages <= L.stages) L.stages = ev.stages;
   // The consumers release chunk c's stage after they have waited for chunk c + 1, and a cp.async producer publishes
   // chunk c only after the free-stage wait of chunk c + lag - stages.  lag <= stages - 2 keeps that wait behind a
@@ -1834,7 +1195,7 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       L.ws_tiles = reinterpret_cast<float*>(reinterpret_cast<char*>(p.workspace) + (size_t)SK_CNT_INTS * 4);
     }
   }
-  const int smem = L.stages * stage_bytes + img_bytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  const int smem = L.stages * stage_bytes + img_bytes + lo_bytes + EPI_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
   const bool cp = is_mn(AK) || is_mn(BK) || !(L.tma_a && L.tma_b);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)units);
@@ -1849,16 +1210,17 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
   // VLFB_DEBUG: one record per launch, space-separated key=value (tests/gemm_paths.py parses it; keep the keys stable)
   if (ev.debug)
     fprintf(stderr, "vlfb gemm_tc: kinds=%d,%d mask=%d M=%d N=%d K=%d z=%d bn=%d sk=%d split=%d tiles=%d units=%d stages=%d "
-            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d wide=%d det=%d\n",
+            "lag=%d tma=%d,%d cap=%d patch=%d par=%d cp=%d fix=%d lean=%d bits2=%d wide=%d det=%d prec=%d\n",
             AK, BK, MASK ? 1 : 0, p.M, p.N, p.K, zbase, L.bn, L.sk, p.split_k, L.total_tiles, units, L.stages, L.lag, L.tma_a,
             L.tma_b, cap, L.stem_patch, L.par, cp ? 1 : 0, L.ws_tiles != nullptr ? 1 : 0, lean ? 1 : 0, bits_after ? 1 : 0,
-            L.wide, det ? 1 : 0);
+            L.wide, det ? 1 : 0, x3 ? 1 : 0);
   int rc = VLFB_OK;
   // (cp.async fix-ups exist only in the MN x MN builds, for deterministic atomic launches: the planning loop above
   // gives any other cp.async launch no workspace)
   if (cp && L.ws_tiles) {
     if constexpr (cp_fix) {
-      rc = launch_variant<AK, BK, MASK, true, true>(cfg, p, L, tmA, tmB);
+      rc = x3 ? launch_variant<AK, BK, MASK, true, true, true>(cfg, p, L, tmA, tmB)
+              : launch_variant<AK, BK, MASK, true, true, false>(cfg, p, L, tmA, tmB);
       if (rc == VLFB_OK) {
         launch_k(gemm_fixup_kernel, dim3((unsigned)L.total_tiles), 256, 0, stream, p, L);
         VLFB_CHECK_LAUNCH();
@@ -1868,10 +1230,13 @@ int launch(const vlfb_gemm_params_t& p_in, cudaStream_t stream) {
       return VLFB_E_UNSUPPORTED;
     }
   } else if (cp) {
-    rc = launch_variant<AK, BK, MASK, true, false>(cfg, p, L, tmA, tmB);
+    rc = x3 ? launch_variant<AK, BK, MASK, true, false, true>(cfg, p, L, tmA, tmB)
+            : launch_variant<AK, BK, MASK, true, false, false>(cfg, p, L, tmA, tmB);
   } else if constexpr (!is_mn(AK) && !is_mn(BK)) {       // TMA-only builds exist for K-major pairs only
-    if (L.ws_tiles) rc = launch_variant<AK, BK, MASK, false, true>(cfg, p, L, tmA, tmB);
-    else rc = launch_variant<AK, BK, MASK, false, false>(cfg, p, L, tmA, tmB);
+    if (L.ws_tiles) rc = x3 ? launch_variant<AK, BK, MASK, false, true, true>(cfg, p, L, tmA, tmB)
+                            : launch_variant<AK, BK, MASK, false, true, false>(cfg, p, L, tmA, tmB);
+    else rc = x3 ? launch_variant<AK, BK, MASK, false, false, true>(cfg, p, L, tmA, tmB)
+                 : launch_variant<AK, BK, MASK, false, false, false>(cfg, p, L, tmA, tmB);
   }
   if (rc == VLFB_OK && bits_after) rc = relu_bits(p.d, bits_after, (int64_t)p.M * p.N, stream);
   return rc;

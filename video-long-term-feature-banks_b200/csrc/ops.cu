@@ -702,8 +702,10 @@ __global__ void weight_transpose_k(const float* __restrict__ w, float* __restric
   }
 }
 
-// the same for every convolution of the net in one launch (block -> job by binary search over block_begin)
-__global__ void weight_transpose_multi_k(const vlfb_wt_job_t* __restrict__ jobs, int njobs) {
+// the same for every convolution of the net in one launch (block -> job by binary search over block_begin); ROUND =
+// false stores w * scale unrounded (the fp32-accuracy dgrad operand of VLFB_PREC_X3 GEMMs)
+template <bool ROUND>
+__device__ __forceinline__ void weight_transpose_multi_body(const vlfb_wt_job_t* __restrict__ jobs, int njobs) {
   __shared__ float tile[32][33];
   // block -> job: the table's block_begin column is fetched by ONE coalesced load into shared memory and searched
   // there (a search over global memory costs ~6 dependent L2 round trips per 4 KB tile)
@@ -736,8 +738,17 @@ __global__ void weight_transpose_multi_k(const vlfb_wt_job_t* __restrict__ jobs,
   __syncthreads();
   for (int r = threadIdx.y; r < 32; r += blockDim.y) {
     const int ci = ci0 + r, co = co0 + threadIdx.x;
-    if (ci < jb.Ci && co < jb.Co) jb.wt[((int64_t)ci * jb.taps + tap) * jb.Co + co] = round_tf32(tile[threadIdx.x][r]);
+    if (ci < jb.Ci && co < jb.Co) {
+      const float v = tile[threadIdx.x][r];
+      jb.wt[((int64_t)ci * jb.taps + tap) * jb.Co + co] = ROUND ? round_tf32(v) : v;
+    }
   }
+}
+__global__ void weight_transpose_multi_k(const vlfb_wt_job_t* __restrict__ jobs, int njobs) {
+  weight_transpose_multi_body<true>(jobs, njobs);
+}
+__global__ void weight_scale_transpose_multi_k(const vlfb_wt_job_t* __restrict__ jobs, int njobs) {
+  weight_transpose_multi_body<false>(jobs, njobs);
 }
 
 // ------------------------------------------------------------------ losses (single block; R*classes is small)
@@ -1125,6 +1136,13 @@ int vlfb_weight_transpose(const float* w, float* wt, const float* scale, int Co,
 int vlfb_weight_transpose_multi(const vlfb_wt_job_t* jobs, int njobs, int total_blocks, void* stream) {
   VLFB_CHECK_ARG(jobs && njobs > 0 && total_blocks > 0);
   launch_k(weight_transpose_multi_k, dim3(total_blocks), dim3(32, 8), 0, ST(stream), jobs, njobs);
+  VLFB_CHECK_LAUNCH();
+  return VLFB_OK;
+}
+
+int vlfb_weight_scale_transpose_multi(const vlfb_wt_job_t* jobs, int njobs, int total_blocks, void* stream) {
+  VLFB_CHECK_ARG(jobs && njobs > 0 && total_blocks > 0);
+  launch_k(weight_scale_transpose_multi_k, dim3(total_blocks), dim3(32, 8), 0, ST(stream), jobs, njobs);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }

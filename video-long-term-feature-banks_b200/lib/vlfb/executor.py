@@ -1096,6 +1096,12 @@ class CompiledNet(object):
         self.model = model
         self.ws = ws
         self.name = model.net.Proto().name
+        # B200.COMPUTE: 'tf32' is the only lowering.  Any other value (the reserved 'fp32' included) is refused rather
+        # than run as TF32: fp32-accuracy products exist per GEMM call (kernels precision=PREC_X3, DESIGN.md 4.7), not yet
+        # as a net-level mode that keeps every tensor of the step unrounded.
+        compute = cfg.B200.get('COMPUTE', 'tf32')
+        if compute != 'tf32':
+            raise VlfbError("%s: B200.COMPUTE = %r is not supported; nets lower with 'tf32' only" % (self.name, compute))
         # read once, when the net is created.  A deterministic net also skips everything the first run's record of
         # gradient contributions (self.contrib) switches on later -- the grad-finish fusion, producer-side rounding of
         # sole gradients -- so that its first eager run computes exactly what every later run and graph replay does, and a

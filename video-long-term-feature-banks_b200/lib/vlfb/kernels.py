@@ -162,7 +162,7 @@ def _run_gemm(p, kind='gemm', flops=None, nbytes=0.0, keep=()):
                          lambda: lib.vlfb_gemm(C.byref(q), st), flops, nbytes, LABEL, keep))
 
 
-def _base_params(M, N, K, d, ldd, alpha=1.0):
+def _base_params(M, N, K, d, ldd, alpha=1.0, precision=L.PREC_TF32):
     p = L.GemmParams()
     p.M, p.N, p.K = int(M), int(N), int(K)
     p.batch, p.taps, p.split_k = 1, 1, 1
@@ -177,7 +177,16 @@ def _base_params(M, N, K, d, ldd, alpha=1.0):
     ws = gemm_workspace(d.device)
     p.workspace = ws.data_ptr()
     p.workspace_bytes = ws.numel() * 4
+    p.precision = _precision(precision)
     return p
+
+
+def _precision(precision):
+    """vlfb_gemm_params_t.precision: L.PREC_TF32 (TF32 products; operands rounded by their producers) or L.PREC_X3 (split
+    TF32: fp32-accuracy products of unrounded operands)."""
+    if precision not in (L.PREC_TF32, L.PREC_X3):
+        raise ValueError('precision must be libvlfb.PREC_TF32 or PREC_X3, not %r' % (precision,))
+    return int(precision)
 
 
 def _set_epilogue(p, scale=None, bias=None, row_scale=None, residual=None, relu=False, tf32=False):
@@ -205,11 +214,13 @@ def _check_groups(g, groups):
     return groups
 
 
-def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_out=False, relu_bits=None, groups=1):
+def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_out=False, relu_bits=None, groups=1,
+             precision=L.PREC_TF32):
     """y = epi(conv(x, w)).  x [N,T,H,W,C], w [Co,kT,kH,kW,C], y [N,To,Ho,Wo,Co];
     epi: *scale[co] + bias[co] (+ residual) (ReLU).  C == 4 selects the stem (conv1) path with
     w [Co,kT,kH,8,4].  relu_bits (int32 [y.numel() / 32], with relu): also the sign bits of y, the mask of the
-    ReLU's backward (conv_dgrad relu_mask_bits).  groups > 1: Caffe2 grouped Conv, w [Co,kT,kH,kW,C/groups]."""
+    ReLU's backward (conv_dgrad relu_mask_bits).  groups > 1: Caffe2 grouped Conv, w [Co,kT,kH,kW,C/groups].
+    precision: vlfb_gemm_params_t.precision of the call (every GEMM wrapper takes it)."""
     _f32c(w, 'w'), _f32c(y, 'y')
     assert tuple(x.shape) == (g.N, g.T, g.H, g.W, g.C) and tuple(y.shape) == out_shape(g)
     M = g.N * g.To * g.Ho * g.Wo
@@ -229,7 +240,7 @@ def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_
         K = g.kT * g.kH * g.kW * g.C
         assert tuple(w.shape) == (g.Co, g.kT, g.kH, g.kW, g.C)
         a = _operand(_f32c(x, 'x'), L.OP_CONV_K)
-    p = _base_params(M, g.Co, K, y, g.Co)
+    p = _base_params(M, g.Co, K, y, g.Co, precision=precision)
     p.a = a
     p.b = _operand(w, L.OP_DENSE_K, ld=K)
     p.g = g
@@ -244,7 +255,7 @@ def conv_fwd(x, w, y, g, scale=None, bias=None, residual=None, relu=False, tf32_
 
 
 def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, tf32_out=False, relu_mask_bits=None,
-               groups=1):
+               groups=1, precision=L.PREC_TF32):
     """dx = finish(conv_transpose(dy, w) [+ dx if accumulate] [+ residual]).  wt [C, kT,kH,kW, Co] (see
     weight_transpose), dx [N,T,H,W,C].  finish = the backward of the ReLU that produced this layer's input
     (relu_mask = that activation, dx zeroed where it is <= 0) and the TF32 rounding the next GEMM needs: when
@@ -264,7 +275,7 @@ def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, t
     else:
         K = g.kT * g.kH * g.kW * g.Co
         a = _operand(dy, L.OP_DGRAD_K)
-    p = _base_params(M, g.C, K, dx, g.C)
+    p = _base_params(M, g.C, K, dx, g.C, precision=precision)
     p.a = a
     p.b = _operand(wt, L.OP_DENSE_K, ld=K)
     p.g = g
@@ -289,20 +300,20 @@ def conv_dgrad(dy, wt, dx, g, accumulate=False, residual=None, relu_mask=None, t
               keep=(dy, wt, dx, residual, relu_mask, relu_mask_bits))
 
 
-def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None, groups=1):
+def conv_wgrad(dy, x, dw, g, row_scale=None, col_mask=None, groups=1, precision=L.PREC_TF32):
     """dw[co,tap,ci] += row_scale[co] * sum_m dy[m,co] * x[gather(m,tap),ci]  (atomic accumulate:
     dw must be zero-initialised or hold a partial sum).  Stem path when C == 4 (dw [Co,kT,kH,8,4],
     col_mask [32] zeroes the padding lanes).  groups > 1: dw [Co,kT,kH,kW,C/groups], ci within co's group."""
-    _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, False)
+    _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, False, precision)
 
 
-def conv_wgrad_det(dy, x, dw, g, row_scale=None, col_mask=None, groups=1):
+def conv_wgrad_det(dy, x, dw, g, row_scale=None, col_mask=None, groups=1, precision=L.PREC_TF32):
     """conv_wgrad with a reproducible sum: every dw element receives one contribution per launch (split 1 or stream-K
     with the workspace fix-up; grouped: partial slabs summed in split order)."""
-    _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, True)
+    _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, True, precision)
 
 
-def _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, det):
+def _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, det, precision):
     _f32c(dy, 'dy'), _f32c(dw, 'dw')
     Kpos = g.N * g.To * g.Ho * g.Wo
     groups = _check_groups(g, groups)
@@ -322,7 +333,7 @@ def _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, det):
     else:
         taps, n = g.kT, g.kH * g.kW * g.C          # one z-slice per temporal tap; N spans (kh, kw, ci)
         b = _operand(_f32c(x, 'x'), L.OP_CONV_MN)
-    p = _base_params(g.Co, n, Kpos, dw, taps * n)
+    p = _base_params(g.Co, n, Kpos, dw, taps * n, precision=precision)
     p.a = _operand(dy, L.OP_DENSE_MN, ld=g.Co)
     p.b = b
     p.g = g
@@ -337,10 +348,15 @@ def _conv_wgrad(dy, x, dw, g, row_scale, col_mask, groups, det):
               _nbytes(dy, x, dw), keep=(dy, x, dw, row_scale, col_mask))
 
 
-def weight_transpose(w, wt, scale=None, groups=1):
-    """wt[ci][tap][co] = w[co][tap][ci] * scale[co].  groups > 1: w [Co][taps][Cig] -> wt [C][taps][Cog], each group's
-    slab transposed on its own (the dgrad B operand of a grouped conv)."""
+def weight_transpose(w, wt, scale=None, groups=1, precision=L.PREC_TF32):
+    """wt[ci][tap][co] = w[co][tap][ci] * scale[co], TF32-rounded (precision = L.PREC_X3: not rounded).  groups > 1:
+    w [Co][taps][Cig] -> wt [C][taps][Cog], each group's slab transposed on its own (the dgrad B operand of a grouped
+    conv).  The PREC_X3 form uploads a one-off job table (a host-to-device copy per call, not allowed during graph
+    capture): a per-step caller keeps its jobs in weight_transpose_multi's persistent cache instead."""
     _f32c(w), _f32c(wt)
+    if _precision(precision) == L.PREC_X3:
+        weight_transpose_multi(grouped_wt_slices(w, wt, scale, groups), {}, precision)
+        return
     for w_, wt_, s_ in grouped_wt_slices(w, wt, scale, groups):
         co, ci = w_.shape[0], w_.shape[-1]
         taps = w_.numel() // (co * ci)
@@ -383,23 +399,24 @@ def _mat_operand(t, rows_dim, k_dim):
                      % (tuple(t.shape), tuple(t.stride())))
 
 
-def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32_optional=False):
+def matmul(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32_optional=False, precision=L.PREC_TF32):
     """d[i] (+)= alpha * a[i] @ b[i] (+ bias[n]) for 3-D strided views a (B,M,K), b (B,K,N), d (B,M,N).
     Each matrix needs unit stride along one of its two dims (16-byte aligned rows).  Returns whether d was stored
     TF32-rounded: with `tf32_optional` a product that qualifies for split-K (atomic accumulation cannot round) keeps
     the split and leaves the rounding to the consumer -- the split is worth 2x on the K = 3136 non-local gradient
     products."""
-    return _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, False)
+    return _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, False, precision)
 
 
-def matmul_det(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32_optional=False):
+def matmul_det(a, b, d, alpha=1.0, accumulate=False, bias=None, tf32_out=False, tf32_optional=False,
+               precision=L.PREC_TF32):
     """matmul with a reproducible sum: the long-K products that matmul splits over atomics run as one deterministic
     launch (split 1 or stream-K with the workspace fix-up).  Every element gets one contribution onto a zeroed d, so the
     TF32 rounding is kept (tf32_optional changes nothing) unless d is accumulated."""
-    return _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, True)
+    return _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, True, precision)
 
 
-def _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, det):
+def _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, det, precision):
     assert a.dim() == 3 and b.dim() == 3 and d.dim() == 3
     Bt, M, K = a.shape
     N = b.shape[2]
@@ -409,10 +426,10 @@ def _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, det):
         assert _dim_ok(d.stride(1), M), 'matmul output needs a unit stride'
         assert bias is None
         return _matmul(b.transpose(1, 2), a.transpose(1, 2), d.transpose(1, 2), alpha, accumulate, None, tf32_out,
-                       tf32_optional, det)
+                       tf32_optional, det, precision)
     ka, lda, sba = _mat_operand(a, 1, 2)
     kb, ldb, sbb = _mat_operand(b, 2, 1)
-    p = _base_params(M, N, K, d, d.stride(1) if M > 1 else N, alpha)
+    p = _base_params(M, N, K, d, d.stride(1) if M > 1 else N, alpha, precision)
     p.a = _operand(a, ka, lda, sba)
     p.b = _operand(b, kb, ldb, sbb)
     p.batch = Bt
@@ -448,9 +465,10 @@ def _matmul(a, b, d, alpha, accumulate, bias, tf32_out, tf32_optional, det):
     return bool(tf32_out)
 
 
-def weight_transpose_multi(jobs, cache):
-    """jobs = [(w, wt, scale_or_None)]: every dgrad weight operand of the step in one launch.  The device job
-    table is built once and kept in `cache` (all addresses are static: parameters and persistent wt buffers)."""
+def weight_transpose_multi(jobs, cache, precision=L.PREC_TF32):
+    """jobs = [(w, wt, scale_or_None)]: every dgrad weight operand of the step in one launch, TF32-rounded (precision =
+    L.PREC_X3: unrounded, vlfb_weight_scale_transpose_multi).  The device job table is built once and kept in `cache`
+    (all addresses are static: parameters and persistent wt buffers)."""
     import numpy as np
     key = tuple((w.data_ptr(), wt.data_ptr(), 0 if s is None else s.data_ptr()) for w, wt, s in jobs)
     if cache.get('key') != key:
@@ -468,8 +486,12 @@ def weight_transpose_multi(jobs, cache):
         cache['table'] = torch.from_numpy(tab.view(np.uint8).copy()).to(jobs[0][0].device)
         cache['blocks'] = blocks
         cache['key'] = key
-    _check(L.load().vlfb_weight_transpose_multi(_ptr(cache['table']), len(jobs), cache['blocks'], _stream()),
-           'weight_transpose_multi')
+    if _precision(precision) == L.PREC_X3:
+        _check(L.load().vlfb_weight_scale_transpose_multi(_ptr(cache['table']), len(jobs), cache['blocks'], _stream()),
+               'weight_scale_transpose_multi')
+    else:
+        _check(L.load().vlfb_weight_transpose_multi(_ptr(cache['table']), len(jobs), cache['blocks'], _stream()),
+               'weight_transpose_multi')
 
 
 # --------------------------------------------------------------------------- streaming ops

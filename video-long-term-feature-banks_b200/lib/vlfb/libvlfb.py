@@ -34,7 +34,7 @@ class GemmParams(C.Structure):
                 ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t),
                 ('engine', C.c_int), ('tile_n', C.c_int), ('pair', C.c_int), ('stream_k', C.c_int),
                 ('relu_mask_bits', C.c_void_p), ('relu_bits_out', C.c_void_p), ('groups', C.c_int),
-                ('deterministic', C.c_int)]
+                ('deterministic', C.c_int), ('precision', C.c_int)]
 
 
 class GemmPlan(C.Structure):
@@ -42,6 +42,7 @@ class GemmPlan(C.Structure):
 
 
 ENGINE_TCGEN05, ENGINE_SIMT = 0, 1
+PREC_TF32, PREC_X3 = 0, 1           # vlfb_gemm_params_t.precision
 DT_F32, DT_BF16 = 0, 1              # vlfb_dtype_t
 
 
@@ -138,6 +139,10 @@ LIVE_SIGNATURES = {
     'vlfb_roi_align_bwd_det_live': [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _I, _P, C.c_size_t, _P, _P],
     'vlfb_fbo_bank_scan_live': [_P, _I, _P, _F, _P, _P, _I, _I, _I, _I, _P, C.c_size_t, _P, _P],
 }
+# include/vlfb_prec.h (included by vlfb.h): the split-TF32 precision's unrounded dgrad weight operand
+PREC_SIGNATURES = {
+    'vlfb_weight_scale_transpose_multi': [_P, _I, _I, _P],
+}
 RESTYPES = {'vlfb_last_error': C.c_char_p, 'vlfb_roi_align_bwd_det_scratch_bytes': C.c_size_t, 'vlfb_fbo_bank_scan_workspace': C.c_size_t,
             'vlfb_fbo_bank_scan_workspace_dt': C.c_size_t,
             'vlfb_fbo_nl_scratch_floats': C.c_size_t,
@@ -156,7 +161,8 @@ def load():
             'libvlfb.so not found at %s -- build it first (python -c "import __graft_entry__ as g; '
             'g.build()" or make -C csrc).  There is no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, argtypes in list(SIGNATURES.items()) + list(DET_SIGNATURES.items()) + list(LIVE_SIGNATURES.items()):
+    for name, argtypes in list(SIGNATURES.items()) + list(DET_SIGNATURES.items()) + list(LIVE_SIGNATURES.items()) + \
+            list(PREC_SIGNATURES.items()):
         fn = getattr(lib, name)        # AttributeError if the symbol is missing
         fn.argtypes = argtypes
         fn.restype = RESTYPES.get(name, C.c_int)
