@@ -99,8 +99,10 @@ __C = _tree({
     'IMG_LOAD_RETRY': 10,
     'GET_TRAIN_LFB': False,
     # ---- additions of this implementation (not in the reference) -------------
-    # B200.COMPUTE: 'tf32' = parity mode (fp32 storage, tensor-core tf32 MMA, fp32 accumulate), the only value CreateNet
-    #   accepts (any other raises VlfbError).
+    # B200.COMPUTE: 'tf32' = parity mode (fp32 storage, GEMM operands rounded to TF32 where they are produced, tensor-core
+    #   tf32 MMA, fp32 accumulate); 'tf32x3' = nothing rounded, every tensor-core GEMM on split-TF32 products (3xTF32,
+    #   about 2x the step time; DESIGN.md 4.7).  Any other value raises VlfbError: 'fp32' is reserved for a mode whose
+    #   products are fp32 FMAs, which split-TF32 products are not.
     # B200.FBO_FOLD: inference nets run each FBO-NL layer as one pass over the raw bank (vlfb.executor.FboFoldStep).
     # B200.LFB_DTYPE: 'f32' | 'bf16' = storage type of the feature-bank windows the folded inference FBO scans (a bf16
     #   copy is made when the bank is fed; scores / softmax / sums stay fp32; parity tolerance 1e-2 instead of 1e-3).

@@ -166,7 +166,8 @@ class DeviceLfb(object):
 
     def feed(self, blob_name, index_table):
         """Assemble the windows directly into the net's `lfb{suffix}` input blob (what FeedBlob(name, windows) would
-        have produced, TF32 rounding of the GEMM operand included) -- R*L*4 bytes cross PCIe instead of R*L*dim*4.
+        have produced, TF32 rounding of the GEMM operand included unless a B200.COMPUTE 'tf32x3' net reads it) -- R*L*4
+        bytes cross PCIe instead of R*L*dim*4.
         In a B200.ROI_CAPACITY net the table is extended to C rows with -1 (zero windows), as FeedBlob pads."""
         from vlfb import workspace
         name = workspace._unscoped(blob_name)
@@ -178,11 +179,12 @@ class DeviceLfb(object):
             index_table = table
         shape = tuple(np.shape(index_table)) + (self.dim,)
         dst = workspace._static(name, shape, self.bank.dtype)
-        self.gather(index_table, out=dst, tf32_out=True)
+        rnd = not workspace.feeds_unrounded(name)
+        self.gather(index_table, out=dst, tf32_out=rnd)
         workspace.bank_companion(name, dst)                  # B200.LFB_DTYPE 'bf16': the scan operand of the folded FBO
         if cap is not None:
             workspace.set_live_rows(name, rows)
         ws = workspace.current()
         ws.blobs[name] = dst
-        ws.rounded.add(name)
+        workspace._mark_rounded(name, rnd)
         return dst

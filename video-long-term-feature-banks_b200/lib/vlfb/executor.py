@@ -11,15 +11,18 @@ Representation
     epilogue (the reference runs 3-4 kernels, model_builder_video.py:211-219,
     resnet_helper.py:112-117); Scale -> Softmax likewise;
   * every tensor that feeds a tensor-core GEMM is rounded to TF32 (round-to-nearest) by its
-    producer, because kind::tf32 MMAs truncate fp32 operands.
+    producer, because kind::tf32 MMAs truncate fp32 operands -- except in a B200.COMPUTE 'tf32x3' net, whose GEMMs
+    multiply unrounded fp32 operands with split-TF32 products (precision=PREC_X3) and which rounds nothing.
 """
 import collections
+import functools
 import math
 import os
 
 import torch
 
 from . import kernels as K_default
+from . import libvlfb as L
 from .libvlfb import VlfbError
 
 K = K_default          # tests may swap in a torch-CPU kernel set (tests/fake_kernels.py)
@@ -38,11 +41,13 @@ RELU_BITS = os.environ.get('VLFB_RELU_BITS', '1') == '1'
 POOL_GATHER = int(os.environ.get('VLFB_POOL_GATHER', '1'))     # 2 = gather form only for non-overlapping windows
 # the per-RoI inputs of an AVA net (model_builder_video.py), suffixed like 'proposals{sfx}': B200.ROI_CAPACITY buffers
 ROI_INPUTS = ('proposals', 'labels', 'original_boxes', 'metadata', 'lfb')
+COMPUTE_MODES = ('tf32', 'tf32x3')     # B200.COMPUTE values CreateNet accepts
 
 
 def _mm(ctx):
-    """The matmul of this net: the deterministic form in a B200.DETERMINISTIC net."""
-    return K.matmul_det if ctx.net.det else K.matmul
+    """The matmul of this net: the deterministic form in a B200.DETERMINISTIC net, split-TF32 in a 'tf32x3' net."""
+    mm = K.matmul_det if ctx.net.det else K.matmul
+    return functools.partial(mm, **ctx.prec) if ctx.prec else mm
 
 
 def _live_kw(ctx, blob):
@@ -151,6 +156,10 @@ class Ctx(object):
         # residual branch).  A conv that owns `key` folds the sum into its ReLU-backward / rounding pass.
         self.pending = {}
         self.bound = {}          # blob name -> rounded flag of everything this run bound (re-installed after a graph replay)
+        # B200.COMPUTE: `tf32` = GEMM operands are TF32-rounded where they are produced; False in a 'tf32x3' net, whose
+        # GEMM calls all carry `prec` (precision=PREC_X3) and whose tensors are never rounded
+        self.tf32 = not net.x3
+        self.prec = {'precision': L.PREC_X3} if net.x3 else {}
 
     # ---- blobs
     def get(self, name):
@@ -165,13 +174,19 @@ class Ctx(object):
             self.ws.rounded.discard(name)
 
     def rounded(self, name):
-        """TF32-rounded version of blob `name` (GEMM operand)."""
+        """Blob `name` as a GEMM operand: TF32-rounded (a parameter's Pt copy), or the blob itself in a 'tf32x3' net."""
+        if not self.tf32:
+            return self.ws.params.phys(name) if self.ws.params.has(name) else self.ws.blobs[name]
         t = self.ws.blobs[name]
         if name in self.ws.rounded or self.ws.params.has(name):
             return self.ws.params.tf32(name) if self.ws.params.has(name) else t
         r = empty_like_strided(t)
         K.round_tf32(flat(t), flat(r))
         return r
+
+    def weight(self, name):
+        """Parameter `name` as a GEMM operand: its TF32-rounded copy Pt, or the fp32 master P in a 'tf32x3' net."""
+        return self.ws.params.tf32(name) if self.tf32 else self.ws.params.phys(name)
 
     # ---- grads
     def is_last_contribution(self, key):
@@ -190,7 +205,7 @@ class Ctx(object):
         that consumes this gradient -- the blob's producer, through views -- feeds it to GEMMs, i.e. would round it to
         TF32 anyway: the kernel that computes the gradient then stores it rounded, and the consumer's copy + rounding
         passes disappear.  (A pooling / ReLU / LayerNorm backward keeps receiving the unrounded fp32 values.)"""
-        if self.net.contrib is None or self.net.det:
+        if self.net.contrib is None or self.net.det or not self.tf32:
             return False
         while True:
             if self.net.contrib.get(key) != 1:
@@ -236,7 +251,15 @@ class Ctx(object):
 
     def pop_grad_finished(self, key, y):
         """Gradient of a conv output, ready to be a GEMM operand: summed, masked by the conv's ReLU (y = its
-        output, or None) and TF32-rounded -- in one pass when a deferred sum is pending."""
+        output, or None) and TF32-rounded -- in one pass when a deferred sum is pending.  A 'tf32x3' net sums and masks
+        only."""
+        if not self.tf32:
+            if y is None:
+                return self.pop_grad(key)             # read-only operand: nothing to mask or round
+            g = self.pop_grad_owned(key)
+            if g is not None:
+                K.relu_bwd(flat(g), flat(y), flat(g))
+            return g
         pend = self.pending.pop(key, None)
         if pend is None:
             if y is None and key in self.grad_rounded:
@@ -309,7 +332,7 @@ class ConvStep(Step):
         x = ctx.rounded(self.x)
         xp = as5d(phys(x))
         g = self._geom(ctx, xp)
-        w = ctx.ws.params.tf32(self.w)
+        w = ctx.weight(self.w)
         y = cl_alloc((g.N, g.Co, g.To, g.Ho, g.Wo))
         scale = bias = None
         if self.affine:
@@ -329,10 +352,11 @@ class ConvStep(Step):
             # sign bits of the ReLU output: the backward mask the consumer's dgrad epilogue reads (1/32 of the bytes)
             bits = empty((y.numel() // 32,), torch.int32)
             ctx.relu_bits[self.out_keys[0]] = bits
-        K.conv_fwd(xp, w, phys(y), g, scale=scale, bias=bias, residual=res, relu=self.relu, tf32_out=self.round_out,
-                   relu_bits=bits, **self.gkw)
+        round_out = self.round_out and ctx.tf32
+        K.conv_fwd(xp, w, phys(y), g, scale=scale, bias=bias, residual=res, relu=self.relu, tf32_out=round_out,
+                   relu_bits=bits, **self.gkw, **ctx.prec)
         ctx.saved[id(self)] = (xp, g)
-        ctx.put(self.out, y, rounded=self.round_out)
+        ctx.put(self.out, y, rounded=round_out)
 
     def bwd(self, ctx):
         # the gradient is a GEMM operand of dgrad/wgrad: mask (ReLU) and round it to TF32 in one pass
@@ -350,13 +374,13 @@ class ConvStep(Step):
             xp, g = ctx.saved.pop(id(self))
             gp = as5d(phys(gy))
         if self.res_key is not None:
-            ctx.add_grad(self.res_key, gy, owned=False, rounded=True)       # gy is masked + rounded already
+            ctx.add_grad(self.res_key, gy, owned=False, rounded=ctx.tf32)       # gy is masked (+ rounded) already
         scale = ctx.ws.params.phys(self.affine[0]) if self.affine else None
         store = ctx.ws.params
         if store.trainable(self.w):
             mask = store.stem_mask() if g.C == 4 else None
             wgrad = K.conv_wgrad_det if ctx.net.det else K.conv_wgrad
-            wgrad(gp, xp, store.grad(self.w), g, row_scale=scale, col_mask=mask, **self.gkw)
+            wgrad(gp, xp, store.grad(self.w), g, row_scale=scale, col_mask=mask, **self.gkw, **ctx.prec)
         if self.b and store.trainable(self.b):
             db = store.grad(self.b)
             rows = gp.numel() // g.Co
@@ -374,6 +398,8 @@ class ConvStep(Step):
             taps = g.kT * g.kH * g.kW
             wt = ctx.net.wt_buffers.get(id(self))                 # filled for all convs by one launch (_prepare_wt)
             if wt is None:
+                # (a 'tf32x3' net must not get here: the unrounded transpose uploads a job table per call)
+                assert ctx.tf32, 'tf32x3: dgrad weight operand of %s missing from _prepare_wt' % self.out
                 wt = empty((g.C, taps, g.Co // self.groups))
                 K.weight_transpose(store.phys(self.w), wt, scale, **self.gkw)     # wt = round_tf32(w * s)
             cur = ctx.grads.get(xkey)
@@ -382,7 +408,8 @@ class ConvStep(Step):
                     and (cur is None or (is_cl(cur) and as5d(phys(cur)).shape == xp.shape))):
                 # Last contribution to the gradient of a conv output: sum the earlier contributions, apply that
                 # conv's ReLU backward (mask = its output = our input xp) and the TF32 rounding its own
-                # dgrad / wgrad GEMMs need -- all in this GEMM's epilogue (saves ~6 passes over the tensor).
+                # dgrad / wgrad GEMMs need (none in a 'tf32x3' net) -- all in this GEMM's epilogue (saves ~6 passes
+                # over the tensor).
                 mask = xp if prod.relu else None
                 mbits = ctx.relu_bits.get(xkey) if prod.relu else None
                 if mbits is not None:
@@ -390,23 +417,23 @@ class ConvStep(Step):
                 ctx._settle(xkey)                 # a deferred sum must be complete before the gradient is finalised
                 if cur is not None and ctx.owned.get(xkey, False):
                     dx = cur
-                    K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, relu_mask=mask, relu_mask_bits=mbits, tf32_out=True,
-                                 **self.gkw)
+                    K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, relu_mask=mask, relu_mask_bits=mbits,
+                                 tf32_out=ctx.tf32, **self.gkw, **ctx.prec)
                 else:
                     dx = cl_alloc((g.N, g.C, g.T, g.H, g.W))
                     if dx.shape != ctx.get(self.x).shape:
                         dx = dx.view(ctx.get(self.x).shape)
                     K.conv_dgrad(gp, wt, as5d(phys(dx)), g, residual=None if cur is None else as5d(phys(cur)),
-                                 relu_mask=mask, relu_mask_bits=mbits, tf32_out=True, **self.gkw)
+                                 relu_mask=mask, relu_mask_bits=mbits, tf32_out=ctx.tf32, **self.gkw, **ctx.prec)
                 ctx.set_final_grad(xkey, dx)
                 STATS['fused_grad_finish'] += 1
             elif cur is not None and ctx.owned.get(xkey, False):
                 ctx.counts[xkey] = ctx.counts.get(xkey, 0) + 1
-                K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, **self.gkw)
+                K.conv_dgrad(gp, wt, as5d(phys(cur)), g, accumulate=True, **self.gkw, **ctx.prec)
             else:
                 dx = cl_alloc((g.N, g.C, g.T, g.H, g.W))
                 sole = ctx.sole(xkey)
-                K.conv_dgrad(gp, wt, phys(dx), g, accumulate=False, tf32_out=sole, **self.gkw)
+                K.conv_dgrad(gp, wt, phys(dx), g, accumulate=False, tf32_out=sole, **self.gkw, **ctx.prec)
                 ctx.add_grad(xkey, dx.view(ctx.get(self.x).shape) if dx.shape != ctx.get(self.x).shape else dx,
                              owned=True, rounded=sole)
 
@@ -484,8 +511,8 @@ class ReluStep(Step):
     def fwd(self, ctx):
         x = ctx.get(self.op.inputs[0])
         y = x if self.op.outputs[0] == self.op.inputs[0] else empty_like_strided(x)
-        K.relu_tf32(flat(x), flat(y))
-        ctx.put(self.op.outputs[0], y, rounded=True)
+        (K.relu_tf32 if ctx.tf32 else K.relu_fwd)(flat(x), flat(y))
+        ctx.put(self.op.outputs[0], y, rounded=ctx.tf32)
 
     def bwd(self, ctx):
         gy = ctx.pop_grad_owned(self.out_keys[0])
@@ -500,8 +527,11 @@ class SumStep(Step):
         ins = [ctx.get(n) for n in self.op.inputs]
         assert len(ins) == 2 and ins[0].shape == ins[1].shape and ins[0].stride() == ins[1].stride()
         y = ins[0] if self.op.outputs[0] == self.op.inputs[0] else empty_like_strided(ins[0])
-        K.add_tf32(flat(ins[0]), flat(ins[1]), flat(y))
-        ctx.put(self.op.outputs[0], y, rounded=True)
+        if ctx.tf32:
+            K.add_tf32(flat(ins[0]), flat(ins[1]), flat(y))
+        else:
+            K.axpby(flat(ins[0]), 1.0, flat(ins[1]), 1.0, flat(y))
+        ctx.put(self.op.outputs[0], y, rounded=ctx.tf32)
 
     def bwd(self, ctx):
         gy = ctx.pop_grad(self.out_keys[0])
@@ -539,8 +569,8 @@ class SoftmaxStep(Step):
         x = ctx.get(self.src)
         assert x.is_contiguous() and self.op.args.get('axis', 1) == x.dim() - 1
         p = empty(x.shape)
-        K.softmax_fwd(x, p, self.scale, tf32_out=True)
-        ctx.put(self.op.outputs[0], p, rounded=True)
+        K.softmax_fwd(x, p, self.scale, tf32_out=ctx.tf32)
+        ctx.put(self.op.outputs[0], p, rounded=ctx.tf32)
 
     def bwd(self, ctx):
         gp = ctx.pop_grad(self.out_keys[0])
@@ -606,7 +636,7 @@ class PoolStep(Step):
             prod = ctx.net.producer.get(xkey)
             fuse = (FUSE_GRAD_FINISH and not ctx.net.det and isinstance(prod, ConvStep) and prod.relu and ctx.net.contrib is not None
                     and ctx.net.contrib.get(xkey) == 1)
-            K.maxpool_bwd_gather(gp, arg, yp if fuse else None, as5d(phys(dx)), g, tf32_out=fuse)
+            K.maxpool_bwd_gather(gp, arg, yp if fuse else None, as5d(phys(dx)), g, tf32_out=fuse and ctx.tf32)
             if fuse:
                 ctx.set_final_grad(xkey, dx)
                 STATS['fused_grad_finish'] += 1
@@ -701,13 +731,15 @@ class BatchMatMulStep(Step):
             d = empty((Bt, N, M)).transpose(1, 2)
         else:
             d = empty((Bt, M, N))
-        _mm(ctx)(A, B, d, tf32_out=True)
+        _mm(ctx)(A, B, d, tf32_out=ctx.tf32)
         ctx.saved[id(self)] = (a, b)
-        ctx.put(self.op.outputs[0], d, rounded=True)
+        ctx.put(self.op.outputs[0], d, rounded=ctx.tf32)
 
     def bwd(self, ctx):
-        if self.out_keys[0] in ctx.grad_rounded:
-            g = ctx.pop_grad(self.out_keys[0])       # stored rounded by its producer: a read-only operand
+        if self.out_keys[0] in ctx.grad_rounded or not ctx.tf32:
+            g = ctx.pop_grad(self.out_keys[0])       # stored rounded by its producer ('tf32x3': unrounded): read-only
+            if g is None:
+                return
         else:
             g = ctx.pop_grad_owned(self.out_keys[0])
             if g is None:
@@ -756,26 +788,26 @@ class FboFoldStep(Step):
         b16 = self._bf16_bank(ctx)
         if b16 is not None and tuple(b16.shape) == (R, L_, D):
             bank = b16                                          # B200.LFB_DTYPE 'bf16': half the bytes per pass
-        w1 = P.tf32(self.w1).view(1, -1, D)                     # [d1][D]
+        w1 = ctx.weight(self.w1).view(1, -1, D)                 # [d1][D]
         d1 = int(w1.shape[1])
-        wphi = P.tf32(self.wphi).view(1, d, d1)                 # [d][d1]
-        wg = P.tf32(self.wg).view(1, -1, d1)                    # [dg][d1]
+        wphi = ctx.weight(self.wphi).view(1, d, d1)             # [d][d1]
+        wg = ctx.weight(self.wg).view(1, -1, d1)                # [dg][d1]
         dg = int(wg.shape[1])
         u = empty((1, R, d1))
-        _mm(ctx)(flat(theta).view(1, R, d), wphi, u, tf32_out=True)
+        _mm(ctx)(flat(theta).view(1, R, d), wphi, u, tf32_out=ctx.tf32)
         q = empty((1, R, D))
         _mm(ctx)(u, w1, q)
         s = empty((R, D))
         prob = empty((R, L_)) if self.prob_name else None
-        K.fbo_bank_scan(bank, q.view(R, D), s, self.scale, prob=prob, tf32_out=True, **_live_kw(ctx, self.theta))
+        K.fbo_bank_scan(bank, q.view(R, D), s, self.scale, prob=prob, tf32_out=ctx.tf32, **_live_kw(ctx, self.theta))
         t = empty((1, R, d1))
         _mm(ctx)(s.view(1, R, D), w1.transpose(1, 2), t, bias=None if self.b1 is None else P.phys(self.b1),
-                 tf32_out=True)
+                 tf32_out=ctx.tf32)
         y = empty((1, R, dg))
-        _mm(ctx)(t, wg.transpose(1, 2), y, bias=None if self.bg is None else P.phys(self.bg), tf32_out=True)
+        _mm(ctx)(t, wg.transpose(1, 2), y, bias=None if self.bg is None else P.phys(self.bg), tf32_out=ctx.tf32)
         if prob is not None:
             ctx.put(self.prob_name, prob.view(R, 1, L_))
-        ctx.put(self.op.outputs[0], y.view(R, dg, 1), rounded=True)
+        ctx.put(self.op.outputs[0], y.view(R, dg, 1), rounded=ctx.tf32)
 
     def _bf16_bank(self, ctx):
         """The bf16 copy of the bank made when it was fed (workspace.bank_companion), found through the view chain
@@ -948,7 +980,7 @@ class FCStep(Step):
     def fwd(self, ctx):
         x = ctx.rounded(self.op.inputs[0])
         x2 = flat(x).view(x.shape[0], -1)
-        w = ctx.ws.params.tf32(self.op.inputs[1])
+        w = ctx.weight(self.op.inputs[1])
         b = ctx.ws.params.phys(self.op.inputs[2])
         y = empty((x2.shape[0], w.shape[0]))
         _mm(ctx)(x2.unsqueeze(0), w.t().unsqueeze(0), y.unsqueeze(0), bias=b)
@@ -956,10 +988,11 @@ class FCStep(Step):
         ctx.put(self.op.outputs[0], y)
 
     def bwd(self, ctx):
-        gy = ctx.pop_grad_owned(self.out_keys[0])
+        gy = ctx.pop_grad_owned(self.out_keys[0]) if ctx.tf32 else ctx.pop_grad(self.out_keys[0])
         if gy is None:
             return
-        K.round_tf32(flat(gy), flat(gy))
+        if ctx.tf32:
+            K.round_tf32(flat(gy), flat(gy))
         x2, xshape, xstride = ctx.saved.pop(id(self))
         store = ctx.ws.params
         wname, bname = self.op.inputs[1], self.op.inputs[2]
@@ -970,7 +1003,7 @@ class FCStep(Step):
             colsum(gy, gy.shape[1], store.grad(bname), gy.shape[0], gy.shape[1], accumulate=True)
         if ctx.net.requires.get(self.in_keys[0], False):
             dx = torch.empty_strided(xshape, xstride, dtype=DTYPE, device=DEVICE)
-            _mm(ctx)(gy.unsqueeze(0), store.tf32(wname).unsqueeze(0), flat(dx).view(1, x2.shape[0], -1))
+            _mm(ctx)(gy.unsqueeze(0), ctx.weight(wname).unsqueeze(0), flat(dx).view(1, x2.shape[0], -1))
             ctx.add_grad(self.in_keys[0], dx, owned=True)
 
 
@@ -1096,12 +1129,18 @@ class CompiledNet(object):
         self.model = model
         self.ws = ws
         self.name = model.net.Proto().name
-        # B200.COMPUTE: 'tf32' is the only lowering.  Any other value (the reserved 'fp32' included) is refused rather
-        # than run as TF32: fp32-accuracy products exist per GEMM call (kernels precision=PREC_X3, DESIGN.md 4.7), not yet
-        # as a net-level mode that keeps every tensor of the step unrounded.
+        # B200.COMPUTE, read once, when the net is created: 'tf32' rounds every GEMM operand to TF32 where it is produced;
+        # 'tf32x3' rounds nothing and runs every tensor-core GEMM with split-TF32 products (precision=PREC_X3, DESIGN.md
+        # 4.7).  Any other value (the reserved 'fp32' included) is refused rather than run as one of these.
         compute = cfg.B200.get('COMPUTE', 'tf32')
-        if compute != 'tf32':
-            raise VlfbError("%s: B200.COMPUTE = %r is not supported; nets lower with 'tf32' only" % (self.name, compute))
+        if compute not in COMPUTE_MODES:
+            raise VlfbError("%s: B200.COMPUTE = %r is not supported; nets lower with %s" % (
+                self.name, compute, ' or '.join(repr(m) for m in COMPUTE_MODES)))
+        self.compute = compute
+        self.x3 = compute == 'tf32x3'
+        if self.x3 and cfg.B200.get('LFB_DTYPE', 'f32') == 'bf16':
+            raise VlfbError("%s: B200.COMPUTE = 'tf32x3' with B200.LFB_DTYPE = 'bf16': a bf16 feature bank would undo the "
+                            "fp32 accuracy the mode computes at" % self.name)
         # read once, when the net is created.  A deterministic net also skips everything the first run's record of
         # gradient contributions (self.contrib) switches on later -- the grad-finish fusion, producer-side rounding of
         # sole gradients -- so that its first eager run computes exactly what every later run and graph replay does, and a
@@ -1154,6 +1193,31 @@ class CompiledNet(object):
         self._graphs = collections.OrderedDict()     # input signature -> captured step (LRU)
         self._eager_runs = {}                        # input signature -> eager runs so far (two before capture)
         self._setup_roi_capacity(int(cfg.B200.get('ROI_CAPACITY', 0)), ops)
+        self._register_inputs(ops)
+
+    # ---- B200.COMPUTE of the fed inputs
+    def _register_inputs(self, ops):
+        """Register this net's float external inputs with the workspace under its compute mode: feeds of the names a
+        'tf32x3' net reads are stored unrounded (workspace._feed_activation, DeviceLfb.feed).  A name registered by a net
+        of the other mode is refused: one stored copy cannot be both TF32-rounded and unrounded."""
+        targets = set(op.inputs[1] for op in ops if op.type in ('SigmoidCrossEntropyLoss', 'SoftmaxWithLoss'))
+        self.float_inputs = [n for n in self.external_inputs if n not in targets]
+        if self.ws is None:
+            return                                            # the builder's gradient analysis (data_parallel.py)
+        for n in self.float_inputs:
+            other = self.ws.input_compute.get(n)
+            if other is not None and other[0] != self.compute:
+                raise VlfbError("%s: input %s is read by net %s with B200.COMPUTE = %r; net %s cannot read it with %r"
+                                % (self.name, n, other[1], other[0], self.name, self.compute))
+        for n in self.float_inputs:
+            self.ws.input_compute[n] = (self.compute, self.name)
+
+    def _check_unrounded_inputs(self):
+        """A 'tf32x3' net must not read an input that was stored TF32-rounded (fed before the net was created)."""
+        for n in self.float_inputs:
+            if n in self.ws.rounded:
+                raise VlfbError("%s: input %s holds TF32-rounded values (fed before B200.COMPUTE = 'tf32x3' net %s was "
+                                "created?); feed it again" % (self.name, n, self.name))
 
     # ---- B200.ROI_CAPACITY (DESIGN.md 4.6)
     def _setup_roi_capacity(self, cap, ops):
@@ -1462,7 +1526,7 @@ class CompiledNet(object):
         return ws.reducer
 
     def _prepare_wt(self, ctx):
-        """Transposed, affine-scaled, TF32-rounded weights of every conv whose input needs a gradient: persistent
+        """Transposed, affine-scaled, TF32-rounded ('tf32x3': unrounded) weights of every conv whose input needs a gradient: persistent
         buffers (static addresses -> one device job table) filled by ONE launch per step instead of one per conv."""
         if self._wt_jobs is None:
             store = self.ws.params
@@ -1472,7 +1536,7 @@ class CompiledNet(object):
                         any(self.requires.get(k, False) for k in st.out_keys):
                     w = store.phys(st.w)
                     co, ci = w.shape[0], w.shape[-1]
-                    if ci == 4:
+                    if ci == 4 and st.groups == 1:
                         continue                                # the stem never propagates a gradient
                     taps = w.numel() // (co * ci)
                     wt = empty((ci * st.groups, taps, co // st.groups))      # grouped: [C][taps][Cog], one job per group
@@ -1480,7 +1544,7 @@ class CompiledNet(object):
                     jobs.extend(K_default.grouped_wt_slices(w, wt, store.phys(st.affine[0]) if st.affine else None, st.groups))
             self._wt_jobs = jobs
         if self._wt_jobs:
-            K.weight_transpose_multi(self._wt_jobs, self._wt_cache)
+            K.weight_transpose_multi(self._wt_jobs, self._wt_cache, **ctx.prec)
 
     MAX_GRAPHS = 4          # captured steps kept per net (each owns its activation memory): LRU over input signatures
 
@@ -1494,6 +1558,8 @@ class CompiledNet(object):
         if self.roi_capacity:
             self._check_roi_rows()
             ws.roi_blobs.update(self._roi_marks)        # names shared with another net (train / test) are this net's now
+        if self.x3:
+            self._check_unrounded_inputs()
         ws.begin_run()
         if self.det:
             # every run draws the dropout offsets its first run drew, as a graph replay does (the step counter varies

@@ -224,6 +224,9 @@ class Workspace(object):
         self.roi_blobs = {}
         self.roi_live = {}
         self.roi_fed = {}
+        # B200.COMPUTE: float input name -> (compute mode, net name) of the nets that read it (executor.CompiledNet
+        # _register_inputs); inputs of 'tf32x3' nets are stored unrounded
+        self.input_compute = {}
 
     def begin_run(self):
         """Advance the device-side step counter (dropout masks of captured graphs depend on it)."""
@@ -449,8 +452,14 @@ def _input_buffer(name, src, dtype):
     return dst
 
 
+def feeds_unrounded(name):
+    """True when input `name` is read by B200.COMPUTE 'tf32x3' nets: its feeds are stored without the TF32 rounding."""
+    return _ws.input_compute.get(name, ('tf32',))[0] == 'tf32x3'
+
+
 def _feed_activation(name, arr):
     src = arr if isinstance(arr, torch.Tensor) else torch.as_tensor(np.ascontiguousarray(arr))
+    rnd = not feeds_unrounded(name)
     if src.dtype in _INT_DTYPES:
         dst = _input_buffer(name, src, torch.int32)
         _ws.blobs[name] = dst
@@ -476,23 +485,30 @@ def _feed_activation(name, arr):
             if buf is None or tuple(buf.shape) != (n, t_, h_, pitch, cpad):
                 buf = torch.zeros((n, t_, h_, pitch, cpad), dtype=X.DTYPE, device=X.DEVICE)     # pads stay zero
                 _ws.input_cache[key] = buf
-            X.K.nc_to_cl(stage, buf, n, c, inner, cpad, tf32_out=True, width=w_, pitch=pitch, left=STEM_PAD_L)
+            X.K.nc_to_cl(stage, buf, n, c, inner, cpad, tf32_out=rnd, width=w_, pitch=pitch, left=STEM_PAD_L)
             _ws.blobs[name] = buf[:, :, :, STEM_PAD_L:STEM_PAD_L + w_, :].permute(0, 4, 1, 2, 3)
-            _ws.rounded.add(name)
+            _mark_rounded(name, rnd)
             return
         p = _static(name, (n, t_, h_, w_, cpad), X.DTYPE)
-        X.K.nc_to_cl(stage, p, n, c, inner, cpad, tf32_out=True)  # reference NCTHW blob -> NDHWC (+pad 3->4), TF32-rounded
+        X.K.nc_to_cl(stage, p, n, c, inner, cpad, tf32_out=rnd)   # reference NCTHW blob -> NDHWC (+pad 3->4), TF32-rounded
         _ws.blobs[name] = p.permute(0, 4, 1, 2, 3)
-        _ws.rounded.add(name)
+        _mark_rounded(name, rnd)
         return
     dst = _input_buffer(name, src, X.DTYPE)
     bank_companion(name, dst)
-    if dst.dim() >= 2 and dst.shape[-1] >= 64:                    # feature banks are GEMM operands
+    if rnd and dst.dim() >= 2 and dst.shape[-1] >= 64:            # feature banks are GEMM operands
         X.K.round_tf32(dst.view(-1), dst.view(-1))
         _ws.rounded.add(name)
     else:
         _ws.rounded.discard(name)
     _ws.blobs[name] = dst
+
+
+def _mark_rounded(name, rounded):
+    if rounded:
+        _ws.rounded.add(name)
+    else:
+        _ws.rounded.discard(name)
 
 
 def bank_companion(name, dst):
