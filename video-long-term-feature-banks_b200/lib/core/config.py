@@ -115,8 +115,13 @@ __C = _tree({
     #   kernels which rows are real, and FetchBlob returns the r live rows.  C is a memory and compute budget the data
     #   pipeline chooses (clips per GPU x boxes per clip after the detection threshold).  0 = the RoI count is part of
     #   the captured graph's key, as before (DESIGN.md 4.6).
+    # B200.ITER_SIZE: k > 1 = training nets (with update ops) created while it is set accumulate gradients over k RunNet
+    #   calls (micro-steps, one micro-batch each) and all-reduce + apply SGD once, at the k-th; NUM_GPUS must equal k x
+    #   the number of processes, so that an iteration computes the update of NUM_GPUS GPUs of the reference on fewer
+    #   H100s.  Test, val, lfb_infer_only, precise-BN and gradient-only nets ignore it.  1 = one update per RunNet
+    #   (DESIGN.md 4.8).
     'B200': {'COMPUTE': 'tf32', 'GEMM_BACKEND': 'tcgen05', 'CUDA_GRAPH': True, 'FBO_FOLD': True, 'FBO_STACK': True,
-             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False, 'ROI_CAPACITY': 0},
+             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False, 'ROI_CAPACITY': 0, 'ITER_SIZE': 1},
 })
 config = __C
 _DEFAULTS = None

@@ -1151,6 +1151,7 @@ class CompiledNet(object):
         self.update_ops = [op for op in model.net.ops if op.type in OPTIMIZER_OPS]
         self.losses = list(getattr(model, '_losses', []) or [])
         self.train = bool(self.losses) and bool(self.update_ops or getattr(model, '_want_grads', False))
+        self._setup_iter_size(cfg)
         self._version(ops)
         self.steps = self._lower(ops)
         self.requires = {}
@@ -1194,6 +1195,22 @@ class CompiledNet(object):
         self._eager_runs = {}                        # input signature -> eager runs so far (two before capture)
         self._setup_roi_capacity(int(cfg.B200.get('ROI_CAPACITY', 0)), ops)
         self._register_inputs(ops)
+
+    # ---- B200.ITER_SIZE (DESIGN.md 4.8)
+    def _setup_iter_size(self, cfg):
+        """k = B200.ITER_SIZE micro-steps per iteration for a training net with update ops (1 for every other net).  The
+        k micro-batches of the NUM_GPUS = k x world_size 'virtual GPUs' of an iteration are spread over the processes."""
+        k = cfg.B200.get('ITER_SIZE', 1)
+        if isinstance(k, bool) or not isinstance(k, int) or k < 1:
+            raise VlfbError('%s: B200.ITER_SIZE = %r; it must be an integer >= 1' % (self.name, k))
+        self.iter_size = k if (self.train and self.update_ops) else 1
+        self.micro = 0                      # micro-steps of the current iteration run so far
+        if self.iter_size > 1:
+            from . import dist as vdist
+            world = vdist.world_size()
+            if cfg.NUM_GPUS != k * world:
+                raise VlfbError('%s: B200.ITER_SIZE = %d on %d process(es) trains NUM_GPUS = %d virtual GPUs, but '
+                                'NUM_GPUS = %d' % (self.name, k, world, k * world, cfg.NUM_GPUS))
 
     # ---- B200.COMPUTE of the fed inputs
     def _register_inputs(self, ops):
@@ -1488,7 +1505,8 @@ class CompiledNet(object):
             st.fwd(ctx)
         if not self.train:
             return
-        self.ws.params.begin_step(self.trainable)
+        if self.iter_size == 1:
+            self.ws.params.begin_step(self.trainable)
         self._prepare_wt(ctx)
         red = self._reducer()
         if red is not None:
@@ -1516,6 +1534,8 @@ class CompiledNet(object):
         ws = self.ws
         if not (self.train and ws.allreduce is not None and getattr(ws, 'overlap_allreduce', False)):
             return None
+        if self.iter_size > 1:
+            return None               # only the boundary micro-step all-reduces, eagerly between the two graphs
         from core.config import config as cfg
         if not cfg.B200.get('OVERLAP_ALLREDUCE', True):
             return None
@@ -1552,7 +1572,8 @@ class CompiledNet(object):
         """One pass.  Eager for the first runs of a given input signature; after that the whole
         step (forward + backward [+ SGD]) is replayed from a captured CUDA graph, which removes the
         per-launch host cost of the ~600 kernels of a step.  The gradient all-reduce (N > 1) stays
-        eager between the two captured halves.  Graphs are cached per input signature (e.g. per RoI count)."""
+        eager between the two captured halves.  Graphs are cached per input signature (e.g. per RoI count).
+        B200.ITER_SIZE = k > 1: the pass is one micro-step; only the k-th of an iteration all-reduces and updates."""
         from core.config import config as cfg
         ws = self.ws
         if self.roi_capacity:
@@ -1567,30 +1588,48 @@ class CompiledNet(object):
             if self._rng_base is None:
                 self._rng_base = ws.rng_offset
             ws.rng_offset = self._rng_base
+        boundary = self._micro_step()
         use_graph = (DEVICE != 'cpu' and cfg.B200.CUDA_GRAPH and not ws.force_eager and K is K_default)
         key = self._input_key() if use_graph else None
         if use_graph:
             entry = self._graphs.get(key)
             if entry is not None:
                 self._graphs.move_to_end(key)
-                return self._replay(entry)
+                return self._replay(entry, boundary)
             if self._eager_runs.get(key, 0) >= 2:
                 entry = self._capture()
                 self._graphs[key] = entry
                 while len(self._graphs) > self.MAX_GRAPHS:
                     self._graphs.popitem(last=False)
-                return self._replay(entry)
+                return self._replay(entry, boundary)
             self._eager_runs[key] = self._eager_runs.get(key, 0) + 1
             while len(self._eager_runs) > 4 * self.MAX_GRAPHS:
                 self._eager_runs.pop(next(iter(self._eager_runs)))
         ctx = Ctx(ws, self)
         self._forward_backward(ctx)
-        if not self.train:
+        if not self.train or not boundary:
             return
         if ws.allreduce is not None and self._reducer() is None:
             ws.allreduce(ws.params)
         if self.update_ops:
             self._update(ws.params)
+
+    def _micro_step(self):
+        """B200.ITER_SIZE = k > 1: before micro-step 0 of an iteration, zero the gradients (a few fills, eager, outside
+        any captured graph, whose backward then only adds into them) and hold the parameter store for this net until the
+        boundary.  Returns True when this run ends an iteration (always for k = 1)."""
+        if self.iter_size == 1:
+            return True
+        ws = self.ws
+        if self.micro == 0:
+            ws.params.begin_step(self.trainable)
+            ws.open_iteration = self
+        self.micro += 1
+        if self.micro < self.iter_size:
+            return False
+        self.micro = 0
+        ws.open_iteration = None
+        return True
 
     def _capture(self):
         """Capture the step for the current input signature.  Returns (g1, g2, n1, n2, written, rounded, split):
@@ -1609,7 +1648,7 @@ class CompiledNet(object):
                 sys.stderr.write('vlfb: capturing the overlapped all-reduce failed (%r); falling back to the split step\n' % (exc,))
                 ws.overlap_allreduce = False
                 torch.cuda.synchronize()
-        return self._capture_graphs(self.train and ws.allreduce is not None)
+        return self._capture_graphs(self.train and (ws.allreduce is not None or self.iter_size > 1))
 
     def _capture_graphs(self, split):
         ws = self.ws
@@ -1632,16 +1671,18 @@ class CompiledNet(object):
         rounded = set(k for k, r in ctx.bound.items() if r)
         return (g1, g2, n1, n2, written, rounded, split)
 
-    def _replay(self, entry):
+    def _replay(self, entry, boundary=True):
+        """Replay a captured step; a non-boundary micro-step (B200.ITER_SIZE > 1) replays the forward + backward only."""
         g1, g2, n1, n2, written, rounded, split = entry
         ws = self.ws
         g1.replay()
         K.LAUNCHES += n1
-        if split:
-            ws.allreduce(ws.params)
-        if g2 is not None:
-            g2.replay()
-            K.LAUNCHES += n2
+        if boundary:
+            if split and ws.allreduce is not None:
+                ws.allreduce(ws.params)
+            if g2 is not None:
+                g2.replay()
+                K.LAUNCHES += n2
         ws.blobs.update(written)
         ws.rounded.difference_update(written)
         ws.rounded.update(rounded)

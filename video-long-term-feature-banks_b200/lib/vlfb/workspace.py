@@ -227,6 +227,9 @@ class Workspace(object):
         # B200.COMPUTE: float input name -> (compute mode, net name) of the nets that read it (executor.CompiledNet
         # _register_inputs); inputs of 'tf32x3' nets are stored unrounded
         self.input_compute = {}
+        # B200.ITER_SIZE > 1: the training net whose iteration is under way (its gradients G hold a partial sum until the
+        # boundary micro-step), else None
+        self.open_iteration = None
 
     def begin_run(self):
         """Advance the device-side step counter (dropout masks of captured graphs depend on it)."""
@@ -340,9 +343,21 @@ def RunNet(name, num_iter=1):
     """One forward (+ backward + all-reduce + SGD for a training net) pass (tools/train_net.py:152)."""
     net = _ws.nets[str(name)]
     for _ in range(num_iter):
+        _check_open_iteration(net)
         _dequeue_blobs()
         net.run()
     return True
+
+
+def _check_open_iteration(net):
+    """B200.ITER_SIZE: between the micro-steps of an iteration, G holds the gradients summed so far.  Another training
+    net writes the same parameter store's G (and would update the parameters), so it may not run before the boundary;
+    test nets only read the parameters and may."""
+    owner = _ws.open_iteration
+    if owner is not None and owner is not net and net.train:
+        raise VlfbError('RunNet(%s): training net %s is at micro-step %d of %d of an iteration (B200.ITER_SIZE); '
+                        'finish it before running another training net' % (net.name, owner.name, owner.micro,
+                                                                           owner.iter_size))
 
 
 def EnqueueBlobs(feed):
