@@ -402,4 +402,5 @@ int vlfb_lfb_gather(const float* bank, int64_t bank_rows, const int32_t* idx, fl
 #include "vlfb_det.h"
 #include "vlfb_live.h"
 #include "vlfb_prec.h"
+#include "vlfb_seg.h"
 #endif /* VLFB_H_ */

@@ -811,6 +811,64 @@ __global__ void softmax_ce_bwd_k(const float* __restrict__ prob, const int32_t* 
   }
 }
 
+// Segmented sigmoid cross-entropy (include/vlfb_seg.h, B200.GPUS_PER_STEP): block j reduces segment j's rows exactly as
+// sigmoid_ce_fwd_k reduces all rows.  The first segment also owns rows before seg[1], the last rows up to `rows`, so
+// every row is covered whatever the offsets hold.
+__device__ __forceinline__ void seg_rows_of(const int32_t* __restrict__ seg, int S, int64_t rows, int j, int64_t* r0,
+                                            int64_t* r1) {
+  int64_t a = j == 0 ? 0 : seg[j], b = j == S - 1 ? rows : seg[j + 1];
+  a = a < 0 ? 0 : (a > rows ? rows : a);
+  b = b < a ? a : (b > rows ? rows : b);
+  *r0 = a;
+  *r1 = b;
+}
+
+__global__ void sigmoid_ce_seg_fwd_k(const float* __restrict__ x, const int32_t* __restrict__ t,
+                                     const int32_t* __restrict__ seg, int S, int64_t rows, int cols, float scale,
+                                     float* __restrict__ part) {
+  __shared__ float red[32];
+  int64_t r0, r1;
+  seg_rows_of(seg, S, rows, blockIdx.x, &r0, &r1);
+  const float* xs = x + r0 * cols;
+  const int32_t* ts = t + r0 * cols;
+  const int64_t n = (r1 - r0) * cols;
+  float s = 0.f, cnt = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const int ti = ts[i];
+    if (ti != -1) { s += sce_elem(xs[i], (float)ti); cnt += 1.f; }
+  }
+  s = block_sum(s, red);
+  cnt = block_sum(cnt, red);
+  if (threadIdx.x == 0) part[blockIdx.x] = scale * s / fmaxf(cnt, 1e-5f);
+}
+
+// the per-segment terms summed in segment order (one thread: S is the number of virtual GPUs of a step)
+__global__ void seg_sum_k(const float* __restrict__ part, int S, float* __restrict__ out) {
+  float a = part[0];
+  for (int j = 1; j < S; ++j) a += part[j];
+  out[0] = a;
+}
+
+__global__ void sigmoid_ce_seg_bwd_k(const float* __restrict__ x, const int32_t* __restrict__ t,
+                                     const int32_t* __restrict__ seg, int S, int64_t rows, int cols,
+                                     const float* __restrict__ dloss, float* __restrict__ dx, float scale) {
+  __shared__ float red[32];
+  int64_t r0, r1;
+  seg_rows_of(seg, S, rows, blockIdx.x, &r0, &r1);
+  const float* xs = x + r0 * cols;
+  const int32_t* ts = t + r0 * cols;
+  float* ds = dx + r0 * cols;
+  const int64_t n = (r1 - r0) * cols;
+  float cnt = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) cnt += (ts[i] != -1) ? 1.f : 0.f;
+  cnt = block_sum(cnt, red);
+  const float k = scale / fmaxf(cnt, 1e-5f) * (dloss ? dloss[0] : 1.f);
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const int ti = ts[i];
+    ds[i] = (ti != -1) ? k * (1.f / (1.f + __expf(-xs[i])) - (float)ti) : 0.f;
+  }
+}
+
 // ------------------------------------------------------------------ optimizer
 __global__ void sgd_k(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ pt, int64_t n,
                       const float* __restrict__ lrp, float mom, float wd, int nesterov) {
@@ -1158,6 +1216,24 @@ int vlfb_sigmoid_ce_bwd(const float* logits, const int32_t* targets, const float
                         float scale, void* stream) {
   VLFB_CHECK_ARG(logits && targets && dlogits && n > 0);
   launch_k(sigmoid_ce_bwd_k, 1, 1024, 0, ST(stream), logits, targets, dloss, dlogits, n, scale);
+  VLFB_CHECK_LAUNCH();
+  return VLFB_OK;
+}
+
+int vlfb_sigmoid_ce_seg_fwd(const float* logits, const int32_t* targets, const int32_t* seg, int S, int64_t rows,
+                            int cols, float* loss, float scale, float* scratch, void* stream) {
+  VLFB_CHECK_ARG(logits && targets && seg && loss && scratch && S > 0 && rows > 0 && cols > 0);
+  launch_k(sigmoid_ce_seg_fwd_k, S, 1024, 0, ST(stream), logits, targets, seg, S, rows, cols, scale, scratch);
+  VLFB_CHECK_LAUNCH();
+  launch_k(seg_sum_k, 1, 1, 0, ST(stream), (const float*)scratch, S, loss);
+  VLFB_CHECK_LAUNCH();
+  return VLFB_OK;
+}
+
+int vlfb_sigmoid_ce_seg_bwd(const float* logits, const int32_t* targets, const int32_t* seg, int S, int64_t rows,
+                            int cols, const float* dloss, float* dlogits, float scale, void* stream) {
+  VLFB_CHECK_ARG(logits && targets && seg && dlogits && S > 0 && rows > 0 && cols > 0);
+  launch_k(sigmoid_ce_seg_bwd_k, S, 1024, 0, ST(stream), logits, targets, seg, S, rows, cols, dloss, dlogits, scale);
   VLFB_CHECK_LAUNCH();
   return VLFB_OK;
 }

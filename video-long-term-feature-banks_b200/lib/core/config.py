@@ -120,8 +120,15 @@ __C = _tree({
     #   the number of processes, so that an iteration computes the update of NUM_GPUS GPUs of the reference on fewer
     #   H100s.  Test, val, lfb_infer_only, precise-BN and gradient-only nets ignore it.  1 = one update per RunNet
     #   (DESIGN.md 4.8).
+    # B200.GPUS_PER_STEP: v > 1 = training nets (with update ops) created while it is set run v of the recipe's virtual
+    #   GPUs in one RunNet, as one packed batch of v x (TRAIN.BATCH_SIZE / NUM_GPUS) clips: clips [j b, (j+1) b) and the
+    #   RoIs with batch index in that range are virtual GPU j's.  The sigmoid loss is normalised per virtual GPU and
+    #   SpatialBN takes batch statistics per virtual GPU; NUM_GPUS must equal v x ITER_SIZE x the number of processes.
+    #   Test, val, lfb_infer_only, precise-BN and gradient-only nets ignore it.  1 = one virtual GPU per step
+    #   (DESIGN.md 4.9).
     'B200': {'COMPUTE': 'tf32', 'GEMM_BACKEND': 'tcgen05', 'CUDA_GRAPH': True, 'FBO_FOLD': True, 'FBO_STACK': True,
-             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False, 'ROI_CAPACITY': 0, 'ITER_SIZE': 1},
+             'LFB_DTYPE': 'f32', 'DETERMINISTIC': False, 'ROI_CAPACITY': 0, 'ITER_SIZE': 1,
+             'GPUS_PER_STEP': 1},
 })
 config = __C
 _DEFAULTS = None

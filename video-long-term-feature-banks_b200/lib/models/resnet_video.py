@@ -60,7 +60,12 @@ def create_model(model, data, labels, split, lfb_infer_only, suffix=''):
     blocks = BLOCK_CONFIG[cfg.MODEL.DEPTH]
     group, width = cfg.RESNETS.NUM_GROUPS, cfg.RESNETS.WIDTH_PER_GROUP
     dim_inner = group * width
-    batch_size = get_batch_size(split)
+    # a net that gets update ops packs B200.GPUS_PER_STEP virtual GPUs per step; precise-BN and other forward-only
+    # training-split nets keep one GPU's clips
+    packed = (split == 'train' and not lfb_infer_only and getattr(model, 'train', False)
+              and not getattr(model, 'force_fw_only', False))
+    batch_size = get_batch_size(split, packed)
+    model.recorded_batch_size = batch_size           # CreateNet checks it against B200.GPUS_PER_STEP
     test_mode = split in ('test', 'val')
     crop_size = cfg.TRAIN.CROP_SIZE if (split == 'train' and not lfb_infer_only) else cfg.TEST.CROP_SIZE
     logger.info('ResNet-%d %dx%dd %s, dataset %s, split %s, infer LFB %s, suffix "%s"',

@@ -479,12 +479,25 @@ class SpatialBNStep(Step):
             K.spatial_bn_infer(xp, st.phys(self.s), st.phys(self.b), st.phys(self.rm), st.phys(self.riv), phys(y), self.eps)
         else:
             c = xp.shape[-1]
-            sm, siv = empty((c,)), empty((c,))
-            bn_fwd = K.spatial_bn_fwd_det if ctx.net.det else K.spatial_bn_fwd
-            bn_fwd(xp, st.phys(self.s), st.phys(self.b), st.phys(self.rm), st.phys(self.riv), sm, siv, phys(y),
-                   self.eps, self.momentum)
-            ctx.put(self.op.outputs[3], sm)
-            ctx.put(self.op.outputs[4], siv)
+            v = ctx.net.gpus_per_step
+            if v > 1:
+                # B200.GPUS_PER_STEP: statistics per virtual GPU (its contiguous rows); the running statistics and the
+                # '_sm' / '_siv' blobs are virtual GPU 0's, the other segments' statistics stay in this scratch
+                if (xp.numel() // c) % v:
+                    raise VlfbError('%s: %d rows do not split into B200.GPUS_PER_STEP = %d virtual GPUs'
+                                    % (self.op.outputs[0], xp.numel() // c, v))
+                sm, siv = empty((v, c)), empty((v, c))
+                K.spatial_bn_seg_fwd(xp, st.phys(self.s), st.phys(self.b), st.phys(self.rm), st.phys(self.riv), sm, siv,
+                                     phys(y), self.eps, self.momentum, v, det=ctx.net.det)
+                ctx.put(self.op.outputs[3], sm[0])
+                ctx.put(self.op.outputs[4], siv[0])
+            else:
+                sm, siv = empty((c,)), empty((c,))
+                bn_fwd = K.spatial_bn_fwd_det if ctx.net.det else K.spatial_bn_fwd
+                bn_fwd(xp, st.phys(self.s), st.phys(self.b), st.phys(self.rm), st.phys(self.riv), sm, siv, phys(y),
+                       self.eps, self.momentum)
+                ctx.put(self.op.outputs[3], sm)
+                ctx.put(self.op.outputs[4], siv)
             ctx.saved[id(self)] = (xp, sm, siv)
         ctx.put(self.op.outputs[0], y)
 
@@ -499,10 +512,13 @@ class SpatialBNStep(Step):
         st = ctx.ws.params
         need_dx = ctx.net.requires.get(self.in_keys[0], False)
         dx = empty_like_strided(gy)
-        bn_bwd = K.spatial_bn_bwd_det if ctx.net.det else K.spatial_bn_bwd
-        bn_bwd(gp, xp, st.phys(self.s), sm, siv, phys(dx),
-               st.grad(self.s) if st.trainable(self.s) else None,
-               st.grad(self.b) if st.trainable(self.b) else None)
+        ds = st.grad(self.s) if st.trainable(self.s) else None
+        db = st.grad(self.b) if st.trainable(self.b) else None
+        if sm.dim() == 2:                                   # B200.GPUS_PER_STEP: each segment's own statistics
+            K.spatial_bn_seg_bwd(gp, xp, st.phys(self.s), sm, siv, phys(dx), ds, db, sm.shape[0], det=ctx.net.det)
+        else:
+            bn_bwd = K.spatial_bn_bwd_det if ctx.net.det else K.spatial_bn_bwd
+            bn_bwd(gp, xp, st.phys(self.s), sm, siv, phys(dx), ds, db)
         if need_dx:
             ctx.add_grad(self.in_keys[0], dx, owned=True)
 
@@ -1079,25 +1095,39 @@ class SigmoidStep(Step):
 
 
 class SigmoidCELossStep(Step):
+    """B200.GPUS_PER_STEP = v > 1: the loss is the sum of the v virtual GPUs' losses, each normalised by its own count of
+    targets != -1, over the row segments CompiledNet.loss_segments gives (RoI rows of an AVA net, clips otherwise)."""
+
     def fwd(self, ctx):
         x, t = ctx.get(self.op.inputs[0]), ctx.get(self.op.inputs[1])
         loss = empty((1,))
-        K.sigmoid_ce_fwd(x, t, loss, self.op.args['scale'])
+        seg = ctx.net.loss_segments()
+        if seg is None:
+            K.sigmoid_ce_fwd(x, t, loss, self.op.args['scale'])
+        else:
+            K.sigmoid_ce_seg_fwd(x, t, seg, loss, self.op.args['scale'])
         ctx.put(self.op.outputs[0], loss)
 
     def bwd(self, ctx):
         gl = ctx.pop_grad(self.out_keys[0])
         x, t = ctx.get(self.op.inputs[0]), ctx.get(self.op.inputs[1])
         dx = empty(x.shape)
-        K.sigmoid_ce_bwd(x, t, gl, dx, self.op.args['scale'])
+        seg = ctx.net.loss_segments()
+        if seg is None:
+            K.sigmoid_ce_bwd(x, t, gl, dx, self.op.args['scale'])
+        else:
+            K.sigmoid_ce_seg_bwd(x, t, seg, gl, dx, self.op.args['scale'])
         ctx.add_grad(self.in_keys[0], dx, owned=True)
 
 
 class SoftmaxCELossStep(Step):
+    """B200.GPUS_PER_STEP = v: every virtual GPU has the same number of rows, so the sum of their mean losses is the
+    mean over all rows times v -- the existing kernels with scale v x scale."""
+
     def fwd(self, ctx):
         x, t = ctx.get(self.op.inputs[0]), ctx.get(self.op.inputs[1])
         prob, loss = empty(x.shape), empty((1,))
-        K.softmax_ce_fwd(x, t.view(-1), prob, loss, self.op.args['scale'])
+        K.softmax_ce_fwd(x, t.view(-1), prob, loss, self.op.args['scale'] * ctx.net.gpus_per_step)
         ctx.put(self.op.outputs[0], prob)
         ctx.put(self.op.outputs[1], loss)
 
@@ -1106,7 +1136,7 @@ class SoftmaxCELossStep(Step):
         ctx.pop_grad(self.out_keys[1])
         prob, t = ctx.get(self.op.outputs[0]), ctx.get(self.op.inputs[1])
         dx = empty(prob.shape)
-        K.softmax_ce_bwd(prob, t.view(-1), dx, self.op.args['scale'])
+        K.softmax_ce_bwd(prob, t.view(-1), dx, self.op.args['scale'] * ctx.net.gpus_per_step)
         ctx.add_grad(self.in_keys[0], dx, owned=True)
 
 
@@ -1153,6 +1183,7 @@ class CompiledNet(object):
         self.train = bool(self.losses) and bool(self.update_ops or getattr(model, '_want_grads', False))
         self._setup_iter_size(cfg)
         self._version(ops)
+        self._setup_gpus_per_step(cfg, ops)
         self.steps = self._lower(ops)
         self.requires = {}
         self.trainable = []
@@ -1203,14 +1234,60 @@ class CompiledNet(object):
         k = cfg.B200.get('ITER_SIZE', 1)
         if isinstance(k, bool) or not isinstance(k, int) or k < 1:
             raise VlfbError('%s: B200.ITER_SIZE = %r; it must be an integer >= 1' % (self.name, k))
+        v = cfg.B200.get('GPUS_PER_STEP', 1)
+        if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+            raise VlfbError('%s: B200.GPUS_PER_STEP = %r; it must be an integer >= 1' % (self.name, v))
         self.iter_size = k if (self.train and self.update_ops) else 1
+        self.gpus_per_step = v if (self.train and self.update_ops) else 1
         self.micro = 0                      # micro-steps of the current iteration run so far
-        if self.iter_size > 1:
+        if self.iter_size > 1 or self.gpus_per_step > 1:
             from . import dist as vdist
             world = vdist.world_size()
-            if cfg.NUM_GPUS != k * world:
-                raise VlfbError('%s: B200.ITER_SIZE = %d on %d process(es) trains NUM_GPUS = %d virtual GPUs, but '
-                                'NUM_GPUS = %d' % (self.name, k, world, k * world, cfg.NUM_GPUS))
+            v = self.gpus_per_step
+            if cfg.NUM_GPUS != v * k * world:
+                if v == 1:
+                    raise VlfbError('%s: B200.ITER_SIZE = %d on %d process(es) trains NUM_GPUS = %d virtual GPUs, but '
+                                    'NUM_GPUS = %d' % (self.name, k, world, k * world, cfg.NUM_GPUS))
+                raise VlfbError('%s: B200.GPUS_PER_STEP = %d x B200.ITER_SIZE = %d on %d process(es) trains NUM_GPUS = %d '
+                                'virtual GPUs, but NUM_GPUS = %d' % (self.name, v, k, world, v * k * world, cfg.NUM_GPUS))
+
+    # ---- B200.GPUS_PER_STEP (DESIGN.md 4.9)
+    def _setup_gpus_per_step(self, cfg, ops):
+        """v = self.gpus_per_step virtual GPUs of b = TRAIN.BATCH_SIZE / NUM_GPUS clips each in one packed batch.  The
+        net's recorded batch must be v x b.  The sigmoid loss of an AVA net (RoIAlign on 'proposals{sfx}') is segmented by
+        the RoI row offsets the workspace derives from every 'proposals' feed; any other sigmoid loss by the fixed clip
+        offsets j x b."""
+        v = self.gpus_per_step
+        self.seg_rois, self._clip_seg = None, None
+        if v == 1:
+            return
+        b = int(cfg.TRAIN.BATCH_SIZE / cfg.NUM_GPUS)
+        rec = getattr(self.model, 'recorded_batch_size', None)
+        if rec is not None and rec != v * b:
+            raise VlfbError('%s: recorded with a batch of %d clips; B200.GPUS_PER_STEP = %d needs %d x %d = %d (build the '
+                            'net while the setting is in force)' % (self.name, rec, v, v, b, v * b))
+        rois = [op.inputs[1] for op in ops if op.type == 'RoIAlign' and op.inputs[1].startswith('proposals')]
+        if rois:
+            self.seg_rois = rois[0]
+            if self.ws is not None:
+                self.ws.gpus_per_step[self.seg_rois] = (v, b)
+        else:
+            self._clip_seg = torch.arange(0, v * b + 1, b, dtype=torch.int32).to(DEVICE)
+
+    def loss_segments(self):
+        """The device int32 [v + 1] row offsets of the virtual GPUs' loss rows, or None for a one-GPU step."""
+        if self.gpus_per_step == 1:
+            return None
+        if self.seg_rois is None:
+            return self._clip_seg
+        return self.ws.roi_segments[self.seg_rois]
+
+    def _check_segments(self):
+        """The RoIs of this step were fed through the workspace's checks for this net's v and b."""
+        ent = self.ws.seg_fed.get(self.seg_rois)
+        if ent != self.ws.gpus_per_step.get(self.seg_rois):
+            raise VlfbError('%s: not fed as a packed batch of B200.GPUS_PER_STEP = %d virtual GPUs (fed before net %s '
+                            'was created?); feed it again' % (self.seg_rois, self.gpus_per_step, self.name))
 
     # ---- B200.COMPUTE of the fed inputs
     def _register_inputs(self, ops):
@@ -1581,6 +1658,8 @@ class CompiledNet(object):
             ws.roi_blobs.update(self._roi_marks)        # names shared with another net (train / test) are this net's now
         if self.x3:
             self._check_unrounded_inputs()
+        if self.seg_rois is not None:
+            self._check_segments()
         ws.begin_run()
         if self.det:
             # every run draws the dropout offsets its first run drew, as a graph replay does (the step counter varies

@@ -550,6 +550,32 @@ def spatial_bn_bwd_det(dy, x, s, sm, siv, dx, ds, db):
                                             _ptr(ws), nb, _stream()), 'spatial_bn_bwd_det')
 
 
+def _bn_seg_workspace(C_, S):
+    nbytes = int(L.load().vlfb_spatial_bn_seg_workspace_bytes(int(C_), int(S)))
+    return torch.empty((nbytes + 15) // 16 * 16, dtype=torch.uint8, device='cuda'), nbytes
+
+
+def spatial_bn_seg_fwd(x, s, b, rm, rv, sm, siv, y, eps, momentum, segments, det=False):
+    """spatial_bn_fwd with batch statistics per segment of rows // segments contiguous rows (B200.GPUS_PER_STEP):
+    sm / siv are [segments, C]; rm / rv are updated from segment 0's statistics.  det: the reproducible form."""
+    c = x.shape[-1]
+    ws, nb = _bn_seg_workspace(c, segments)
+    fn = L.load().vlfb_spatial_bn_seg_fwd_det if det else L.load().vlfb_spatial_bn_seg_fwd
+    _check(fn(_ptr(_f32c(x)), _ptr(s), _ptr(b), _ptr(rm), _ptr(rv), _ptr(_f32c(sm)), _ptr(_f32c(siv)), _ptr(_f32c(y)),
+              x.numel() // c, c, int(segments), float(eps), float(momentum), _ptr(ws), nb, _stream()),
+           'spatial_bn_seg_fwd' + ('_det' if det else ''))
+
+
+def spatial_bn_seg_bwd(dy, x, s, sm, siv, dx, ds, db, segments, det=False):
+    """spatial_bn_bwd with each segment's own statistics (sm / siv [segments, C]); ds / db summed over segments."""
+    c = x.shape[-1]
+    ws, nb = _bn_seg_workspace(c, segments)
+    fn = L.load().vlfb_spatial_bn_seg_bwd_det if det else L.load().vlfb_spatial_bn_seg_bwd
+    _check(fn(_ptr(_f32c(dy)), _ptr(_f32c(x)), _ptr(s), _ptr(_f32c(sm)), _ptr(_f32c(siv)), _ptr(_f32c(dx)), _ptr(ds),
+              _ptr(db), x.numel() // c, c, int(segments), _ptr(ws), nb, _stream()),
+           'spatial_bn_seg_bwd' + ('_det' if det else ''))
+
+
 def maxpool_fwd(x, y, argmax, g):
     _check(L.load().vlfb_maxpool3d_fwd(_ptr(_f32c(x)), _ptr(_f32c(y)), _ptr(argmax), C.byref(g), _stream()),
             'maxpool_fwd')
@@ -748,6 +774,28 @@ def sigmoid_ce_fwd(logits, targets, loss, scale):
 def sigmoid_ce_bwd(logits, targets, dloss, dlogits, scale):
     _check(L.load().vlfb_sigmoid_ce_bwd(_ptr(_f32c(logits)), _ptr(targets), _ptr(dloss), _ptr(_f32c(dlogits)),
                                          logits.numel(), float(scale), _stream()), 'sigmoid_ce_bwd')
+
+
+def _seg(seg):
+    assert seg.dtype == torch.int32 and seg.dim() == 1 and seg.is_cuda and seg.numel() >= 2
+    return seg.numel() - 1
+
+
+def sigmoid_ce_seg_fwd(logits, targets, seg, loss, scale):
+    """loss[0] = sum_j scale * CE_j / count_j over the row segments seg (device int32 [S+1] row offsets, read in stream
+    order; B200.GPUS_PER_STEP), summed in segment order."""
+    assert targets.dtype == torch.int32
+    S = _seg(seg)
+    part = torch.empty(S, dtype=torch.float32, device='cuda')
+    _check(L.load().vlfb_sigmoid_ce_seg_fwd(_ptr(_f32c(logits)), _ptr(targets), _ptr(seg), S, logits.shape[0],
+                                             logits.numel() // logits.shape[0], _ptr(loss), float(scale), _ptr(part),
+                                             _stream()), 'sigmoid_ce_seg_fwd')
+
+
+def sigmoid_ce_seg_bwd(logits, targets, seg, dloss, dlogits, scale):
+    _check(L.load().vlfb_sigmoid_ce_seg_bwd(_ptr(_f32c(logits)), _ptr(targets), _ptr(seg), _seg(seg), logits.shape[0],
+                                             logits.numel() // logits.shape[0], _ptr(dloss), _ptr(_f32c(dlogits)),
+                                             float(scale), _stream()), 'sigmoid_ce_seg_bwd')
 
 
 def softmax_ce_fwd(logits, labels, prob, loss, scale):

@@ -143,10 +143,21 @@ LIVE_SIGNATURES = {
 PREC_SIGNATURES = {
     'vlfb_weight_scale_transpose_multi': [_P, _I, _I, _P],
 }
+# include/vlfb_seg.h (included by vlfb.h): per-segment losses and SpatialBN statistics (B200.GPUS_PER_STEP)
+SEG_SIGNATURES = {
+    'vlfb_sigmoid_ce_seg_fwd': [_P, _P, _P, _I, _L, _I, _P, _F, _P, _P],
+    'vlfb_sigmoid_ce_seg_bwd': [_P, _P, _P, _I, _L, _I, _P, _P, _F, _P],
+    'vlfb_spatial_bn_seg_workspace_bytes': [_I, _I],
+    'vlfb_spatial_bn_seg_fwd': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _F, _F, _P, C.c_size_t, _P],
+    'vlfb_spatial_bn_seg_bwd': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _P, C.c_size_t, _P],
+    'vlfb_spatial_bn_seg_fwd_det': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _F, _F, _P, C.c_size_t, _P],
+    'vlfb_spatial_bn_seg_bwd_det': [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _P, C.c_size_t, _P],
+}
 RESTYPES = {'vlfb_last_error': C.c_char_p, 'vlfb_roi_align_bwd_det_scratch_bytes': C.c_size_t, 'vlfb_fbo_bank_scan_workspace': C.c_size_t,
             'vlfb_fbo_bank_scan_workspace_dt': C.c_size_t,
             'vlfb_fbo_nl_scratch_floats': C.c_size_t,
-            'vlfb_gemm_workspace_bytes': C.c_size_t, 'vlfb_spatial_bn_workspace_bytes': C.c_size_t}
+            'vlfb_gemm_workspace_bytes': C.c_size_t, 'vlfb_spatial_bn_workspace_bytes': C.c_size_t,
+            'vlfb_spatial_bn_seg_workspace_bytes': C.c_size_t}
 
 _lib = None
 
@@ -162,7 +173,7 @@ def load():
             'g.build()" or make -C csrc).  There is no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, argtypes in list(SIGNATURES.items()) + list(DET_SIGNATURES.items()) + list(LIVE_SIGNATURES.items()) + \
-            list(PREC_SIGNATURES.items()):
+            list(PREC_SIGNATURES.items()) + list(SEG_SIGNATURES.items()):
         fn = getattr(lib, name)        # AttributeError if the symbol is missing
         fn.argtypes = argtypes
         fn.restype = RESTYPES.get(name, C.c_int)

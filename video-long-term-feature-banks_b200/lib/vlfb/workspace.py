@@ -230,6 +230,12 @@ class Workspace(object):
         # B200.ITER_SIZE > 1: the training net whose iteration is under way (its gradients G hold a partial sum until the
         # boundary micro-step), else None
         self.open_iteration = None
+        # B200.GPUS_PER_STEP (DESIGN.md 4.9): 'proposals{sfx}' name -> (v, b) of the packed training net that reads it;
+        # name -> device int32 [v + 1] RoI row offsets of the virtual GPUs (fixed address, written in stream order by
+        # every feed); name -> the (v, b) its last feed was checked for
+        self.gpus_per_step = {}
+        self.roi_segments = {}
+        self.seg_fed = {}
 
     def begin_run(self):
         """Advance the device-side step counter (dropout masks of captured graphs depend on it)."""
@@ -372,6 +378,8 @@ def EnqueueBlobs(feed):
             FeedBlob(name, arr)
         return True
     assert ws.queued is None, 'EnqueueBlobs: the previous batch has not been consumed by RunNet yet'
+    segs = dict((_unscoped(n), _segment_offsets(_unscoped(n), a)) for n, a in feed.items())    # checked on the host
+    segs = dict((n, o) for n, o in segs.items() if o is not None)
     if ws.copy_stream is None:
         ws.copy_stream = torch.cuda.Stream()
     slot = ws.queue_slot
@@ -396,7 +404,7 @@ def EnqueueBlobs(feed):
             staged[_unscoped(name)] = st
         ev = torch.cuda.Event()
         ev.record(ws.copy_stream)
-    ws.queued = (slot, staged, ev)
+    ws.queued = (slot, staged, ev, segs)
     del main
     return True
 
@@ -405,11 +413,13 @@ def _dequeue_blobs():
     ws = _ws
     if ws.queued is None:
         return
-    slot, staged, ev = ws.queued
+    slot, staged, ev, segs = ws.queued
     ws.queued = None
     torch.cuda.current_stream().wait_event(ev)
     for name, st in staged.items():
         _feed_activation(name, st)
+    for name, offs in segs.items():
+        _set_segments(name, offs)
     done = torch.cuda.Event()
     done.record(torch.cuda.current_stream())
     ws.slot_free[slot] = done
@@ -436,6 +446,38 @@ def _roi_rows(name, shape):
     if not 1 <= r <= cap:
         raise VlfbError('%s: %d RoI rows fed; B200.ROI_CAPACITY = %d holds 1 to %d' % (name, r, cap, cap))
     return cap
+
+
+def _segment_offsets(name, arr):
+    """B200.GPUS_PER_STEP: for a 'proposals' input of a packed training net, check the fed RoIs against the packed
+    batch's rules -- batch indices (column 0) in [0, v b) and not decreasing -- and return the v + 1 row offsets of the
+    virtual GPUs' RoIs (virtual GPU j = batch index // b).  None for any other input."""
+    ent = _ws.gpus_per_step.get(name)
+    if ent is None:
+        return None
+    v, b = ent
+    a = arr.detach().cpu().numpy() if isinstance(arr, torch.Tensor) else np.asarray(arr)
+    if a.ndim != 2 or a.shape[1] < 1:
+        raise VlfbError('%s: RoIs of shape %s; B200.GPUS_PER_STEP expects [R, 5] rows (batch index first)'
+                        % (name, tuple(a.shape)))
+    idx = a[:, 0]
+    if idx.size and (not np.all(idx == np.floor(idx)) or idx.min() < 0 or idx.max() >= v * b):
+        raise VlfbError('%s: batch indices must be integers in [0, %d) for B200.GPUS_PER_STEP = %d virtual GPUs of %d '
+                        'clips' % (name, v * b, v, b))
+    if idx.size > 1 and np.any(np.diff(idx) < 0):
+        raise VlfbError('%s: batch indices decrease; a packed batch lists virtual GPU j\'s RoIs (batch index in [j b, '
+                        '(j+1) b)) before those of virtual GPU j + 1' % name)
+    return np.searchsorted(idx.astype(np.int64), np.arange(v + 1) * b, side='left').astype(np.int32)
+
+
+def _set_segments(name, offs):
+    """Write the row offsets of the virtual GPUs' RoIs into the input's fixed device buffer, in stream order (a captured
+    graph reads each replay's offsets), and record which (v, b) the feed was checked for."""
+    buf = _ws.roi_segments.get(name)
+    if buf is None or buf.numel() != len(offs):
+        buf = _ws.roi_segments[name] = torch.zeros(len(offs), dtype=torch.int32, device=X.DEVICE)
+    buf.copy_(torch.from_numpy(offs))
+    _ws.seg_fed[name] = _ws.gpus_per_step[name]
 
 
 def set_live_rows(name, rows):
@@ -551,6 +593,7 @@ def FeedBlob(name, arr, device_option=None):
         _ws.params._ensure_state()
         _ws.params.logical(base, 'Mo').copy_(torch.as_tensor(np.asarray(arr)).to(X.DTYPE).to(X.DEVICE))
         return True
+    offs = _segment_offsets(name, arr)                 # checked before anything is written
     if np.ndim(arr) == 0 or name in ('lr', 'weight_decay', 'weight_decay_bn', 'ONE'):
         v = torch.as_tensor(np.asarray(arr).reshape(-1)).to(X.DTYPE)
         cur = _ws.blobs.get(name)
@@ -560,6 +603,8 @@ def FeedBlob(name, arr, device_option=None):
             _ws.blobs[name] = v.to(X.DEVICE)
         return True
     _feed_activation(name, arr)
+    if offs is not None:
+        _set_segments(name, offs)                      # only once the feed itself has landed
     return True
 
 
